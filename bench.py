@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — images/sec of one compression-aware training step (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over one batch of synthetic input: teacher forward (eval mode),
@@ -18,6 +18,11 @@ gradient all-reduce (N > 1), fused optimizer.  Nothing is skipped inside the tim
   cpu_baseline  : the oracle step (oracle/step_oracle.py: un-fused PyTorch-CPU fp32, all host cores)
                   on a bounded sample of the same workload (TF 1.x cannot run in this image).
 `--impl reference` times that CPU path alone (rank 0 only) and prints the same line.
+`--dump-outputs DIR` writes what the last timed step computed (losses, logits, a fixed sample of the updated
+parameters) as DIR/<name>.npy, so that two builds can be compared output for output on identical seeded inputs.
+
+The ResNet-50 workloads run at batch 128 per GPU: a ResNet-50 step at batch 128 keeps 41 GiB resident on an
+H100 80GB, batch 256 does not fit.
 """
 import argparse
 import json
@@ -36,26 +41,26 @@ METRIC = 'images_per_sec_compression_aware_training_step'
 
 WORKLOADS = {
     # name: (net module, resnet_size, learner, flag overrides, description)
-    'resnet50_uq8_dst_b256': ('resnet_at_ilsvrc12', 50, 'uniform', dict(batch_size=256, enbl_dst=True,
+    'resnet50_uq8_dst_b128': ('resnet_at_ilsvrc12', 50, 'uniform', dict(batch_size=128, enbl_dst=True,
                               uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel'),
                               'ResNet-50 v2 / synthetic 224x224x3, UniformQuantLearner W8(per-channel)A8 + distillation'),
     'resnet20_uq8_dst_b256': ('resnet_at_cifar10', 20, 'uniform', dict(batch_size=256, enbl_dst=True,
                               uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel'),
                               'ResNet-20 v2 / synthetic CIFAR-10 32x32x3, UniformQuantLearner W8(per-channel)A8 + distillation'),
-    'resnet50_ws50_dst_b256': ('resnet_at_ilsvrc12', 50, 'weight-sparse', dict(batch_size=256, enbl_dst=True,
+    'resnet50_ws50_dst_b128': ('resnet_at_ilsvrc12', 50, 'weight-sparse', dict(batch_size=128, enbl_dst=True,
                                ws_prune_ratio=0.5, ws_prune_ratio_prtl='uniform'),
                                'ResNet-50 v2 / synthetic 224x224x3, WeightSparseLearner 50% + distillation'),
     'resnet20_ws50_dst_b256': ('resnet_at_cifar10', 20, 'weight-sparse', dict(batch_size=256, enbl_dst=True,
                                ws_prune_ratio=0.5, ws_prune_ratio_prtl='uniform'),
                                'ResNet-20 v2 / synthetic CIFAR-10, WeightSparseLearner 50% + distillation'),
-    'resnet50_nuq4_dst_b256': ('resnet_at_ilsvrc12', 50, 'non-uniform', dict(batch_size=256, enbl_dst=True,
+    'resnet50_nuq4_dst_b128': ('resnet_at_ilsvrc12', 50, 'non-uniform', dict(batch_size=128, enbl_dst=True,
                                nuql_weight_bits=4), 'ResNet-50 v2 / synthetic 224x224x3, NonUniformQuantLearner 4-bit codebook + distillation'),
     'mobilenet_cpg50_b256': ('mobilenet_at_ilsvrc12', 0, 'chn-pruned-gpu', dict(batch_size=256, cpg_prune_ratio=0.5),
                              'MobileNet-v1 / synthetic 224x224x3, ChannelPrunedGpuLearner masked step at 0.5 channel ratio'),
     'lenet_uq8_b128': ('lenet_at_cifar10', 0, 'uniform', dict(batch_size=128, uql_weight_bits=8),
                        'LeNet-5 / synthetic CIFAR-10, UniformQuantLearner 8-bit (configs[0], plumbing)'),
 }
-DEFAULT_WORKLOAD = os.environ.get('PF_BENCH_WORKLOAD', 'resnet50_uq8_dst_b256')    # the driver passes no --workload
+DEFAULT_WORKLOAD = os.environ.get('PF_BENCH_WORKLOAD', 'resnet50_uq8_dst_b128')
 
 
 def setup_flags(workload, batch_override=None, world=1):
@@ -107,7 +112,7 @@ def conv_flops_per_image(ex):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -143,7 +148,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d['hbm_gbs'], d['bf16_tflops'], d.get('bf16_tflops_sustained', d['bf16_tflops']), 'measured'
-    return 6650.0, 1590.0, 1400.0, 'fallback'
+    return 3350.0, 989.0, 989.0, 'H100 SXM datasheet'
 
 
 def build_learner(workload, world, batch_override=None):
@@ -325,6 +330,26 @@ def quiet_stdout():
         os.dup2(2, 1)
 
 
+def dump_outputs(ex, out_dir, limit_bytes=64 << 20):
+    """The arrays a caller of the timed step receives from its last run, as float32 .npy files: the losses, the
+    logits of the batch, and the updated flat parameter buffer (a fixed, seeded sample of it when the whole buffer
+    would exceed `limit_bytes` in all)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {'loss_' + k: np.asarray([v], np.float32) for k, v in ex.fetch_losses().items()}
+    arrays['logits'] = ex.T(ex.logits_t).float().cpu().numpy()
+    params = ex.store.P.float().cpu().numpy()
+    room = (limit_bytes - sum(a.nbytes for a in arrays.values()) - 4096 * (len(arrays) + 1)) // 4   # + .npy headers
+    if params.size > room:
+        idx = np.sort(np.random.default_rng(0).choice(params.size, size=room, replace=False))
+        arrays['params_sample'] = params[idx]
+    else:
+        arrays['params'] = params
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 def emit(line):
     data = (json.dumps(line) + '\n').encode()
     if _RESULT_FD is None:
@@ -346,6 +371,8 @@ def main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--workload', default=DEFAULT_WORKLOAD, choices=sorted(WORKLOADS))
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step as DIR/<name>.npy')
     ap.add_argument('--batch', type=int, default=None, help='override the per-GPU batch (smoke runs only)')
     ap.add_argument('--cpu-batch', type=int, default=None)
     ap.add_argument('--no-cpu-baseline', action='store_true')
@@ -415,6 +442,8 @@ def main():
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_total = float(ms.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ex, args.dump_outputs)
     # ---- timed region 2: end to end through the public API (H2D of every batch, D2H of the losses)
     for _ in range(2):
         lrn.train_step()
@@ -461,14 +490,14 @@ def main():
     aq_ms = prof.get('bn_apply', 0.0)
     conv_traffic, traffic_src = None, 'no ncu launch list of this binary under profiles/ (run tools/gpu_launchlist.sh)'
     try:
-        tj = json.load(open(os.path.join(ROOT, 'profiles', 'r2_ncu_conv_traffic.json')))
+        tj = json.load(open(os.path.join(ROOT, 'profiles', 'conv_traffic.json')))
         if tj.get('workload') != args.workload or B != tj.get('batch'):
-            traffic_src = 'profiles/r2_ncu_conv_traffic.json is for another workload / batch'
+            traffic_src = 'profiles/conv_traffic.json is for another workload / batch'
         elif tj.get('kernel_source_stamp') != kernel_source_stamp():
-            traffic_src = 'profiles/r2_ncu_conv_traffic.json is stale (kernel sources changed since it was measured)'
+            traffic_src = 'profiles/conv_traffic.json is stale (kernel sources changed since it was measured)'
         else:
             conv_traffic = tj['conv_dram_bytes_per_step']
-            traffic_src = 'ncu launch list of this binary (kernel source stamp %s), profiles/r2_ncu_conv_traffic.json' % tj['kernel_source_stamp']
+            traffic_src = 'ncu launch list of this binary (kernel source stamp %s), profiles/conv_traffic.json' % tj['kernel_source_stamp']
     except Exception:  # noqa: BLE001
         pass
     # MMA multiplicity per pass (tensor-core work issued per algorithmic product)
@@ -484,7 +513,7 @@ def main():
             'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': {'workload': args.workload, 'description': WORKLOADS[args.workload][4],
                        'batch_per_gpu': B, 'global_batch': B * world, 'parallelism': 'dp%d' % world,
-                       'conv_path': ('tcgen05 + TMEM, persistent warp-specialised kernels, operands fed by TMA (im2col-mode '
+                       'conv_path': ('wgmma, persistent warp-specialised kernels, operands fed by TMA (im2col-mode '
                                      'tensor maps for the NHWC operand, tiled maps for weights / dy) where channel counts are '
                                      'multiples of 64, cp.async elsewhere: %d of %d conv/dense layers (+ the stem through '
                                      'space-to-depth planes); exact-fp32 CUDA-core kernels for the rest.  MMAs per k-slice: '
@@ -493,7 +522,7 @@ def main():
                                      '(split-bf16 x split-bf16 = fp32-equivalent product)'
                                      % (n_tc, sum(1 for o in ex.ops if o.type in ('Conv2D', 'MatMul')), n_lv_w, n_lv_a))
                        if ex.tc or ex.im2col else 'fp32 CUDA-core implicit GEMM (pf_conv.cu)',
-                       'l2': 'per-step working set (GBs of activations) >> 126 MB L2; no explicit flush',
+                       'l2': 'per-step working set (GBs of activations) >> 50 MB L2; no explicit flush',
                        'cuda_graph': graph_ok,
                        'input_pipeline': 'e2e: batch i+1 is copied host->device (pinned memory, copy stream) while step i '
                                          'runs, then moved into the graph input buffers device-to-device; one H2D per step'},

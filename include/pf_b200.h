@@ -1,4 +1,4 @@
-/* pf_b200.h — C ABI of libpf_b200.so: the B200 (sm_100a) kernels behind PocketFlow's
+/* pf_b200.h — C ABI of libpf_b200.so: the H100 (sm_90a) kernels behind PocketFlow's
  * compression-aware training step.
  *
  * The reference (Tencent/PocketFlow) has no FFI: its de-facto operator boundary is the set of
@@ -41,7 +41,7 @@ const char* pf_last_error(void);
 /* Number of kernel launches this library has enqueued in this process (bench.py "gpu_launches"). */
 int64_t pf_launch_count(void);
 void pf_launch_count_reset(void);
-/* Device query helper: SM count of the current device (148 on B200). */
+/* Device query helper: SM count of the current device (132 on H100 SXM). */
 int pf_sm_count(int* out);
 
 /* ---------------------------------------------------------------------------------------------
@@ -270,9 +270,9 @@ int pf_conv2d_wgrad(const pf_conv_desc* d, const float* x_dev, const float* dy_d
                     float* dw_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * a4  Convolution forward / dgrad on the tcgen05 tensor cores (pf_conv_tc.cu), same semantics as
+ * a4  Convolution forward / dgrad on the Hopper tensor cores (wgmma, pf_conv_tc.cu), same semantics as
  *     pf_conv2d_fwd / pf_conv2d_dgrad.  fp32 operands are split x = hi + lo (bf16 each) and each
- *     k-slice issues hi*hi + hi*lo + lo*hi into one fp32 TMEM accumulator (error ~2^-17 relative).
+ *     k-slice issues hi*hi + hi*lo + lo*hi into one fp32 register accumulator (error ~2^-17 relative).
  *     Requires Cin % 16 == 0 and Cout % 16 == 0 (pf_conv2d_tc_supported).
  *     Weights are pre-split and laid out K-major once per step by pf_conv2d_tc_prep_weight into
  *     caller-owned bf16 buffers of pf_conv2d_tc_weight_elems(d, dgrad) elements each, which the caller

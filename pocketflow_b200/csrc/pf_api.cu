@@ -23,6 +23,22 @@ const char* pf_last_error(void) { return g_err; }
 int64_t pf_launch_count(void) { return g_launches.load(); }
 void pf_launch_count_reset(void) { g_launches.store(0); }
 
+}  // extern "C"
+
+int pf_num_sms() {
+  static int cached[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+  if (cached[dev] <= 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 1;
+    cached[dev] = n;
+  }
+  return cached[dev];
+}
+
+extern "C" {
+
 int pf_sm_count(int* out) {
   PF_REQUIRE(out != nullptr, "pf_sm_count: null out");
   int dev = 0;

@@ -3,7 +3,7 @@
 // This is the EXACT-fp32 conv path: it reproduces tf.nn.conv2d / tf.matmul in fp32
 // (/root/reference/learners/uniform_quantization/utils.py:92-104 re-creates every conv on the
 // fake-quantized weight; autodiff supplies dgrad/wgrad, learner.py:247) with fp32 FFMA
-// accumulation, and is the on-device reference the tcgen05 path (pf_conv_tc.cu) is checked against.
+// accumulation, and is the on-device reference the tensor-core path (pf_conv_tc.cu) is checked against.
 // It also covers the shapes the tensor-core path does not take (Cin=3 first layers, Cout=10/1001
 // dense layers).  NHWC activations x HWIO kernels, so the weight is already the row-major
 // [K = R*S*Cin, Cout] B operand and the output is the row-major [M = N*P*Q, Cout] C operand.

@@ -1,10 +1,10 @@
-// pf_conv_tc.cu — convolution forward / dgrad on the 5th-generation tensor cores (tcgen05 + TMEM).
+// pf_conv_tc.cu — convolution forward / dgrad / wgrad on the Hopper tensor cores (warpgroup MMA, wgmma).
 //
 // The one genuine dense contraction of the step (SURVEY §8 a4: tf.nn.conv2d re-created on the
 // quantized weight, /root/reference/learners/uniform_quantization/utils.py:92-104, and its dgrad).
-// tcgen05 has no fp32 x fp32 MMA, and the parity bar is fp32 (1e-5 on losses), so operands are split
+// The tensor cores have no fp32 x fp32 MMA, and the parity bar is fp32 (1e-5 on losses), so operands are split
 //     x = hi + lo,  hi = bf16(x), lo = bf16(x - hi)         (representation error 2^-18)
-// and every k-slice issues three bf16 MMAs into ONE fp32 TMEM accumulator:
+// and every k-slice issues three bf16 MMAs into ONE fp32 register accumulator:
 //     D += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi               (the lo*lo term, 2^-18 relative, is dropped)
 //
 // Implicit GEMM, both operands K-major:  D[M x N] = A[M x K] * B[N x K]^T
@@ -36,14 +36,13 @@ constexpr int kMaxStages = 4;
 __device__ __forceinline__ void split4(const float4 v, uint2& hi, uint2& lo) { pf_split4(v, hi, lo); }
 
 // =============================================================================================
-// v4: PERSISTENT, warp-specialised fwd / dgrad kernel.  One CTA per SM loops over output tiles;
-//   warps 0-3   epilogue  (TMEM -> registers -> per-warp smem transpose -> coalesced global; bias / ReLU /
-//               residual / accumulate), overlapped with the next tile's main loop through a DOUBLE-BUFFERED
-//               TMEM accumulator (2 x BN columns);
-//   warps 4-11  producers (A gather + fp32 -> split-bf16 conversion with a register ping-pong that runs
-//               across tile boundaries; B via cp.async);
-//   warp  12    MMA issuer (one elected thread) + TMEM allocation.
-// BN goes up to 256 (A is read once for 256 output channels).  When one n-tile covers all output channels and
+// PERSISTENT, warp-specialised fwd / dgrad kernel.  One CTA per SM loops over output tiles;
+//   warps 0-7   two MMA warpgroups (wgmma, 64 rows each) that also run the epilogue (registers -> shared
+//               accumulator tile -> coalesced global; bias / ReLU / residual / accumulate) while the producers
+//               already fill the next tile's stages;
+//   warps 8-15  producers (A gather + fp32 -> split-bf16 conversion with a register ping-pong that runs
+//               across tile boundaries; B via cp.async).
+// BN goes up to 128 (the accumulator registers of a warpgroup).  When one n-tile covers all output channels and
 // the whole split weight matrix fits next to >= 2 A stages, B is loaded ONCE per CTA and stays resident
 // ("B-stationary": every 1x1 layer of the early stages, K <= 256).
 // MODE 2 = dgrad of a strided convolution decomposed into stride_h*stride_w pixel-parity classes: the rows of
@@ -59,14 +58,14 @@ struct TcClass {
 };
 struct TcP {
   TcGeom g;
-  int M, Ng, Kdim, Kpad, BN, nk, n_stages, n_bslots, b_stationary, m_tiles, n_tiles, total_tiles, acc_cols;
+  int M, Ng, Kdim, Kpad, BN, nk, n_stages, n_bslots, b_stationary, m_tiles, n_tiles, total_tiles;
   int accumulate, relu, ncls, cblocks, ring;
   FastDiv d_hw, d_w, d_cc, d_s, d_ntiles, d_cblocks;
   TcClass cls[kMaxClasses];
 };
 
 constexpr int kProdWarps = 8;
-constexpr int kThreadsP = (kEpiWarps + kProdWarps + 1) * 32;   // 416
+constexpr int kThreadsP = (kMmaWarps + kProdWarps) * 32;   // 512
 
 template <int MODE>
 __device__ __forceinline__ int tile_class(const TcP& p, int mt) {
@@ -79,7 +78,7 @@ __device__ __forceinline__ int tile_class(const TcP& p, int mt) {
   return ci;
 }
 
-template <int MODE, bool PLANES>
+template <int MODE, bool PLANES, int BN>
 __global__ void __launch_bounds__(kThreadsP, 1)
 conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __restrict__ a_hi_g,
                        const __nv_bfloat16* __restrict__ a_lo_g, const __nv_bfloat16* __restrict__ b_hi,
@@ -89,38 +88,28 @@ conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __res
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const TcGeom& g = p.g;
-  const int BN = p.BN;
   const uint32_t a_bytes = TM * 128, b_bytes = (uint32_t)BN * 128;
   uint8_t* smem_a = smem;                                           // n_stages x (hi, lo)
   uint8_t* smem_b = smem + (size_t)p.n_stages * 2 * a_bytes;        // n_bslots x (hi, lo)
-  float* stage_all = reinterpret_cast<float*>(smem_b + (size_t)p.n_bslots * 2 * b_bytes);
-  long long* rowoff_all = reinterpret_cast<long long*>(stage_all + kEpiWarps * 32 * kStagePitch);
-  uint8_t* ring_all = reinterpret_cast<uint8_t*>(rowoff_all + kEpiWarps * 32);   // p.ring: 4 warps x kRingDepth slots
-  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_s;
+  float* acc_s = reinterpret_cast<float*>(smem_b + (size_t)p.n_bslots * 2 * b_bytes);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  uint8_t* ring_all = reinterpret_cast<uint8_t*>(rowoff_all + kMmaWarps * 32);   // p.ring: 8 warps x kRingDepth slots
+  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
       mbar_init(&full_bar[s], kProdWarps * 32);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], kEpiWarps * 32);
+      mbar_init(&empty_bar[s], kMmaWarps);
     }
     fence_barrier_init();
   }
-  if (warp == kEpiWarps + kProdWarps) tmem_alloc(&tmem_base_s, (uint32_t)(2 * p.acc_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   const int first_tile = blockIdx.x, tile_step = gridDim.x;
 
-  if (warp >= kEpiWarps && warp < kEpiWarps + kProdWarps) {
+  if (warp >= kMmaWarps) {
     // =================================== producers ===================================
-    const int pt_ = tid - kEpiWarps * 32;
+    const int pt_ = tid - kMmaWarps * 32;
     const int l8 = pt_ & 7, rgrp = pt_ >> 3;          // 32-byte slice of the row, row group (rows rgrp + 32*i)
     const int CC = (MODE == 0) ? g.C : g.K;           // channels of the gathered tensor
     const uint32_t chunk_off = (((uint32_t)l8) ^ (uint32_t)(rgrp & 7)) << 4;
@@ -298,59 +287,48 @@ conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __res
       }
     }
     }
-  } else if (warp == kEpiWarps + kProdWarps) {
-    // =================================== MMA issuer ===================================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(TM, BN, 0, 0);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = first_tile; tile < p.total_tiles; tile += tile_step, ++tcount) {
-        int nk = p.nk;
-        if (MODE == 2) nk = p.cls[tile_class<MODE>(p, (int)fdiv((uint32_t)tile, p.d_ntiles))].ntaps * p.cblocks;
-        const uint32_t buf = tcount & 1u;
-        mbar_wait(&tempty_bar[buf], ((tcount >> 1) & 1u) ^ 1u);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * (uint32_t)p.acc_cols;
-        for (int ks = 0; ks < nk; ++ks, ++it) {
-          const uint32_t s = it % (uint32_t)p.n_stages;
-          mbar_wait(&full_bar[s], (it / (uint32_t)p.n_stages) & 1u);
-          if (PLANES) fence_proxy_async_smem();   // cp.async writes -> visible to the tensor core (async proxy)
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(smem_a + (size_t)s * 2 * a_bytes), a_lo = a_hi + a_bytes;
-          const uint32_t bh = smem_u32(smem_b + (size_t)(p.b_stationary ? ks : (int)s) * 2 * b_bytes), bl = bh + b_bytes;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t dah = make_smem_desc(a_hi + kk * 32, 16, 1024);
-            const uint64_t dal = make_smem_desc(a_lo + kk * 32, 16, 1024);
-            const uint64_t dbh = make_smem_desc(bh + kk * 32, 16, 1024);
-            const uint64_t dbl = make_smem_desc(bl + kk * 32, 16, 1024);
-            umma_bf16(d_tmem, dah, dbh, idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-            umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-            umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-          }
-          umma_commit(&empty_bar[s]);   // frees the A (and ring B) stage when these MMAs have completed
-        }
-        if (nk > 0) umma_commit(&tfull_bar[buf]);   // accumulator of this tile complete
-        else mbar_arrive(&tfull_bar[buf]);          // zero-tap class: nothing was issued, the epilogue writes zeros
-      }
-    }
   } else {
-    // =================================== epilogue (warps 0-3) ===================================
-    float* stg = stage_all + (size_t)warp * 32 * kStagePitch;
+    // ============================ MMA warpgroups + epilogue (warps 0-7) ============================
+    const int wg = warp >> 2;                // rows [64 wg, 64 wg + 64) of the tile
     long long* rowoff = rowoff_all + warp * 32;
     const float* extra = residual ? residual : (p.accumulate ? out : nullptr);
-    uint32_t tcount = 0;
-    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step, ++tcount) {
+    uint32_t it = 0;
+    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
       const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
       const int n0 = (tile - mt * p.n_tiles) * BN;
-      bool zero_tile = false;
+      int nk = p.nk;
+      if (MODE == 2) nk = p.cls[tile_class<MODE>(p, mt)].ntaps * p.cblocks;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < nk; ++ks, ++it) {
+        const uint32_t s = it % (uint32_t)p.n_stages;
+        mbar_wait(&full_bar[s], (it / (uint32_t)p.n_stages) & 1u);
+        if (PLANES) fence_proxy_async_smem();   // cp.async writes -> visible to the tensor core (async proxy)
+        const uint32_t a_hi = smem_u32(smem_a + (size_t)s * 2 * a_bytes) + (uint32_t)wg * 64 * 128, a_lo = a_hi + a_bytes;
+        const uint32_t bh = smem_u32(smem_b + (size_t)(p.b_stationary ? ks : (int)s) * 2 * b_bytes), bl = bh + b_bytes;
+        wg_mma_stage<BN, 0>(acc, a_hi, a_lo, bh, bl, 2, 2, 32, 32, 16, 1024, 16, 1024);
+        wgmma_wait<1>(acc);                      // the previous stage's MMAs have completed: release it
+        if (ks > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = s;
+      }
+      wgmma_wait<0>(acc);
+      if (nk > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
       long long off = -1;                    // global element offset of this lane's row (-1: beyond the problem)
+      const int row = (warp & 3) * 32 + lane;
       if (MODE != 2) {
-        const int m = mt * TM + warp * 32 + lane;
+        const int m = mt * TM + row;
         if (m < p.M) off = (long long)m * p.Ng;
       } else {
         const TcClass& k = p.cls[tile_class<MODE>(p, mt)];
-        zero_tile = k.ntaps == 0;
-        const int mc = (mt - k.tile_begin) * TM + warp * 32 + lane;
+        const int mc = (mt - k.tile_begin) * TM + row;
         if (mc < k.Mc) {
           const int hwc = k.Hc * k.Wc;
           const int n_ = (int)fdiv((uint32_t)mc, k.d_hw);
@@ -359,14 +337,11 @@ conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __res
           off = (((long long)n_ * g.H + (k.ph + y * g.sh)) * g.W + (k.pw + x * g.sw)) * g.C;
         }
       }
-      epilogue_tile(tmem_base + (tcount & 1u) * (uint32_t)p.acc_cols, &tfull_bar[tcount & 1u], &tempty_bar[tcount & 1u],
-                    (tcount >> 1) & 1u, zero_tile, off, rowoff, stg, out, extra, bias, p.relu, n0, BN, p.Ng, warp, lane,
+      wg_tile_to_smem<BN>(acc, acc_s, tid);
+      epilogue_tile(acc_s, warp, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
                     p.ring ? ring_all + (size_t)warp * kRingDepth * kRingSlotBytes : nullptr);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kEpiWarps + kProdWarps) tmem_dealloc(tmem_base, (uint32_t)(2 * p.acc_cols));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -388,14 +363,15 @@ split_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
 // wgrad v4: persistent, warp-specialised, operands read from PRE-SPLIT bf16 planes with cp.async straight into
 // the swizzled MN-major tiles (no register staging, no conversion in the loop; completion is signalled by
 // cp.async.mbarrier.arrive so producers never wait for data, only for a free stage).  Work unit = (kf tile of
-// 128, cout tile of BN <= 256, pixel range); units are ordered range-major so that the CTAs running together
+// 128, cout tile of BN <= 128, pixel range); units are ordered range-major so that the CTAs running together
 // read the same pixels.  Epilogue: the shared epilogue_tile() into partial[split][kf][cout].
 struct WgP {
   TcGeom g;
-  int Mtot, Npix, pps, splits, BN, m_tiles, n_tiles, tiles, total_units, n_stages, acc_cols;
+  int Mtot, Npix, pps, splits, BN, m_tiles, n_tiles, tiles, total_units, n_stages;
   FastDiv d_pq, d_q, d_c, d_s, d_tiles, d_ntiles;
 };
 
+template <int BN>
 __global__ void __launch_bounds__(kThreadsP, 1)
 conv_tc_wgrad_persist_kernel(const __nv_bfloat16* __restrict__ x_hi, const __nv_bfloat16* __restrict__ x_lo,
                              const __nv_bfloat16* __restrict__ dy_hi, const __nv_bfloat16* __restrict__ dy_lo,
@@ -403,30 +379,20 @@ conv_tc_wgrad_persist_kernel(const __nv_bfloat16* __restrict__ x_hi, const __nv_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const TcGeom& g = p.g;
-  const int BN = p.BN;
   const uint32_t a_bytes = BK * TM * 2, b_bytes = (uint32_t)BK * BN * 2;   // one bf16 tile
   const uint32_t stage_bytes = 2 * a_bytes + 2 * b_bytes;
-  float* stage_all = reinterpret_cast<float*>(smem + (size_t)p.n_stages * stage_bytes);
-  long long* rowoff_all = reinterpret_cast<long long*>(stage_all + kEpiWarps * 32 * kStagePitch);
-  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_s;
+  float* acc_s = reinterpret_cast<float*>(smem + (size_t)p.n_stages * stage_bytes);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
       mbar_init(&full_bar[s], kProdWarps * 32);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], kEpiWarps * 32);
+      mbar_init(&empty_bar[s], kMmaWarps);
     }
     fence_barrier_init();
   }
-  if (warp == kEpiWarps + kProdWarps) tmem_alloc(&tmem_base_s, (uint32_t)(2 * p.acc_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   const int mbA = TM / 64, mbB = BN / 64;
   struct Unit {
     int split, m0, n0, pbeg, nk;
@@ -444,9 +410,9 @@ conv_tc_wgrad_persist_kernel(const __nv_bfloat16* __restrict__ x_hi, const __nv_
     return r;
   };
 
-  if (warp >= kEpiWarps && warp < kEpiWarps + kProdWarps) {
+  if (warp >= kMmaWarps) {
     // =================================== producers ===================================
-    const int pt_ = tid - kEpiWarps * 32;
+    const int pt_ = tid - kMmaWarps * 32;
     const int l16 = pt_ & 15, pg = pt_ >> 4;           // 16-byte chunk of the 128-wide MN extent, pixel group
     const uint32_t k8 = (uint32_t)(pg & 7);            // (pixel & 7) of every pixel of this thread (pixels pg + 16*i)
     const uint32_t a_mblk = (uint32_t)(l16 >> 3), chunk = (uint32_t)(l16 & 7);
@@ -500,58 +466,44 @@ conv_tc_wgrad_persist_kernel(const __nv_bfloat16* __restrict__ x_hi, const __nv_
       }
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
-  } else if (warp == kEpiWarps + kProdWarps) {
-    // =================================== MMA issuer ===================================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(TM, BN, 1, 1);
-      const uint32_t sbo_a = (uint32_t)mbA * 1024u, sbo_b = (uint32_t)mbB * 1024u;
-      uint32_t it = 0, tcount = 0;
-      for (int u = blockIdx.x; u < p.total_units; u += gridDim.x, ++tcount) {
-        const Unit un = decode(u);
-        const uint32_t buf = tcount & 1u;
-        mbar_wait(&tempty_bar[buf], ((tcount >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * (uint32_t)p.acc_cols;
-        for (int ks = 0; ks < un.nk; ++ks, ++it) {
-          const uint32_t s = it % (uint32_t)p.n_stages;
-          mbar_wait(&full_bar[s], (it / (uint32_t)p.n_stages) & 1u);
-          fence_proxy_async_smem();      // cp.async (generic proxy) writes -> visible to the tensor core (async proxy)
-          tc_fence_after();
-          const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
-          const uint32_t a_hi = base, a_lo = base + a_bytes, bh = base + 2 * a_bytes, bl = bh + b_bytes;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t dah = make_smem_desc(a_hi + kk * 2 * sbo_a, 1024, sbo_a);
-            const uint64_t dal = make_smem_desc(a_lo + kk * 2 * sbo_a, 1024, sbo_a);
-            const uint64_t dbh = make_smem_desc(bh + kk * 2 * sbo_b, 1024, sbo_b);
-            const uint64_t dbl = make_smem_desc(bl + kk * 2 * sbo_b, 1024, sbo_b);
-            umma_bf16(d_tmem, dah, dbh, idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-            umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-            umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        if (un.nk > 0) umma_commit(&tfull_bar[buf]);
-        else mbar_arrive(&tfull_bar[buf]);
-      }
-    }
   } else {
-    // =================================== epilogue: D rows = kf, columns = cout ===================================
-    float* stg = stage_all + (size_t)warp * 32 * kStagePitch;
+    // ============================ MMA warpgroups + epilogue: D rows = kf, columns = cout ============================
+    const int wg = warp >> 2;                // kf rows [64 wg, 64 wg + 64) = MN block wg of the A tile
+    const uint32_t sbo_a = (uint32_t)mbA * 1024u, sbo_b = (uint32_t)mbB * 1024u;
     long long* rowoff = rowoff_all + warp * 32;
-    uint32_t tcount = 0;
-    for (int u = blockIdx.x; u < p.total_units; u += gridDim.x, ++tcount) {
+    uint32_t it = 0;
+    for (int u = blockIdx.x; u < p.total_units; u += gridDim.x) {
       const Unit un = decode(u);
-      const int em = un.m0 + warp * 32 + lane;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < un.nk; ++ks, ++it) {
+        const uint32_t s = it % (uint32_t)p.n_stages;
+        mbar_wait(&full_bar[s], (it / (uint32_t)p.n_stages) & 1u);
+        fence_proxy_async_smem();      // cp.async (generic proxy) writes -> visible to the tensor core (async proxy)
+        const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t a_hi = base + (uint32_t)wg * 1024u, a_lo = a_hi + a_bytes, bh = base + 2 * a_bytes, bl = bh + b_bytes;
+        // MN-major: LBO = stride between 64-wide MN blocks, SBO = stride between 8-pixel groups; 16 pixels per MMA
+        wg_mma_stage<BN, 1>(acc, a_hi, a_lo, bh, bl, 2, 2, 2 * sbo_a, 2 * sbo_b, 1024, sbo_a, 1024, sbo_b);
+        wgmma_wait<1>(acc);
+        if (ks > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = s;
+      }
+      wgmma_wait<0>(acc);
+      if (un.nk > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      const int em = un.m0 + (warp & 3) * 32 + lane;
       const long long off = em < p.Mtot ? ((long long)un.split * p.Mtot + em) * g.K : -1;
-      epilogue_tile(tmem_base + (tcount & 1u) * (uint32_t)p.acc_cols, &tfull_bar[tcount & 1u], &tempty_bar[tcount & 1u],
-                    (tcount >> 1) & 1u, un.nk == 0, off, rowoff, stg, partial, nullptr, nullptr, 0, un.n0, BN, g.K, warp,
-                    lane);
+      wg_tile_to_smem<BN>(acc, acc_s, tid);
+      epilogue_tile(acc_s, warp, off, rowoff, partial, nullptr, nullptr, 0, un.n0, BN, g.K, lane);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kEpiWarps + kProdWarps) tmem_dealloc(tmem_base, (uint32_t)(2 * p.acc_cols));
 }
 
 __global__ void __launch_bounds__(256)
@@ -660,27 +612,17 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
                    const void* b_lo, float* out, const float* bias, const float* residual, cudaStream_t st,
                    const char* who) {
   const int Ng = p.Ng;
-  // ---- tile width: wide tiles read A once per 256 channels, but quantise worse over the 148 SMs
-  int BN;
-  if (Ng >= 256) {
-    const int64_t t256 = (int64_t)p.m_tiles * ((Ng + 255) / 256), t128 = (int64_t)p.m_tiles * ((Ng + 127) / 128);
-    const double c256 = (double)((t256 + PF_NUM_SMS - 1) / PF_NUM_SMS) * 1.3;   // measured: a 256-wide tile costs ~1.3x
-    const double c128 = (double)((t128 + PF_NUM_SMS - 1) / PF_NUM_SMS);
-    BN = c256 <= c128 ? 256 : 128;
-  } else {
-    BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
-  }
+  // ---- tile width: the widest the warpgroup accumulators allow
+  int BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
   const int forced = env_int("PF_TC_BN", 0);           // development knob
-  if (forced >= 16 && forced <= 256 && forced <= ((Ng + 15) / 16) * 16 && (forced & (forced - 1)) == 0) BN = forced;
+  if (forced >= 16 && forced <= kMaxBN && forced <= ((Ng + 15) / 16) * 16 && (forced & (forced - 1)) == 0) BN = forced;
   p.BN = BN;
   p.n_tiles = (Ng + BN - 1) / BN;
   p.total_tiles = p.m_tiles * p.n_tiles;
   p.d_ntiles = make_fastdiv((uint32_t)p.n_tiles);
-  p.acc_cols = 32;
-  while (p.acc_cols < BN) p.acc_cols <<= 1;
   // ---- shared memory plan
   const int a_stage = 2 * TM * 128, b_slot = 2 * BN * 128;
-  const int fixed = 1024 + kEpiWarps * 32 * kStagePitch * 4 + kEpiWarps * 32 * 8 + 256;
+  const int fixed = epi_fixed_bytes(BN);
   const int budget = kSmemLimit - fixed;
   int max_nk = p.nk;
   if (MODE == 2) {
@@ -688,7 +630,7 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
     for (int c = 0; c < p.ncls; ++c) max_nk = std::max(max_nk, p.cls[c].ntaps * p.cblocks);
   }
   // the epilogue's residual / accumulate operand goes through a cp.async ring when the stages leave room for it
-  const int ring_bytes = kEpiWarps * kRingDepth * kRingSlotBytes;
+  const int ring_bytes = kMmaWarps * kRingDepth * kRingSlotBytes;
   const bool has_extra = residual != nullptr || p.accumulate;
   int budget_r = budget;
   p.ring = 0;
@@ -715,17 +657,23 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
   const size_t smem = (size_t)p.n_stages * a_stage + (size_t)p.n_bslots * b_slot + fixed + (p.ring ? ring_bytes : 0);
   if (p.total_tiles == 0) return PF_OK;
   const int grid = std::min(p.total_tiles, PF_NUM_SMS);
-  if (a_hi) {
-    auto kern = conv_tc_persist_kernel<MODE, true>;
-    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kThreadsP, smem, st>>>(nullptr, (const __nv_bfloat16*)a_hi, (const __nv_bfloat16*)a_lo,
-                                        (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo, out, bias, residual, p);
-  } else {
-    auto kern = conv_tc_persist_kernel<MODE, false>;
-    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kThreadsP, smem, st>>>(src, nullptr, nullptr, (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo, out,
-                                        bias, residual, p);
-  }
+  cudaError_t err = cudaSuccess;
+  with_bn(BN, [&](auto bn) {
+    if (a_hi) {
+      auto kern = conv_tc_persist_kernel<MODE, true, decltype(bn)::value>;
+      err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (err == cudaSuccess)
+        kern<<<grid, kThreadsP, smem, st>>>(nullptr, (const __nv_bfloat16*)a_hi, (const __nv_bfloat16*)a_lo,
+                                            (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo, out, bias, residual, p);
+    } else {
+      auto kern = conv_tc_persist_kernel<MODE, false, decltype(bn)::value>;
+      err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (err == cudaSuccess)
+        kern<<<grid, kThreadsP, smem, st>>>(src, nullptr, nullptr, (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo,
+                                            out, bias, residual, p);
+    }
+  });
+  PF_CUDA(err);
   PF_CHECK_LAUNCH(who);
   return PF_OK;
 }
@@ -818,15 +766,15 @@ inline void wgrad_plan(const TcGeom& g, WgP* pp) {
   p.g = g;
   p.Mtot = g.R * g.S * g.C;
   p.Npix = g.N * g.P * g.Q;
-  int BN = g.K >= 256 ? 256 : (g.K >= 128 ? 128 : 64);
+  int BN = g.K >= 128 ? 128 : 64;
   const int forced = env_int("PF_TC_WGRAD_BN", 0);
-  if ((forced == 64 || forced == 128 || forced == 256) && forced <= g.K) BN = forced;
+  if ((forced == 64 || forced == 128) && forced <= g.K) BN = forced;
   p.BN = BN;
   p.m_tiles = (p.Mtot + TM - 1) / TM;
   p.n_tiles = (g.K + BN - 1) / BN;
   p.tiles = p.m_tiles * p.n_tiles;
   // enough units to fill the SMs a few times over, but at least 8 k-stages (512 pixels) per unit
-  // (rounded DOWN: total units just under a whole number of waves over the 148 SMs)
+  // (rounded DOWN: total units just under a whole number of waves over the SMs)
   int splits = (env_int("PF_TC_WGRAD_WAVES", 1) * PF_NUM_SMS) / p.tiles;
   const int max_by_k = (p.Npix + 8 * BK - 1) / (8 * BK);
   splits = std::max(1, std::min(std::min(splits, max_by_k), PF_CONV_TC_WGRAD_MAX_SPLITS));
@@ -835,9 +783,7 @@ inline void wgrad_plan(const TcGeom& g, WgP* pp) {
   p.pps = pps;
   p.splits = (p.Npix + pps - 1) / pps;
   p.total_units = p.tiles * p.splits;
-  p.acc_cols = 32;
-  while (p.acc_cols < BN) p.acc_cols <<= 1;
-  const int fixed = 1024 + kEpiWarps * 32 * kStagePitch * 4 + kEpiWarps * 32 * 8 + 256;
+  const int fixed = epi_fixed_bytes(BN);
   p.n_stages = std::max(1, std::min(kMaxStages, (kSmemLimit - fixed) / (2 * BK * TM * 2 + 2 * BK * BN * 2)));
   p.d_pq = make_fastdiv((uint32_t)(g.P * g.Q));
   p.d_q = make_fastdiv((uint32_t)g.Q);
@@ -1029,13 +975,12 @@ static int tc_wgrad_impl(const pf_conv_desc* d, const pf_tc_act& x, const pf_tc_
     if (rc) return rc;
   } else {
     PF_REQUIRE(x.hdr == nullptr && x.plane1 != nullptr, "%s: quantizer-level operands need the TMA kernels (Cin %% 64 == 0)", who);
-    const int fixed = 1024 + kEpiWarps * 32 * kStagePitch * 4 + kEpiWarps * 32 * 8 + 256;
-    const size_t smem = (size_t)p.n_stages * (2 * BK * TM * 2 + 2 * BK * p.BN * 2) + fixed;
-    PF_CUDA(cudaFuncSetAttribute(conv_tc_wgrad_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = (size_t)p.n_stages * (2 * BK * TM * 2 + 2 * BK * p.BN * 2) + epi_fixed_bytes(p.BN);
     const int grid = std::min(p.total_units, PF_NUM_SMS);
-    conv_tc_wgrad_persist_kernel<<<grid, kThreadsP, smem, st>>>(
-        (const __nv_bfloat16*)x.plane0, (const __nv_bfloat16*)x.plane1, (const __nv_bfloat16*)dy.plane0,
-        (const __nv_bfloat16*)dy.plane1, partial, p);
+    auto kern = p.BN == 128 ? conv_tc_wgrad_persist_kernel<128> : conv_tc_wgrad_persist_kernel<64>;
+    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, kThreadsP, smem, st>>>((const __nv_bfloat16*)x.plane0, (const __nv_bfloat16*)x.plane1,
+                                        (const __nv_bfloat16*)dy.plane0, (const __nv_bfloat16*)dy.plane1, partial, p);
     PF_CHECK_LAUNCH(who);
   }
   if (p.splits > 1 && dw_dev) {

@@ -1,10 +1,11 @@
-// pf_conv_tc.cuh — pieces shared by the tcgen05 convolution kernels (pf_conv_tc.cu: cp.async-fed, any channel
+// pf_conv_tc.cuh — pieces shared by the wgmma convolution kernels (pf_conv_tc.cu: cp.async-fed, any channel
 // count that is a multiple of 16; pf_conv_tma.cu: TMA-fed, channel counts that are multiples of 64):
-// tile constants, geometry, exact division by runtime constants, and the TMEM -> global epilogue.
+// tile constants, geometry, exact division by runtime constants, the warpgroup main loop and the epilogue.
 #pragma once
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "pf_common.cuh"
 #include "pf_tc_common.cuh"
@@ -12,9 +13,9 @@
 namespace pfconv {
 using namespace pftc;
 
-constexpr int TM = 128;      // GEMM rows per CTA (= TMEM lanes)
+constexpr int TM = 128;      // GEMM rows per CTA (two m64 warpgroups)
 constexpr int BK = 64;       // bf16 elements per k-stage (= one 128-byte swizzled row)
-constexpr int kSmemLimit = 232448;   // 227 KB opt-in maximum of dynamic shared memory per CTA on sm_100
+constexpr int kSmemLimit = 232448;   // 227 KB opt-in maximum of dynamic shared memory per CTA on sm_90
 
 struct TcGeom {
   int N, H, W, C, K, R, S, P, Q, sh, sw, pt, pl;
@@ -41,11 +42,51 @@ inline int env_int(const char* name, int dflt) {
 int tc_geom(const pf_conv_desc* d, TcGeom* g, const char* who);
 
 // ---------------------------------------------------------------------------------------------------------
-// Epilogue of one 128 x BN accumulator tile by 4 epilogue warps (the warp with quarter index q = warp % 4 owns TMEM
-// lanes [32q, 32q+32)): TMEM -> registers (thread = row, 32 columns) -> per-warp smem transpose -> 128-byte row
-// segments to global.
-// `extra` (residual / accumulate operand, same indexing as `out`) is prefetched one 32-column chunk ahead,
-// and the first chunk is requested BEFORE waiting for the accumulator, so its latency hides behind the main loop.
+// Main loop and epilogue warps.  Warps 0-7 of every tensor-core kernel are two warpgroups: warpgroup g issues the
+// wgmma of GEMM rows [64 g, 64 g + 64) of the 128 x BN tile into registers; at the end of a tile both write their
+// accumulators into one fp32 tile in shared memory (row pitch BN + 4 floats), and the same 8 warps then run the
+// epilogue from there: warp w owns rows [32 (w % 4), 32 (w % 4) + 32) and every other 32-column chunk starting at
+// chunk w / 4.  The producers (cp.async warps or the TMA thread) keep filling the next tile's stages meanwhile.
+constexpr int kMmaWarps = 8;
+constexpr int kMaxBN = 128;                                    // 64 accumulator registers per thread and warpgroup
+__host__ __device__ constexpr int acc_pitch(int BN) { return BN + 4; }
+__host__ __device__ constexpr int acc_tile_bytes(int BN) { return TM * acc_pitch(BN) * 4; }
+// accumulator tile + per-warp row-offset and J tables
+__host__ __device__ constexpr int epi_fixed_bytes(int BN) { return 1024 + acc_tile_bytes(BN) + kMmaWarps * 32 * (8 + 4) + 256; }
+
+// One k-stage of MMAs of warpgroup `wg` (wtid = thread index inside the warpgroup is implied): per 16-wide k-slice
+// the products  A0 B0 (+ A0 B1 when nb == 2) (+ A1 B0 when na == 2)  of the bf16 planes (hi / lo, or integer levels).
+// a0 / a1 / b0 / b1 are the shared-memory addresses of the planes; a_kstep / b_kstep the byte step of one 16-wide
+// k-slice; lbo / sbo the descriptor strides.
+template <int BN, int TMN>
+__device__ __forceinline__ void wg_mma_stage(float (&acc)[BN / 2], uint32_t a0, uint32_t a1, uint32_t b0, uint32_t b1,
+                                             int na, int nb, uint32_t a_kstep, uint32_t b_kstep, uint32_t lbo_a,
+                                             uint32_t sbo_a, uint32_t lbo_b, uint32_t sbo_b) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < BK / 16; ++kk) {
+    const uint64_t da0 = make_smem_desc(a0 + kk * a_kstep, lbo_a, sbo_a);
+    const uint64_t db0 = make_smem_desc(b0 + kk * b_kstep, lbo_b, sbo_b);
+    Wgmma<BN>::template mma<TMN, TMN>(acc, da0, db0);
+    if (nb == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, da0, make_smem_desc(b1 + kk * b_kstep, lbo_b, sbo_b));
+    if (na == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, make_smem_desc(a1 + kk * a_kstep, lbo_a, sbo_a), db0);
+  }
+  wgmma_commit();
+}
+
+// End of a tile's main loop: wait for the last MMAs, release their stage, and hand the accumulator to the epilogue
+// through the shared tile.  Named barrier 1 spans the 8 MMA warps: the first one keeps this tile's stores behind the
+// previous tile's epilogue reads, the second makes the stores visible to every epilogue warp.
+template <int BN>
+__device__ __forceinline__ void wg_tile_to_smem(float (&acc)[BN / 2], float* acc_s, int tid) {
+  named_bar_sync(1, kMmaWarps * 32);
+  wgmma_store_acc<BN>(acc, acc_s, acc_pitch(BN), 64 * (tid >> 7), tid & 127);
+  named_bar_sync(1, kMmaWarps * 32);
+}
+
+// Epilogue of one 128 x BN accumulator tile by one warp: rows of this warp are `acc` + i * pitch (i < 32); the warp's
+// lanes write 128-byte row segments to global.
+// `extra` (residual / accumulate operand, same indexing as `out`) is prefetched one 32-column chunk ahead.
 // EXTRA: 0 = none; 1 = extra operand prefetched one chunk ahead in registers; 2 = extra operand streamed through a
 // per-warp cp.async ring in shared memory, kRingDepth chunks (4 KB each) in flight per warp.
 // AFF: the accumulator holds a product of INTEGER quantizer levels (SURVEY §7 hard part 1b): with
@@ -53,16 +94,8 @@ int tc_geom(const pf_conv_desc* d, TcGeom* g, const char* who);
 // the convolution of the fake-quantized tensors is   s_a s_c * sum_k j (n - centre)  +  s_a o_c * J[m],
 // J[m] = sum of the activation levels under the filter window of output row m (computed by the row's thread from
 // per-pixel channel sums and handed in as `my_j`).  AFF 1: only the scalar s_a (weight gradient: j (x) dy).
-constexpr int kEpiWarps = 4;
-constexpr int kStagePitch = 36;                                // floats per staged row (32 + 4: conflict-free)
 constexpr int kRingDepth = 4;
 constexpr int kRingSlotBytes = 32 * 32 * 4;
-constexpr int kEpiFixedBytes = 1024 + kEpiWarps * 32 * kStagePitch * 4 + kEpiWarps * 32 * 8 + kEpiWarps * 32 * 4 + 256;
-
-// TMA-fed kernels: 8 epilogue warps (two per TMEM lane quarter, even / odd 32-column chunks), each with its own staging
-// tile, row-offset table, J table and (optional) residual ring
-constexpr int kTmaEpiWarps = 8;
-constexpr int kTmaEpiFixedBytes = 1024 + kTmaEpiWarps * (32 * kStagePitch * 4 + 32 * 8 + 32 * 4) + 256;
 
 struct EpiAff {
   const float* w_alpha;    // per-bucket alpha = (max - min) + 1e-10 of the weight quantizer (device)
@@ -73,18 +106,15 @@ struct EpiAff {
 };
 
 template <int EXTRA, int AFF, int RD = kRingDepth>
-__device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull, uint64_t* tempty, uint32_t parity,
-                                                bool zero_tile, long long my_row_off, long long* __restrict__ rowoff,
-                                                float* __restrict__ stg, float* __restrict__ out,
+__device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, int pitch, long long my_row_off,
+                                                long long* __restrict__ rowoff, float* __restrict__ out,
                                                 const float* __restrict__ extra, const float* __restrict__ bias,
-                                                int relu, int n0, int BN, int Ng, int q, int lane, uint8_t* ring,
+                                                int relu, int n0, int BN, int Ng, int lane, uint8_t* ring,
                                                 const EpiAff& aff, float my_j, float* __restrict__ jrow,
-                                                int c_begin = 0, int c_step = 32,
-                                                const float* __restrict__ aff_tab = nullptr) {
+                                                int c_begin, int c_step, const float* __restrict__ aff_tab) {
   // aff_tab (AFF == 2, TMA-fed kernels): the tile's per-column epilogue constants e1[c] (at c) and e2[c] (at 256 + c)
   // in shared memory, computed once per tile column range instead of being re-derived from global memory per chunk
-  // c_begin / c_step: this warp handles the 32-column chunks c_begin, c_begin + c_step, ... (two warps of the same TMEM
-  // lane quarter split a tile's columns between them in the TMA-fed kernels: c_step = 64)
+  // c_begin / c_step: this warp handles the 32-column chunks c_begin, c_begin + c_step, ...
   rowoff[lane] = my_row_off;
   if (AFF == 2) jrow[lane] = my_j;
   __syncwarp();
@@ -97,6 +127,7 @@ __device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull,
     ro[u] = o < 0 ? -1 : (int)(o >> 2);          // row offsets are multiples of 4 elements (channel counts % 16 == 0)
     jr[u] = (AFF == 2) ? jrow[4 * u + rsub] : 0.f;
   }
+  __syncwarp();                                  // rowoff / jrow are rewritten by the next tile
   const float a_s = (AFF && aff.a_scale && !(AFF == 2 && aff_tab)) ? __ldg(aff.a_scale) : 1.f;
   auto load_extra = [&](int c0, float4 (&xv)[8]) {
     const int cv = c0 + csub;
@@ -130,12 +161,8 @@ __device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull,
 #pragma unroll
     for (int c = 0; c < RD; ++c) ring_issue(c_begin + c_step * c, c);
   }
-  mbar_wait_bounded(tfull, parity);
-  tc_fence_after();
-  const uint32_t t_addr = t_acc + (((uint32_t)(q * 32)) << 16);
   int it = 0;
   for (int c0 = c_begin; c0 < BN; c0 += c_step, ++it) {
-    // per-column constants first: their global loads overlap the TMEM read below
     // rows 4*u + (lane >> 3), 16-byte chunk (lane & 7): 8 lanes write one row's 128 contiguous bytes
     const int cv = c0 + csub;
     const bool cok = cv < BN && n0 + cv + 3 < Ng;
@@ -162,24 +189,6 @@ __device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull,
       e2 = make_float4(fmaf(aff.w_centre, sx, be.x) * a_s, fmaf(aff.w_centre, sy, be.y) * a_s,
                        fmaf(aff.w_centre, sz, be.z) * a_s, fmaf(aff.w_centre, sw_, be.w) * a_s);
     }
-    // (issuing the NEXT chunk's TMEM read right after the staging stores, to run its latency under this chunk's
-    // read-back and global stores, keeps 32 more registers live through that phase: 2-3 KB of spills at the 168
-    // registers 10 warps allow — measured at compile time, not pursued)
-    uint32_t r[32];
-    if (!zero_tile) {
-      tmem_ld_32x32(t_addr + (uint32_t)c0, r);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) r[j] = 0u;
-    }
-    if (c0 + c_step >= BN) {                     // last read of this accumulator: hand it back to the MMA warp
-      tc_fence_before();
-      mbar_arrive(tempty);
-    }
-#pragma unroll
-    for (int j = 0; j < 32; j += 4)
-      *reinterpret_cast<uint4*>(stg + lane * kStagePitch + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-    __syncwarp();
     if (EXTRA == 1 && c0 + c_step < BN) load_extra(c0 + c_step, xb);
     if (EXTRA == 2) asm volatile("cp.async.wait_group %0;" ::"n"(RD - 1) : "memory");   // chunk c0 has landed
     const float* slot = reinterpret_cast<const float*>(ring + (size_t)(it & (RD - 1)) * kRingSlotBytes);
@@ -188,7 +197,8 @@ __device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull,
       float4 v[4], xr[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        v[u] = *reinterpret_cast<const float4*>(stg + (4 * (4 * half + u) + rsub) * kStagePitch + csub);
+        v[u] = (cv < BN) ? *reinterpret_cast<const float4*>(acc + (size_t)(4 * (4 * half + u) + rsub) * pitch + cv)
+                         : make_float4(0.f, 0.f, 0.f, 0.f);
         if (EXTRA == 2) xr[u] = *reinterpret_cast<const float4*>(slot + (4 * (4 * half + u) + rsub) * 32 + csub);
       }
 #pragma unroll
@@ -211,41 +221,50 @@ __device__ __forceinline__ void epilogue_tile_t(uint32_t t_acc, uint64_t* tfull,
         *reinterpret_cast<float4*>(out + ((size_t)ro[uu] << 2) + n0 + cv) = w;
       }
     }
-    __syncwarp();                                // the staging buffer is overwritten by the next chunk
     if (EXTRA == 1) {
 #pragma unroll
       for (int u = 0; u < 8; ++u) xa[u] = xb[u];
     }
-    if (EXTRA == 2) ring_issue(c0 + c_step * RD, it + RD);   // refill the slot just consumed
+    if (EXTRA == 2) {
+      __syncwarp();                              // every lane has read the slot before it is refilled
+      ring_issue(c0 + c_step * RD, it + RD);
+    }
   }
   if (EXTRA == 2) asm volatile("cp.async.wait_group 0;" ::: "memory");
-  if (c_begin >= BN) {                           // no chunk for this warp (BN < 64): release the accumulator all the same
-    tc_fence_before();
-    mbar_arrive(tempty);
-  }
 }
 
+// the epilogue of warp `ew` (0..7) of the MMA warps: rows 32 (ew % 4) .., chunks ew / 4, ew / 4 + 2, ...
 template <int AFF>
-__device__ __forceinline__ void epilogue_tile_a(uint32_t t_acc, uint64_t* tfull, uint64_t* tempty, uint32_t parity,
-                                                bool zero_tile, long long my_row_off, long long* rowoff, float* stg,
+__device__ __forceinline__ void epilogue_tile_a(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
                                                 float* __restrict__ out, const float* __restrict__ extra,
                                                 const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
-                                                int q, int lane, uint8_t* ring, const EpiAff& aff, float my_j,
-                                                float* jrow, int c_begin = 0, int c_step = 32,
+                                                int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
                                                 const float* aff_tab = nullptr, int ring_depth = kRingDepth) {
-  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2>(t_acc, tfull, tempty, parity, zero_tile, my_row_off, rowoff, stg, out, extra, bias, relu, n0, BN, Ng, q, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra && ring) epilogue_tile_t<2, AFF>(t_acc, tfull, tempty, parity, zero_tile, my_row_off, rowoff, stg, out, extra, bias, relu, n0, BN, Ng, q, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra) epilogue_tile_t<1, AFF>(t_acc, tfull, tempty, parity, zero_tile, my_row_off, rowoff, stg, out, extra, bias, relu, n0, BN, Ng, q, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else epilogue_tile_t<0, AFF>(t_acc, tfull, tempty, parity, zero_tile, my_row_off, rowoff, stg, out, nullptr, bias, relu, n0, BN, Ng, q, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  const int pitch = acc_pitch(BN);
+  const float* acc = acc_s + (size_t)(32 * (ew & 3)) * pitch;
+  const int c_begin = 32 * (ew >> 2), c_step = 64;
+  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else if (extra && ring) epilogue_tile_t<2, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else if (extra) epilogue_tile_t<1, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else epilogue_tile_t<0, AFF>(acc, pitch, my_row_off, rowoff, out, nullptr, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
 }
-__device__ __forceinline__ void epilogue_tile(uint32_t t_acc, uint64_t* tfull, uint64_t* tempty, uint32_t parity,
-                                              bool zero_tile, long long my_row_off, long long* rowoff, float* stg,
+__device__ __forceinline__ void epilogue_tile(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
                                               float* __restrict__ out, const float* __restrict__ extra,
                                               const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
-                                              int q, int lane, uint8_t* ring = nullptr) {
+                                              int lane, uint8_t* ring = nullptr) {
   const EpiAff none{};
-  epilogue_tile_a<0>(t_acc, tfull, tempty, parity, zero_tile, my_row_off, rowoff, stg, out, extra, bias, relu, n0, BN, Ng,
-                     q, lane, ring, none, 0.f, nullptr);
+  epilogue_tile_a<0>(acc_s, ew, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, none, 0.f, nullptr);
+}
+
+// dispatch on the tile width (the wgmma N is an immediate): f is called with std::integral_constant<int, BN>
+template <class F>
+inline void with_bn(int BN, F&& f) {
+  switch (BN) {
+    case 16: f(std::integral_constant<int, 16>()); break;
+    case 32: f(std::integral_constant<int, 32>()); break;
+    case 64: f(std::integral_constant<int, 64>()); break;
+    default: f(std::integral_constant<int, 128>()); break;
+  }
 }
 
 // ---- TMA-fed kernels (pf_conv_tma.cu)

@@ -1,4 +1,4 @@
-// pf_conv_tma.cu — the tcgen05 convolution kernels fed by the Tensor Memory Accelerator (sm_100a).
+// pf_conv_tma.cu — the wgmma convolution kernels fed by the Tensor Memory Accelerator (sm_90a).
 //
 // Same contraction as pf_conv_tc.cu (SURVEY §8 a4: tf.nn.conv2d re-created on the quantized weight,
 // /root/reference/learners/uniform_quantization/utils.py:92-104, its dgrad and wgrad), for channel counts that are
@@ -7,7 +7,8 @@
 //     (128 filter-window positions x 64 channels of one tap; the padding is TMA's out-of-bounds zero fill), the
 //     K-major weight matrix / the dy matrix by tiled TMA loads — one elected thread issues them, completion is counted
 //     in bytes on the stage's mbarrier.  No LSU instruction touches an operand; producer warps are gone
-//     (6 warps: TMA, MMA, 4 x epilogue instead of 13), stages are as deep as shared memory allows (up to 8);
+//     (9 warps: two MMA + epilogue warpgroups and the TMA warp instead of 16), stages are as deep as shared memory
+//     allows (up to 8);
 //   * an operand that is a <= 8-bit fake-quantized tensor arrives as its INTEGER LEVELS (exact in bf16): one plane
 //     instead of hi + lo.  MMAs per k-slice: levels x levels 1, levels x split 2, split x split 3; the per-channel
 //     scale, and the rank-1 term that the weight offset contributes, are applied by the epilogue (pf_conv_tc.cuh).
@@ -20,17 +21,17 @@ namespace pfconv {
 using namespace pftma;
 
 constexpr int kTmaMaxStages = 8;
-constexpr int kTmaThreads = (2 + kTmaEpiWarps) * 32;     // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-9: epilogue
+constexpr int kTmaThreads = (kMmaWarps + 1) * 32;     // warps 0-7: MMA warpgroups + epilogue, warp 8: TMA producer
 constexpr uint32_t kATileBytes = TM * 128;
 
 struct TmaP {
-  int M, Ng, BN, nk, n_tiles, total_tiles, acc_cols;
+  int M, Ng, BN, nk, n_tiles, total_tiles;
   int cblocks, R, S;                       // k-stage ks -> tap = ks / cblocks (r = tap / S, q = tap % S), channel block
   int rows_hw, rows_w;                     // GEMM row m -> (image, y, x)
   int src_h, src_w;                        // gathered tensor
   int base_w, base_h, str_w, str_h, flip;  // window origin of row (y, x): (base + x * str); flip: tap offsets mirrored
   int na, nb;                              // operand planes (na: upper bound when a_hdr decides)
-  int accumulate, relu, ring, stage_budget, epi_warps;     // ring: 0 = none, else the residual ring's depth (2 or 4)
+  int accumulate, relu, ring, stage_budget;     // ring: 0 = none, else the residual ring's depth (2 or 4)
   FastDiv d_hw, d_w, d_ntiles, d_cblocks, d_s;
   EpiAff aff;
   const pf_tc_act_hdr* a_hdr;
@@ -40,8 +41,8 @@ struct TmaP {
 
 // ---------------------------------------------------------------------------------------------------------
 // fwd / dgrad (unit stride): D[M x Ng] = A[M x K] * B[Ng x K]^T, both operands K-major, 128 x BN output tiles,
-// persistent CTAs, double-buffered TMEM accumulator (the epilogue of tile i overlaps the main loop of tile i+1).
-template <int AFF>
+// persistent CTAs (the TMA loads of tile i+1 run under the epilogue of tile i).
+template <int AFF, int BN>
 __global__ void __launch_bounds__(kTmaThreads, 1)
 conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
@@ -49,42 +50,31 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
                 const __grid_constant__ TmaP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int BN = p.BN;
   int na = p.na;
   if (p.a_hdr) na = (__ldg(&p.a_hdr->nplanes) == 2) ? 2 : 1;
   const int nb = p.nb;
   const uint32_t b_bytes = (uint32_t)BN * 128u;
   const uint32_t stage_bytes = (uint32_t)na * kATileBytes + (uint32_t)nb * b_bytes;
   const uint32_t n_stages = min((uint32_t)kTmaMaxStages, (uint32_t)p.stage_budget / stage_bytes);
-  uint8_t* epi = smem + p.stage_budget;
-  float* stage_all = reinterpret_cast<float*>(epi);
-  long long* rowoff_all = reinterpret_cast<long long*>(stage_all + p.epi_warps * 32 * kStagePitch);
-  float* jrow_all = reinterpret_cast<float*>(rowoff_all + p.epi_warps * 32);
-  float* aff_tab = jrow_all + p.epi_warps * 32;               // AFF == 2: e1[256], e2[256] of the current tile columns
+  float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
+  float* aff_tab = jrow_all + kMmaWarps * 32;               // AFF == 2: e1[256], e2[256] of the current tile columns
   uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : 0));
 
   if (tid == 0) {
     for (int s = 0; s < kTmaMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], p.epi_warps * 32);
+      mbar_init(&empty_bar[s], kMmaWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_s, (uint32_t)(2 * p.acc_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   const int first_tile = blockIdx.x, tile_step = gridDim.x;
 
-  if (warp == 0) {
+  if (warp == kMmaWarps) {
     // =================================== TMA producer (one thread) ===================================
     if (lane == 0) {
       prefetch_map(&tmA0);
@@ -117,46 +107,38 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // =================================== MMA issuer (one thread) ===================================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(TM, BN, 0, 0);
-      uint32_t s = 0, ph = 0, tcount = 0;
-      for (int tile = first_tile; tile < p.total_tiles; tile += tile_step, ++tcount) {
-        const uint32_t buf = tcount & 1u;
-        mbar_wait_bounded(&tempty_bar[buf], ((tcount >> 1) & 1u) ^ 1u);    // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * (uint32_t)p.acc_cols;
-        for (int ks = 0; ks < p.nk; ++ks) {
-          mbar_wait_bounded(&full_bar[s], ph);                             // TMA bytes have landed
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), a1 = a0 + kATileBytes;
-          const uint32_t b0 = a0 + (uint32_t)na * kATileBytes, b1 = b0 + b_bytes;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t da0 = make_smem_desc(a0 + kk * 32, 16, 1024);
-            const uint64_t db0 = make_smem_desc(b0 + kk * 32, 16, 1024);
-            umma_bf16(d_tmem, da0, db0, idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-            if (nb == 2) umma_bf16(d_tmem, da0, make_smem_desc(b1 + kk * 32, 16, 1024), idesc, 1u);
-            if (na == 2) umma_bf16(d_tmem, make_smem_desc(a1 + kk * 32, 16, 1024), db0, idesc, 1u);
-          }
-          umma_commit(&empty_bar[s]);        // frees the stage when these MMAs have completed
-          if (++s == n_stages) { s = 0; ph ^= 1u; }
-        }
-        umma_commit(&tfull_bar[buf]);        // accumulator of this tile complete
-      }
-    }
-  } else if (warp < 2 + p.epi_warps) {
-    // =================================== epilogue (warps 2-9, or 2-5 when shared memory is short) =================
-    const int q = warp & 3;                  // TMEM lane quarter this warp may read
-    const int ew = warp - 2, half = ew >> 2; // two warps per quarter: even / odd 32-column chunks
-    float* stg = stage_all + (size_t)ew * 32 * kStagePitch;
+  } else {
+    // ============================ MMA warpgroups + epilogue (warps 0-7) ============================
+    const int wg = warp >> 2, q = warp & 3;  // MMA rows [64 wg, 64 wg + 64); epilogue rows [32 q, 32 q + 32)
+    const int ew = warp;
     long long* rowoff = rowoff_all + ew * 32;
     float* jrow = jrow_all + ew * 32;
     const float* extra = residual ? residual : (p.accumulate ? out : nullptr);
-    uint32_t tcount = 0;
     int tab_n0 = -1;
-    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step, ++tcount) {
+    uint32_t s = 0, ph = 0;
+    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < p.nk; ++ks) {
+        mbar_wait_bounded(&full_bar[s], ph);                             // TMA bytes have landed
+        const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)wg * 64 * 128, a1 = a0 + kATileBytes;
+        const uint32_t b0 = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)na * kATileBytes, b1 = b0 + b_bytes;
+        wg_mma_stage<BN, 0>(acc, a0, a1, b0, b1, na, nb, 32, 32, 16, 1024, 16, 1024);
+        wgmma_wait<1>(acc);                    // the previous stage's MMAs have completed: release it
+        if (ks > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = s;
+        if (++s == n_stages) { s = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>(acc);
+      if (p.nk > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
       const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
       const int n0 = (tile - mt * p.n_tiles) * BN;
       const int m = mt * TM + q * 32 + lane;
@@ -165,7 +147,7 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         // per-column constants of this tile's columns, once (every epilogue warp walks the same tile sequence, so the
         // named barrier below is reached by all of them; with one n-tile per row of tiles this runs once per CTA):
         //   e1[c] = s_a * alpha_c / k_w ,  e2[c] = s_a * (centre * alpha_c / k_w + beta_c)
-        const int nthr = p.epi_warps * 32;
+        const int nthr = kMmaWarps * 32;
         asm volatile("bar.sync 1, %0;" ::"r"(nthr) : "memory");          // readers of the previous table are done
         const float a_s = p.aff.a_scale ? __ldg(p.aff.a_scale) : 1.f;
         for (int c = ew * 32 + lane; c < BN; c += nthr) {
@@ -205,15 +187,12 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
         }
         my_j = (a0 + a1) + (a2 + a3);
       }
-      epilogue_tile_a<AFF>(tmem_base + (tcount & 1u) * (uint32_t)p.acc_cols, &tfull_bar[tcount & 1u],
-                           &tempty_bar[tcount & 1u], (tcount >> 1) & 1u, false, off, rowoff, stg, out, extra, bias, p.relu,
-                           n0, BN, p.Ng, q, lane, p.ring ? ring_all + (size_t)ew * p.ring * kRingSlotBytes : nullptr,
-                           p.aff, my_j, jrow, 32 * half, 8 * p.epi_warps, AFF == 2 ? aff_tab : nullptr, p.ring);
+      wg_tile_to_smem<BN>(acc, acc_s, tid);
+      epilogue_tile_a<AFF>(acc_s, ew, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
+                           p.ring ? ring_all + (size_t)ew * p.ring * kRingSlotBytes : nullptr, p.aff, my_j, jrow,
+                           AFF == 2 ? aff_tab : nullptr, p.ring);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)(2 * p.acc_cols));
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -224,52 +203,42 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
 // belongs to), dy through a tiled map.
 struct WgTmaP {
   TcGeom g;
-  int Mtot, Npix, pps, splits, BN, n_tiles, tiles, total_units, acc_cols;
-  int na, nb, stage_budget, epi_warps;
+  int Mtot, Npix, pps, splits, BN, n_tiles, tiles, total_units;
+  int na, nb, stage_budget;
   FastDiv d_pq, d_q, d_c, d_s, d_tiles, d_ntiles;
   EpiAff aff;
   const pf_tc_act_hdr* x_hdr;
 };
 constexpr uint32_t kWgBlockBytes = BK * 128;   // one 64 (MN) x 64 (pixels) block
 
-template <int AFF>
+template <int AFF, int BN>
 __global__ void __launch_bounds__(kTmaThreads, 1)
 conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant__ CUtensorMap tmX1,
                       const __grid_constant__ CUtensorMap tmY0, const __grid_constant__ CUtensorMap tmY1,
                       float* __restrict__ partial, const __grid_constant__ WgTmaP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages], tfull_bar[2], tempty_bar[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const TcGeom& g = p.g;
-  const int BN = p.BN, nblkB = BN / 64;
+  const int nblkB = BN / 64;
   int na = p.na;
   if (p.x_hdr) na = (__ldg(&p.x_hdr->nplanes) == 2) ? 2 : 1;
   const int nb = p.nb;
   const uint32_t a_bytes = 2 * kWgBlockBytes, b_bytes = (uint32_t)nblkB * kWgBlockBytes;
   const uint32_t stage_bytes = (uint32_t)na * a_bytes + (uint32_t)nb * b_bytes;
   const uint32_t n_stages = min((uint32_t)kTmaMaxStages, (uint32_t)p.stage_budget / stage_bytes);
-  uint8_t* epi = smem + p.stage_budget;
-  float* stage_all = reinterpret_cast<float*>(epi);
-  long long* rowoff_all = reinterpret_cast<long long*>(stage_all + p.epi_warps * 32 * kStagePitch);
-  float* jrow_all = reinterpret_cast<float*>(rowoff_all + p.epi_warps * 32);
+  float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
   if (tid == 0) {
     for (int s = 0; s < kTmaMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], p.epi_warps * 32);
+      mbar_init(&empty_bar[s], kMmaWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_s, (uint32_t)(2 * p.acc_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   struct Unit {
     int split, m0, n0, pbeg, nk;
   };
@@ -286,7 +255,7 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
     return r;
   };
 
-  if (warp == 0) {
+  if (warp == kMmaWarps) {
     if (lane == 0) {
       prefetch_map(&tmX0);
       prefetch_map(&tmY0);
@@ -332,57 +301,46 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(TM, BN, 1, 1);
-      uint32_t s = 0, ph = 0, tcount = 0;
-      for (int u = blockIdx.x; u < p.total_units; u += gridDim.x, ++tcount) {
-        const Unit un = decode(u);
-        const uint32_t buf = tcount & 1u;
-        mbar_wait_bounded(&tempty_bar[buf], ((tcount >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * (uint32_t)p.acc_cols;
-        for (int ks = 0; ks < un.nk; ++ks) {
-          mbar_wait_bounded(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), a1 = a0 + a_bytes;
-          const uint32_t b0 = a0 + (uint32_t)na * a_bytes, b1 = b0 + b_bytes;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            // MN-major: LBO = stride between 64-wide MN blocks (8 KB), SBO = stride between 8-pixel groups (1 KB);
-            // one MMA consumes 16 pixels = 2 KB
-            const uint64_t da0 = make_smem_desc(a0 + kk * 2048, kWgBlockBytes, 1024);
-            const uint64_t db0 = make_smem_desc(b0 + kk * 2048, kWgBlockBytes, 1024);
-            umma_bf16(d_tmem, da0, db0, idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-            if (nb == 2) umma_bf16(d_tmem, da0, make_smem_desc(b1 + kk * 2048, kWgBlockBytes, 1024), idesc, 1u);
-            if (na == 2) umma_bf16(d_tmem, make_smem_desc(a1 + kk * 2048, kWgBlockBytes, 1024), db0, idesc, 1u);
-          }
-          umma_commit(&empty_bar[s]);
-          if (++s == n_stages) { s = 0; ph ^= 1u; }
-        }
-        if (un.nk > 0) umma_commit(&tfull_bar[buf]);
-        else mbar_arrive(&tfull_bar[buf]);
-      }
-    }
-  } else if (warp < 2 + p.epi_warps) {
-    const int q = warp & 3;
-    const int ew = warp - 2, half = ew >> 2;
-    float* stg = stage_all + (size_t)ew * 32 * kStagePitch;
-    long long* rowoff = rowoff_all + ew * 32;
-    float* jrow = jrow_all + ew * 32;
-    uint32_t tcount = 0;
-    for (int u = blockIdx.x; u < p.total_units; u += gridDim.x, ++tcount) {
+  } else {
+    // MMA warpgroups + epilogue: warpgroup wg multiplies kf rows [64 wg, 64 wg + 64) = MN block wg of the x tile
+    const int wg = warp >> 2, q = warp & 3;
+    long long* rowoff = rowoff_all + warp * 32;
+    float* jrow = jrow_all + warp * 32;
+    uint32_t s = 0, ph = 0;
+    for (int u = blockIdx.x; u < p.total_units; u += gridDim.x) {
       const Unit un = decode(u);
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < un.nk; ++ks) {
+        mbar_wait_bounded(&full_bar[s], ph);
+        const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t a0 = base + (uint32_t)wg * kWgBlockBytes, a1 = a0 + a_bytes;
+        const uint32_t b0 = base + (uint32_t)na * a_bytes, b1 = b0 + b_bytes;
+        // MN-major: LBO = stride between 64-wide MN blocks (8 KB), SBO = stride between 8-pixel groups (1 KB);
+        // one MMA consumes 16 pixels = 2 KB
+        wg_mma_stage<BN, 1>(acc, a0, a1, b0, b1, na, nb, 2048, 2048, kWgBlockBytes, 1024, kWgBlockBytes, 1024);
+        wgmma_wait<1>(acc);
+        if (ks > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = s;
+        if (++s == n_stages) { s = 0; ph ^= 1u; }
+      }
+      wgmma_wait<0>(acc);
+      if (un.nk > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
       const int em = un.m0 + q * 32 + lane;
       const long long off = em < p.Mtot ? ((long long)un.split * p.Mtot + em) * g.K : -1;
-      epilogue_tile_a<AFF>(tmem_base + (tcount & 1u) * (uint32_t)p.acc_cols, &tfull_bar[tcount & 1u],
-                           &tempty_bar[tcount & 1u], (tcount >> 1) & 1u, un.nk == 0, off, rowoff, stg, partial, nullptr,
-                           nullptr, 0, un.n0, BN, g.K, q, lane, nullptr, p.aff, 0.f, jrow, 32 * half, 8 * p.epi_warps);
+      wg_tile_to_smem<BN>(acc, acc_s, tid);
+      epilogue_tile_a<AFF>(acc_s, warp, off, rowoff, partial, nullptr, nullptr, 0, un.n0, BN, g.K, lane, nullptr, p.aff,
+                           0.f, jrow);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)(2 * p.acc_cols));
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -406,24 +364,10 @@ bool conv_tma_eligible(int pass, const TcGeom& g) {
   return g.C % 64 == 0 && g.K % 64 == 0 && g.sh <= 8 && g.sw <= 8;
 }
 
-static int pick_bn(int Ng, int m_tiles, bool has_extra, bool split_planes, int nk) {
-  int BN;
-  if (Ng >= 256 && has_extra && (split_planes || nk >= 2)) {
-    // an epilogue that also streams a residual / accumulate operand: 128-wide tiles leave shared memory for the ring
-    // (and for 8 epilogue warps) that 256-wide stages take away.  Measured on the conv3 + shortcut layers of ResNet-50
-    // (batch 256, ms at BN 256 -> 128): split planes 64->256 0.516 -> 0.319, 128->512 0.267 -> 0.265; levels 128->512
-    // 0.299 -> 0.223, 256->1024 0.176 -> 0.133 — but levels 64->256 (one k-stage per tile) 0.354 -> 0.407: stays 256.
-    BN = 128;
-  } else if (Ng >= 256) {
-    const int64_t t256 = (int64_t)m_tiles * ((Ng + 255) / 256), t128 = (int64_t)m_tiles * ((Ng + 127) / 128);
-    const double c256 = (double)((t256 + PF_NUM_SMS - 1) / PF_NUM_SMS) * 1.3;   // a 256-wide tile costs ~1.3x a 128-wide one
-    const double c128 = (double)((t128 + PF_NUM_SMS - 1) / PF_NUM_SMS);
-    BN = c256 <= c128 ? 256 : 128;
-  } else {
-    BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
-  }
+static int pick_bn(int Ng) {
+  int BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
   const int forced = env_int("PF_TC_BN", 0);
-  if (forced >= 16 && forced <= 256 && forced <= ((Ng + 15) / 16) * 16 && (forced & (forced - 1)) == 0) BN = forced;
+  if (forced >= 16 && forced <= kMaxBN && forced <= ((Ng + 15) / 16) * 16 && (forced & (forced - 1)) == 0) BN = forced;
   return BN;
 }
 
@@ -465,12 +409,10 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   p.accumulate = accumulate;
   p.relu = relu;
   const int m_tiles = (p.M + TM - 1) / TM;
-  const int BN = pick_bn(p.Ng, m_tiles, residual != nullptr || accumulate, a.plane1 != nullptr && a.hdr == nullptr, p.nk);
+  const int BN = pick_bn(p.Ng);
   p.BN = BN;
   p.n_tiles = (p.Ng + BN - 1) / BN;
   p.total_tiles = m_tiles * p.n_tiles;
-  p.acc_cols = 32;
-  while (p.acc_cols < BN) p.acc_cols <<= 1;
   p.d_hw = make_fastdiv((uint32_t)p.rows_hw);
   p.d_w = make_fastdiv((uint32_t)p.rows_w);
   p.d_ntiles = make_fastdiv((uint32_t)p.n_tiles);
@@ -497,38 +439,31 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     aff = 1;
     p.aff.a_scale = &a.hdr->scale;
   }
-  // ---- shared memory: [stages][epilogue staging, row offsets, J][residual ring]; 8 epilogue warps when at least two
-  // (three with a residual ring) stages still fit beside their staging tiles, else 4
+  // ---- shared memory: [stages][accumulator tile, row offsets, J, column constants][residual ring]
   const int stage_max = p.na * (int)kATileBytes + p.nb * BN * 128;
   const bool has_extra = residual != nullptr || accumulate;
   const int aff_tab_bytes = aff == 2 ? 2 * 256 * 4 : 0;       // the tile's per-column epilogue constants
-  auto epi_bytes = [aff_tab_bytes](int warps) {
-    return 1024 + warps * (32 * kStagePitch * 4 + 32 * 8 + 32 * 4) + aff_tab_bytes + 256;
-  };
-  // 8 epilogue warps unless their staging tiles cost a pipeline stage that 4 warps would leave (below 4 stages)
-  const int st8 = (kSmemLimit - epi_bytes(kTmaEpiWarps)) / 1024 * 1024 / stage_max, st4 = (kSmemLimit - epi_bytes(4)) / 1024 * 1024 / stage_max;
-  p.epi_warps = (BN >= 64 && st8 >= 2 && (st8 >= 4 || st8 == st4)) ? kTmaEpiWarps : 4;
-  p.epi_warps = env_int("PF_TC_EPI_WARPS", p.epi_warps) == 4 ? 4 : p.epi_warps;
+  const int epi_bytes = epi_fixed_bytes(BN) + aff_tab_bytes;
   // the residual / accumulate operand streams through a per-warp cp.async ring of 4 (else 2) 4 KB chunks when the
   // pipeline keeps enough stages beside it: 3, or nk + 1 for the short reductions of the 1x1 layers (a 64 -> 256 layer
   // has ONE k-stage per tile: two stages already let the next tile's loads fly during this tile's MMAs)
-  int budget = (kSmemLimit - epi_bytes(p.epi_warps)) / 1024 * 1024;
+  int budget = (kSmemLimit - epi_bytes) / 1024 * 1024;
   int ring_bytes = 0;
   p.ring = 0;
   if (has_extra && env_int("PF_TC_RING", 1) && BN >= 64) {
     const int need = std::min(3, p.nk + 1);
     for (int depth = kRingDepth; depth >= 2 && !p.ring; depth >>= 1) {
-      const int rb = p.epi_warps * depth * kRingSlotBytes;
+      const int rb = kMmaWarps * depth * kRingSlotBytes;
       if ((budget - rb) / stage_max >= need) {
         p.ring = depth;
         ring_bytes = rb;
       }
     }
-    if (p.ring) budget = (kSmemLimit - epi_bytes(p.epi_warps) - ring_bytes) / 1024 * 1024;
+    if (p.ring) budget = (kSmemLimit - epi_bytes - ring_bytes) / 1024 * 1024;
   }
   PF_REQUIRE(budget / stage_max >= 2 || p.nk <= 1, "%s: shared-memory plan failed (BN %d)", who, BN);
   p.stage_budget = budget;
-  const size_t smem = 1024 + (size_t)budget + (epi_bytes(p.epi_warps) - 1024) + (p.ring ? ring_bytes : 0);
+  const size_t smem = (size_t)budget + epi_bytes + (p.ring ? ring_bytes : 0);
   if (p.total_tiles == 0) return PF_OK;
   // ---- tensor maps
   alignas(64) CUtensorMap tA0, tA1, tB0, tB1;
@@ -544,16 +479,14 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   else
     tB1 = tB0;
   const int grid = std::min(p.total_tiles, PF_NUM_SMS);
-#define PF_TMA_LAUNCH(AFFV)                                                                                         \
-  do {                                                                                                              \
-    auto kern = conv_tma_kernel<AFFV>;                                                                              \
-    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                    \
-    kern<<<grid, kTmaThreads, smem, st>>>(tA0, tA1, tB0, tB1, out, bias, residual, p);                              \
-  } while (0)
-  if (aff == 2) PF_TMA_LAUNCH(2);
-  else if (aff == 1) PF_TMA_LAUNCH(1);
-  else PF_TMA_LAUNCH(0);
-#undef PF_TMA_LAUNCH
+  cudaError_t err = cudaSuccess;
+  with_bn(BN, [&](auto bn) {
+    constexpr int B = decltype(bn)::value;
+    auto kern = aff == 2 ? conv_tma_kernel<2, B> : (aff == 1 ? conv_tma_kernel<1, B> : conv_tma_kernel<0, B>);
+    err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) kern<<<grid, kTmaThreads, smem, st>>>(tA0, tA1, tB0, tB1, out, bias, residual, p);
+  });
+  PF_CUDA(err);
   PF_CHECK_LAUNCH(who);
   return PF_OK;
 }
@@ -572,8 +505,6 @@ int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& 
   p.n_tiles = (g.K + BN - 1) / BN;
   p.tiles = m_tiles * p.n_tiles;
   p.total_units = p.tiles * p.splits;
-  p.acc_cols = 32;
-  while (p.acc_cols < BN) p.acc_cols <<= 1;
   p.d_pq = make_fastdiv((uint32_t)(g.P * g.Q));
   p.d_q = make_fastdiv((uint32_t)g.Q);
   p.d_c = make_fastdiv((uint32_t)g.C);
@@ -591,13 +522,10 @@ int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& 
     p.aff.a_scale = &x.hdr->scale;
   }
   const int stage_max = p.na * 2 * (int)kWgBlockBytes + p.nb * (BN / 64) * (int)kWgBlockBytes;
-  auto epi_bytes = [](int warps) { return 1024 + warps * (32 * kStagePitch * 4 + 32 * 8 + 32 * 4) + 256; };
-  const int st8 = (kSmemLimit - epi_bytes(kTmaEpiWarps)) / 1024 * 1024 / stage_max, st4 = (kSmemLimit - epi_bytes(4)) / 1024 * 1024 / stage_max;
-  p.epi_warps = (st8 >= 2 && (st8 >= 4 || st8 == st4)) ? kTmaEpiWarps : 4;
-  const int budget = (kSmemLimit - epi_bytes(p.epi_warps)) / 1024 * 1024;
+  const int budget = (kSmemLimit - epi_fixed_bytes(BN)) / 1024 * 1024;
   PF_REQUIRE(budget / stage_max >= 2, "%s: shared-memory plan failed (BN %d)", who, BN);
   p.stage_budget = budget;
-  const size_t smem = 1024 + (size_t)budget + (epi_bytes(p.epi_warps) - 1024);
+  const size_t smem = (size_t)budget + epi_fixed_bytes(BN);
   if (p.total_units == 0) return PF_OK;
   alignas(64) CUtensorMap tX0, tX1, tY0, tY1;
   PF_TMA_ENCODE(encode_im2col_bf16(&tX0, x.plane0, g.N, g.H, g.W, g.C, -g.pl, -g.pt, g.Q, g.P, g.sw, g.sh, BK, BK), who);
@@ -611,15 +539,10 @@ int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& 
   else
     tY1 = tY0;
   const int grid = std::min(p.total_units, PF_NUM_SMS);
-  if (aff == 1) {
-    auto kern = conv_tma_wgrad_kernel<1>;
-    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kTmaThreads, smem, st>>>(tX0, tX1, tY0, tY1, partial, p);
-  } else {
-    auto kern = conv_tma_wgrad_kernel<0>;
-    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, kTmaThreads, smem, st>>>(tX0, tX1, tY0, tY1, partial, p);
-  }
+  auto kern = BN == 128 ? (aff == 1 ? conv_tma_wgrad_kernel<1, 128> : conv_tma_wgrad_kernel<0, 128>)
+                        : (aff == 1 ? conv_tma_wgrad_kernel<1, 64> : conv_tma_wgrad_kernel<0, 64>);
+  PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<grid, kTmaThreads, smem, st>>>(tX0, tX1, tY0, tY1, partial, p);
   PF_CHECK_LAUNCH(who);
   return PF_OK;
 }

@@ -5,7 +5,7 @@
 // Reference semantics: tf.layers.batch_normalization(momentum .997, eps 1e-5, fused)
 // (/root/reference/utils/external/resnet_model.py:55-62), tf.nn.relu (:144), max_pooling2d 3x3 s2
 // SAME (:521-525), reduce_mean over H,W (:547-548), residual add (:199,:314).
-// B200 design: one pass computes the batch statistics (shifted sums, fp64 combine), one pass applies
+// Design: one pass computes the batch statistics (shifted sums, fp64 combine), one pass applies
 // BN+ReLU AND accumulates the per-tensor min/max the activation quantizer needs
 // (uniform_quantization/utils.py:51-79), so the separate reduce_max/reduce_min passes of the
 // reference disappear.

@@ -1,4 +1,4 @@
-// pf_tma.cuh — Tensor Memory Accelerator plumbing for the tcgen05 convolution kernels (sm_100a):
+// pf_tma.cuh — Tensor Memory Accelerator plumbing for the wgmma convolution kernels (sm_90a):
 //   host : CUtensorMap encoding (tiled 2-D for the weight / gradient matrices, im2col 4-D for NHWC activations)
 //          through the driver entry points fetched with cudaGetDriverEntryPoint (no link against libcuda);
 //   device: cp.async.bulk.tensor wrappers (SASS: UTMALDG), mbarrier transaction counts, a bounded mbarrier wait.

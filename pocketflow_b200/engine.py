@@ -3,7 +3,7 @@ gradient reduction, optimizer) and replays them through a CUDA graph.
 
 This is the stand-in for `sess.run(train_op)` into TensorFlow's executor
 (/root/reference/learners/uniform_quantization/learner.py:114-152): one call = one training step
-on one GPU.  State layout (B200, 180 GB HBM): all trainable parameters, their gradients and the
+on one GPU.  State layout: all trainable parameters, their gradients and the
 optimizer slots live in FLAT fp32 buffers so that (a) the data-parallel gradient reduction is one
 collective over one buffer (SURVEY §8e) and (b) the optimizer / mask / weight-decay work is a
 handful of launches instead of ~110 per step.
@@ -147,7 +147,7 @@ class Executor:
         self.loss, self.teacher = loss, teacher
         self.optimizer = optimizer or {}
         self.exact_ste, self.grad_scale = exact_ste, float(grad_scale)
-        # 'tc': tcgen05 split-bf16 conv where the shape allows (Cin, Cout multiples of 16), exact-fp32
+        # 'tc': tensor-core (wgmma) split-bf16 conv where the shape allows (Cin, Cout multiples of 16), exact-fp32
         # CUDA-core kernels elsewhere; 'fp32': exact-fp32 everywhere (the on-device reference)
         import os as _os
         self.conv_path = conv_path or _os.environ.get('PF_CONV_PATH', 'tc')
@@ -332,8 +332,8 @@ class Executor:
                     # fewer than 64 output channels (MobileNet's 3 -> 32 stem): the tensor-core wgrad wants Cout % 64 == 0,
                     # so g = 64 / Cout pixels share one GEMM row — cols [pixels, kpad] and dy [pixels, k] are read as
                     # [pixels / g, g kpad] and [pixels / g, g k]; the weight gradient is the sum of the g diagonal
-                    # kpad x k blocks of the (g kpad) x (g k) result (the exact-fp32 CUDA-core wgrad of this layer took
-                    # 4.3 of MobileNet's 23 ms: profiles/r2_ncu_launchlist_mobilenet_step_v1.txt)
+                    # kpad x k blocks of the (g kpad) x (g k) result (the exact-fp32 CUDA-core wgrad of this layer is
+                    # slow: one output channel block per CTA over every pixel)
                     pair = None
                     if self.train and not as_planes and k in (16, 32) and (kpad * (64 // k)) % 64 == 0 \
                             and (p * q) % (64 // k) == 0:
@@ -390,7 +390,7 @@ class Executor:
                 self.desc[op] = ops.conv_desc(n, h, w, c, c, kh, kw, p, q, sh, sw, pt, pl)
                 if self.train:
                     self.pool_argmax[op] = torch.empty(y.shape, dtype=torch.uint8, device=dev)
-        # ---- residual Add fused into the epilogue of the tcgen05 conv that produces one of its inputs:
+        # ---- residual Add fused into the epilogue of the tensor-core conv that produces one of its inputs:
         # the conv writes conv(x) + shortcut straight into the Add's buffer (one pass instead of three)
         self.fused_add = {}        # conv op -> (add op, other input tensor)
         self.add_fused = set()
@@ -407,7 +407,7 @@ class Executor:
                     self.buf[x_t] = self.buf[op.output]       # the conv output IS the add output
                     break
         # ---- split-bf16 operand planes (tensor-core path): the BN-apply / activation-quantizer that produces a conv
-        # input writes it directly in the operand format of the tcgen05 kernels (x = hi + lo, two bf16 planes);
+        # input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
         # the fp32 copy is only written when some other consumer needs it
         self.xplanes, self.bn_need_f32 = {}, {}
         max_x = max_dy = 8

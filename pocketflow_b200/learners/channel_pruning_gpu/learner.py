@@ -9,7 +9,7 @@ fine-tuning with masked gradients (:404-443):
     INPUT channels at the `prune_perctl`-th percentile of the group norms, the percentile ramping up to the layer's
     target ratio, lr adapted by the sign of the loss change (:375-383, :476-497); then the mask of the surviving
     channels (:250-260) and a layer-wise Adam fine-tuning of the same regression loss with masked gradients
-    (:385-396, :499-507).  Device side: two forward passes (tcgen05 convs), pf_cpg_diff_l2, ONE conv wgrad,
+    (:385-396, :499-507).  Device side: two forward passes (tensor-core convs), pf_cpg_diff_l2, ONE conv wgrad,
     pf_cpg_group_norms -> exact percentile (pf_select_desc) -> pf_cpg_prox_apply / pf_adam_step.
   * steady state: the masked Momentum step of the weight-sparse learner with input-channel masks (pf_momentum_step).
 Flagged deviations: with several workers the reference adapts lr_pgd from each worker's LOCAL loss (the workers'

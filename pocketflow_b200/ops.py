@@ -648,7 +648,7 @@ def conv2d_tc_supported(d):
 
 
 class TcWeights:
-    """Split-bf16, K-major copies of one conv kernel for the tcgen05 path (fwd and dgrad operands)."""
+    """Split-bf16, K-major copies of one conv kernel for the tensor-core path (fwd and dgrad operands)."""
 
     def __init__(self, d, device, need_dgrad=True):
         L = _lib.load()

@@ -369,7 +369,7 @@ def test_weight_sparse_layerwise_regression_matches_the_oracle(monkeypatch, conv
     assert all(abs(m.mean() - 0.5) < 0.05 for m in masks.values())
     core = lrn.pr_core_ops()
     assert len(core) == len(lrn.maskable_vars) == 11
-    assert any(op in ex.fused_add for op in core) == (conv_path == 'tc')    # residual adds fused into tcgen05 epilogues
+    assert any(op in ex.fused_add for op in core) == (conv_path == 'tc')    # residual adds fused into tensor-core epilogues
     orc = StepOracle(ex.ops, ex.logits_t, lrn.images)
     pool = lrn.iterator_train
     pool.prefill()

@@ -1,8 +1,8 @@
 """pf_preprocess_images (ILSVRC-12 resize / flip / crop / mean subtraction of a packed mini-batch on the device) against
 its numpy statement, bit for bit.
 
-Validated on a B200 in round 2 (profiles/r2_gpu_validate_unverified.txt): kernel == numpy statement bit for bit, and
-the --enbl_device_preprocess path fills the image placeholder with exactly the host pipeline's batches."""
+Checked: kernel == numpy statement bit for bit, and the --enbl_device_preprocess path fills the image placeholder with
+exactly the host pipeline's batches."""
 import io
 import os
 

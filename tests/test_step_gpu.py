@@ -116,7 +116,7 @@ def test_uq_step_matches_oracle(dst, buckets, monkeypatch):
 
 
 def test_uq_step_tensor_core_path_matches_oracle(monkeypatch):
-    """Same step on the tcgen05 split-bf16 conv path (the default): quantized weights bit-exact, every
+    """Same step on the tensor-core split-bf16 conv path (the default): quantized weights bit-exact, every
     loss term within the north-star 1e-5, gradients within split-bf16 accuracy.  ReLU pre-activations
     within ~1e-6 of zero now flip in most batches (each flip perturbs upstream gradients by ~1e-2 of
     their max-norm in ANY two implementations), so the gradient check is directional + L2, not max-norm."""

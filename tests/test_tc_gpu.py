@@ -1,4 +1,4 @@
-"""tcgen05 path: (1) the hardware probe pins the shared-memory / instruction descriptor conventions of
+"""wgmma path: (1) the hardware probe pins the shared-memory / instruction descriptor conventions of
 pf_tc_common.cuh; (2) pf_conv2d_tc_fwd / pf_conv2d_tc_dgrad against a float64 reference and against the
 exact-fp32 CUDA-core kernels.  Tolerance: 2e-5 of the output scale (split-bf16: operands carry 16
 mantissa bits, the dropped lo*lo term is 2^-18 relative) — two orders tighter than TF32 would be."""
@@ -57,7 +57,7 @@ CASES = [
     (1, 7, 7, 512, 512, 3, 3, 1, 1, 1),
     (5, 10, 10, 32, 64, 5, 5, 1, 0, 0),
     (2, 32, 32, 16, 16, 3, 3, 1, 1, 1),
-    # persistent kernel: several tiles per CTA, B-stationary 1x1 layers, 256-wide tiles, ragged channel tiles
+    # persistent kernel: several tiles per CTA, B-stationary 1x1 layers, 128-wide tiles, ragged channel tiles
     (8, 56, 56, 64, 256, 1, 1, 1, 0, 0),
     (8, 56, 56, 256, 64, 1, 1, 1, 0, 0),
     (2, 14, 14, 64, 192, 3, 3, 1, 1, 1),

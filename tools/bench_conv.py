@@ -1,4 +1,4 @@
-"""Per-layer conv timing: tcgen05 path vs exact-fp32 path at ResNet-50 / batch-256 shapes."""
+"""Per-layer conv timing: tensor-core path vs exact-fp32 path at ResNet-50 / batch-256 shapes."""
 import json
 import os
 import sys

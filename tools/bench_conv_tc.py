@@ -1,4 +1,4 @@
-"""Per-layer timing of the tcgen05 conv kernels (fwd / dgrad / wgrad) at ResNet-50 / batch-256 shapes.
+"""Per-layer timing of the tensor-core conv kernels (fwd / dgrad / wgrad) at ResNet-50 / batch-256 shapes.
 usage: python tools/bench_conv_tc.py [tag]   (env PF_TC_IMPL / PF_TC_BN select kernel variants)"""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Sweep descriptor conventions of the tcgen05 probe on a real B200 and print which are correct."""
+"""Sweep descriptor conventions of the wgmma probe on a real H100 and print which are correct."""
 import ctypes
 import os
 import sys
