@@ -388,10 +388,34 @@ int pf_bn_apply_quant_levels(const float* x_dev, int64_t m, int c, const float* 
 int pf_conv2d_tc_set_feed(int mode);
 int pf_conv2d_tc_fwd_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, const float* bias_dev, int relu,
                         const float* residual_dev, float* y_dev, void* stream);
+/* dgrad with a pf_tc_act gradient operand.  The weights must be split-bf16 planes (wd->alpha == NULL): dgrad reduces
+ * over output channels, along which per-channel weight scales vary, so weight levels cannot be corrected by a column
+ * epilogue; they are refused with PF_ERR_INVALID_ARG. */
 int pf_conv2d_tc_dgrad_ex(const pf_conv_desc* d, const pf_tc_act* dy, const pf_tc_wt* wd, int accumulate, float* dx_dev,
                           void* stream);
 int pf_conv2d_tc_wgrad_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_act* dy, float* ws_dev, float* dw_dev,
                           void* stream);
+/* host-side decisions of the most recent tensor-core conv launch (fwd / dgrad / wgrad, either feed), recorded by the
+ * launcher from the values it launches with, so that tests can tell which kernel variant a call exercised.  One
+ * process-wide record, not synchronised: read it from the thread that launched.  Returns PF_ERR_INVALID_ARG when
+ * out is NULL or no launch has been recorded yet. */
+typedef struct pf_tc_plan {
+  int32_t seq;             /* number of launches recorded so far (this one included) */
+  int32_t feed;            /* 1: TMA-fed kernel, 0: cp.async-fed kernel */
+  int32_t pass;            /* 0 fwd, 1 dgrad, 2 wgrad */
+  int32_t classes;         /* dgrad: 1 = strided dgrad by pixel-parity classes */
+  int32_t bn;              /* tile width */
+  int32_t aff;             /* epilogue: 0 plain, 1 activation-level scale, 2 weight levels (scale + rank-1 term) */
+  int32_t na, nb;          /* operand planes as seen by the host (na: upper bound when a device header decides) */
+  int32_t a_fp32;          /* cp.async fwd / dgrad: 1 = the activation is fp32, split by the producers */
+  int32_t ring;            /* depth of the residual / accumulate cp.async ring: 0 = none, 2 or 4 */
+  int32_t b_stationary;    /* cp.async fwd / dgrad: weights loaded once per CTA */
+  int32_t stages;          /* cp.async: pipeline stages; TMA: stage budget in bytes (stages = budget / stage bytes) */
+  int32_t tiles;           /* output tiles (fwd / dgrad) or work units (wgrad: tiles x splits) */
+  int32_t grid;            /* CTAs launched */
+  int32_t splits, pps;     /* wgrad: split-K factor and pixels per split */
+} pf_tc_plan;
+int pf_conv2d_tc_last_plan(pf_tc_plan* out);
 /* hardware probe used by tests/test_tc_gpu.py to pin the descriptor conventions (not a product op) */
 int pf_tc_probe(const void* a_dev, const void* b_dev, float* d_dev, int n, int k, int mode, uint32_t lbo_a,
                 uint32_t sbo_a, uint32_t lbo_b, uint32_t sbo_b, uint32_t kstep_a, uint32_t kstep_b, void* stream);

@@ -26,6 +26,13 @@ int tc_geom(const pf_conv_desc* d, TcGeom* g, const char* who) {
   *g = TcGeom{d->n, d->h, d->w, d->c, d->k, d->r, d->s, d->p, d->q, d->stride_h, d->stride_w, d->pad_t, d->pad_l};
   return PF_OK;
 }
+
+static pf_tc_plan g_last_plan;            // seq == 0: nothing recorded yet
+void record_plan(const pf_tc_plan& p) {
+  const int seq = g_last_plan.seq + 1;
+  g_last_plan = p;
+  g_last_plan.seq = seq;
+}
 }  // namespace pfconv
 
 namespace {
@@ -655,8 +662,10 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
   PF_REQUIRE(p.n_stages >= 2 || max_nk <= 1, "%s: shared-memory plan failed (BN %d)", who, BN);
   if (p.n_stages < 1) p.n_stages = 1;
   const size_t smem = (size_t)p.n_stages * a_stage + (size_t)p.n_bslots * b_slot + fixed + (p.ring ? ring_bytes : 0);
-  if (p.total_tiles == 0) return PF_OK;
   const int grid = std::min(p.total_tiles, PF_NUM_SMS);
+  record_plan(pf_tc_plan{0, 0, MODE == 0 ? 0 : 1, MODE == 2, BN, 0, 2, 2, a_hi == nullptr, p.ring ? kRingDepth : 0,
+                         p.b_stationary, p.n_stages, p.total_tiles, grid, 0, 0});
+  if (p.total_tiles == 0) return PF_OK;
   cudaError_t err = cudaSuccess;
   with_bn(BN, [&](auto bn) {
     if (a_hi) {
@@ -977,6 +986,7 @@ static int tc_wgrad_impl(const pf_conv_desc* d, const pf_tc_act& x, const pf_tc_
     PF_REQUIRE(x.hdr == nullptr && x.plane1 != nullptr, "%s: quantizer-level operands need the TMA kernels (Cin %% 64 == 0)", who);
     const size_t smem = (size_t)p.n_stages * (2 * BK * TM * 2 + 2 * BK * p.BN * 2) + epi_fixed_bytes(p.BN);
     const int grid = std::min(p.total_units, PF_NUM_SMS);
+    record_plan(pf_tc_plan{0, 0, 2, 0, p.BN, 0, 2, 2, 0, 0, 0, p.n_stages, p.total_units, grid, p.splits, p.pps});
     auto kern = p.BN == 128 ? conv_tc_wgrad_persist_kernel<128> : conv_tc_wgrad_persist_kernel<64>;
     PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, kThreadsP, smem, st>>>((const __nv_bfloat16*)x.plane0, (const __nv_bfloat16*)x.plane1,
@@ -1002,6 +1012,13 @@ int pf_conv2d_tc_wgrad_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc
                           void* stream) {
   PF_REQUIRE(x && dy, "pf_conv2d_tc_wgrad_ex: null operand");
   return tc_wgrad_impl(d, *x, *dy, ws_dev, dw_dev, stream, "pf_conv2d_tc_wgrad_ex");
+}
+
+int pf_conv2d_tc_last_plan(pf_tc_plan* out) {
+  PF_REQUIRE(out != nullptr, "pf_conv2d_tc_last_plan: null pointer");
+  PF_REQUIRE(g_last_plan.seq > 0, "pf_conv2d_tc_last_plan: no tensor-core conv launch recorded yet");
+  *out = g_last_plan;
+  return PF_OK;
 }
 
 int pf_conv2d_tc_set_feed(int mode) {
@@ -1038,7 +1055,10 @@ int pf_conv2d_tc_dgrad_ex(const pf_conv_desc* d, const pf_tc_act* dy, const pf_t
                           void* stream) {
   const char* who = "pf_conv2d_tc_dgrad_ex";
   PF_REQUIRE(dy && wd && dy->plane0 && wd->plane0 && dx_dev, "%s: null pointer", who);
-  const bool plain = dy->hdr == nullptr && dy->plane1 != nullptr && wd->alpha == nullptr && wd->plane1 != nullptr;
+  // pass 1 reduces over output channels: per-channel weight scales vary along the reduction, so weight levels have no
+  // column-epilogue form (and the dgrad weight copies are split planes of the quantized values anyway)
+  PF_REQUIRE(wd->alpha == nullptr, "%s: weight levels are not supported in dgrad; pass split-bf16 weight planes", who);
+  const bool plain = dy->hdr == nullptr && dy->plane1 != nullptr && wd->plane1 != nullptr;
   if (plain)
     return tc_dgrad_impl(d, nullptr, dy->plane0, dy->plane1, wd->plane0, wd->plane1, accumulate, dx_dev, stream, who);
   TcGeom g;

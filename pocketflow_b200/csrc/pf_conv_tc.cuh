@@ -267,6 +267,9 @@ inline void with_bn(int BN, F&& f) {
   }
 }
 
+// ---- plan record (pf_conv2d_tc_last_plan): every launcher stores the plan it launches with, just before the launch
+void record_plan(const pf_tc_plan& p);
+
 // ---- TMA-fed kernels (pf_conv_tma.cu)
 void conv_tma_set_feed(int mode);
 bool conv_tma_eligible(int pass, const TcGeom& g);      // pass: 0 fwd, 1 dgrad, 2 wgrad

@@ -464,6 +464,8 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   PF_REQUIRE(budget / stage_max >= 2 || p.nk <= 1, "%s: shared-memory plan failed (BN %d)", who, BN);
   p.stage_budget = budget;
   const size_t smem = (size_t)budget + epi_bytes + (p.ring ? ring_bytes : 0);
+  const int grid = std::min(p.total_tiles, PF_NUM_SMS);
+  record_plan(pf_tc_plan{0, 1, pass, 0, BN, aff, p.na, p.nb, 0, p.ring, 0, budget, p.total_tiles, grid, 0, 0});
   if (p.total_tiles == 0) return PF_OK;
   // ---- tensor maps
   alignas(64) CUtensorMap tA0, tA1, tB0, tB1;
@@ -478,7 +480,6 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     PF_TMA_ENCODE(encode_2d_bf16(&tB1, w.plane1, (uint64_t)Kpad, (uint64_t)p.Ng, (uint64_t)Kpad, BK, (uint32_t)BN), who);
   else
     tB1 = tB0;
-  const int grid = std::min(p.total_tiles, PF_NUM_SMS);
   cudaError_t err = cudaSuccess;
   with_bn(BN, [&](auto bn) {
     constexpr int B = decltype(bn)::value;
@@ -526,6 +527,8 @@ int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& 
   PF_REQUIRE(budget / stage_max >= 2, "%s: shared-memory plan failed (BN %d)", who, BN);
   p.stage_budget = budget;
   const size_t smem = (size_t)budget + epi_fixed_bytes(BN);
+  const int grid = std::min(p.total_units, PF_NUM_SMS);
+  record_plan(pf_tc_plan{0, 1, 2, 0, BN, aff, p.na, p.nb, 0, 0, 0, budget, p.total_units, grid, splits, pps});
   if (p.total_units == 0) return PF_OK;
   alignas(64) CUtensorMap tX0, tX1, tY0, tY1;
   PF_TMA_ENCODE(encode_im2col_bf16(&tX0, x.plane0, g.N, g.H, g.W, g.C, -g.pl, -g.pt, g.Q, g.P, g.sw, g.sh, BK, BK), who);
@@ -538,7 +541,6 @@ int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& 
     PF_TMA_ENCODE(encode_2d_bf16(&tY1, dy.plane1, (uint64_t)g.K, (uint64_t)p.Npix, (uint64_t)g.K, BK, BK), who);
   else
     tY1 = tY0;
-  const int grid = std::min(p.total_units, PF_NUM_SMS);
   auto kern = BN == 128 ? (aff == 1 ? conv_tma_wgrad_kernel<1, 128> : conv_tma_wgrad_kernel<0, 128>)
                         : (aff == 1 ? conv_tma_wgrad_kernel<1, 64> : conv_tma_wgrad_kernel<0, 64>);
   PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -67,6 +67,7 @@ SIGNATURES = {
     'pf_conv2d_tc_fwd_ex': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),
     'pf_conv2d_tc_dgrad_ex': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
     'pf_conv2d_tc_wgrad_ex': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'pf_conv2d_tc_last_plan': (c_i32, [c_vp]),
     'pf_tc_probe': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32] + [ctypes.c_uint32] * 6 + [c_vp]),
     'pf_dwconv_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_dwconv_dgrad': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
@@ -126,6 +127,12 @@ class TcWt(ctypes.Structure):
     """pf_tc_wt: weight operand (split-bf16 planes, or integer levels + the quantizer's bucket scales)."""
     _fields_ = [('plane0', c_vp), ('plane1', c_vp), ('alpha', c_vp), ('beta', c_vp), ('per_channel', c_i32),
                 ('bits', c_i32)]
+
+
+class TcPlan(ctypes.Structure):
+    """pf_tc_plan: host-side decisions of the most recent tensor-core conv launch."""
+    _fields_ = [(n, c_i32) for n in ('seq', 'feed', 'pass_', 'classes', 'bn', 'aff', 'na', 'nb', 'a_fp32', 'ring',
+                                     'b_stationary', 'stages', 'tiles', 'grid', 'splits', 'pps')]
 
 
 _lib = None

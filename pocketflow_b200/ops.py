@@ -858,6 +858,16 @@ def conv2d_tc_wgrad_ex(d, x_act, dy_act, ws, dw):
                                                  _stream()), 'pf_conv2d_tc_wgrad_ex')
 
 
+def conv2d_tc_last_plan():
+    """Host-side plan of the most recent tensor-core conv launch (pf_tc_plan) as a dict: which feed, pass and kernel
+    variant ran, and with what tile width, ring depth, stages, grid and split-K."""
+    plan = _lib.TcPlan()
+    _lib.check(_lib.load().pf_conv2d_tc_last_plan(ctypes.byref(plan)), 'pf_conv2d_tc_last_plan')
+    out = {n: int(getattr(plan, n)) for n, _ in _lib.TcPlan._fields_}
+    out['pass'] = out.pop('pass_')
+    return out
+
+
 def s2d_planes(x, pad_t, pad_l, hp, wp, cpad, planes):
     """space-to-depth of a stride-2 first layer's input [n,h,w,c] into operand planes [n,hp,wp,cpad]"""
     n, h, w, c = x.shape

@@ -124,7 +124,12 @@ def test_weight_level_preparation_matches_oracle_quantizer(shape, bits, per_chan
 
 
 CASES = [(2, 9, 7, 64, 64, 3, 3, 1, 1, 1), (2, 12, 12, 128, 128, 3, 3, 2, 0, 1), (2, 14, 14, 256, 512, 1, 1, 2, 0, 0),
-         (2, 7, 7, 512, 2048, 1, 1, 1, 0, 0), (2, 56, 56, 64, 64, 3, 3, 1, 1, 1), (2, 14, 14, 64, 192, 3, 3, 1, 1, 1)]
+         (2, 7, 7, 512, 2048, 1, 1, 1, 0, 0), (2, 56, 56, 64, 64, 3, 3, 1, 1, 1), (2, 14, 14, 64, 192, 3, 3, 1, 1, 1),
+         # 3x3 over 2 and 4 channel segments of the window sum J (nseg = C / 128), stride 1 and 2
+         (2, 14, 14, 256, 256, 3, 3, 1, 1, 1), (2, 13, 13, 512, 512, 3, 3, 2, 1, 1), (2, 14, 14, 512, 128, 3, 3, 2, 0, 1),
+         # 123 x 5 = 615 tiles: every CTA of a 132-SM H100 walks 4-5 tiles, and as 5 does not divide 132 its n0 (and
+         # the per-CTA column table of the epilogue) changes from one tile to the next
+         (20, 28, 28, 128, 640, 1, 1, 1, 0, 0)]
 
 
 def _ref_conv(x, wt, case):
@@ -133,9 +138,33 @@ def _ref_conv(x, wt, case):
                     stride=st).permute(0, 2, 3, 1)
 
 
+def weight_scales(nb, wrange, g):
+    """per-bucket alpha, beta of the weight quantizer.  'sym': a range around zero; 'pos': all weights >= 0; 'offset': a
+    range far from zero, where the rank-1 term o_c * J is most of the result and the level product a small correction"""
+    alpha = torch.rand(nb, generator=g) * 0.5 + 0.05
+    if wrange == 'sym':
+        beta = -alpha * (0.3 + 0.4 * torch.rand(nb, generator=g))
+    elif wrange == 'pos':
+        beta = alpha * 0.2 * torch.rand(nb, generator=g)
+    else:
+        beta = alpha * (20.0 + 10.0 * torch.rand(nb, generator=g))
+    return alpha, beta
+
+
 @pytest.mark.parametrize('case', CASES)
 @pytest.mark.parametrize('bits,per_channel', [(8, True), (4, False)])
 def test_level_operand_kernels_match_float64(case, bits, per_channel):
+    check_level_operand_kernels(case, bits, per_channel, 'sym')
+
+
+@pytest.mark.parametrize('case', CASES)
+@pytest.mark.parametrize('bits,per_channel,wrange', [(8, True, 'pos'), (8, False, 'offset')])
+def test_level_operand_kernels_with_offset_weight_ranges(case, bits, per_channel, wrange):
+    """all-positive weights, and a range far from zero where the rank-1 term o_c * J dominates the result"""
+    check_level_operand_kernels(case, bits, per_channel, wrange)
+
+
+def check_level_operand_kernels(case, bits, per_channel, wrange):
     n, h, w, c, k, r, s, st, p0, p1 = case
     p, q = (h + p0 + p1 - r) // st + 1, (w + p0 + p1 - s) // st + 1
     d = ops.conv_desc(n, h, w, c, k, r, s, p, q, st, st, p0, p0)
@@ -146,8 +175,7 @@ def test_level_operand_kernels_match_float64(case, bits, per_channel):
     s_a = 0.0173
     lv = torch.randint(0, kq + 1, (r, s, c, k), generator=g).float()
     nb = k if per_channel else 1
-    alpha = torch.rand(nb, generator=g) * 0.5 + 0.05
-    beta = -alpha * (0.3 + 0.4 * torch.rand(nb, generator=g))
+    alpha, beta = weight_scales(nb, wrange, g)
     rk = float(np.float32(1.0) / np.float32(kq))
     qw = (alpha.double() * rk) * lv.double() + beta.double()
     qa = j.double() * s_a
@@ -172,8 +200,10 @@ def test_level_operand_kernels_match_float64(case, bits, per_channel):
     wt = torch.randn(r, s, c, k, generator=g) * (2.0 / (r * s * c)) ** 0.5
     tw = ops.TcWeights(d, DEV)
     tw.prepare(wt.to(DEV).contiguous())
-    ref2 = _ref_conv(qa, wt, case)
-    ops.conv2d_tc_fwd_ex(d, act, ops.tc_wt(tw.f_hi, tw.f_lo), None, False, Y)
+    wv = (tw.f_hi.double() + tw.f_lo.double()).cpu().view(k, -1)[:, :r * s * c].reshape(k, r, s, c).permute(1, 2, 3, 0)
+    ref2 = torch.relu(_ref_conv(qa, wv, case) + bias.double()) + res.double()
+    Y.fill_(float('nan'))
+    ops.conv2d_tc_fwd_ex(d, act, ops.tc_wt(tw.f_hi, tw.f_lo), bias.to(DEV), True, Y, res.to(DEV))
     torch.cuda.synchronize()
     assert (Y.double().cpu() - ref2).abs().max().item() <= 2e-5 * ref2.abs().max().item()
     dy = torch.randn(n, p, q, k, generator=g)
@@ -186,6 +216,63 @@ def test_level_operand_kernels_match_float64(case, bits, per_channel):
     DW = torch.full((r, s, c, k), 5.0, device=DEV)
     ops.conv2d_tc_wgrad_ex(d, act, ops.tc_act(dyp), ws, DW)
     torch.cuda.synchronize()
+    assert (DW.double().cpu() - refw).abs().max().item() <= 2e-5 * refw.abs().max().item()
+
+
+W8A32_CASES = [(2, 9, 7, 64, 64, 3, 3, 1, 1, 1), (2, 14, 14, 256, 256, 3, 3, 1, 1, 1), (2, 13, 13, 512, 512, 3, 3, 2, 1, 1),
+               (20, 28, 28, 128, 640, 1, 1, 1, 0, 0)]
+
+
+@pytest.mark.parametrize('case', W8A32_CASES)
+@pytest.mark.parametrize('wrange', ['sym', 'offset'])
+def test_w8a32_operands_match_float64(case, wrange):
+    """W8A32: the activation is not quantized, so pf_bn_apply_quant_levels writes split planes, a header that says
+    2 planes (scale 1) and the fp32 channel sums; the weights are levels.  The kernel learns na = 2 from the device
+    header; the rank-1 correction uses the producer's own channel sums."""
+    n, h, w, c, k, r, s, st, p0, p1 = case
+    p, q = (h + p0 + p1 - r) // st + 1, (w + p0 + p1 - s) // st + 1
+    d = ops.conv_desc(n, h, w, c, k, r, s, p, q, st, st, p0, p0)
+    m = n * h * w
+    x, mean, rstd, gamma, beta_bn = bn_setup(m, c, sum(case), 1)
+    y = torch.empty_like(x)
+    slot = torch.zeros(2, dtype=torch.int32, device=DEV)
+    ops.act_range_reset(slot)
+    ops.bn_apply(x, m, c, mean, rstd, gamma, beta_bn, 1, y, slot)
+    apl = ops.Planes(x.numel(), DEV)
+    hdr = torch.zeros(2, dtype=torch.int32, device=DEV)
+    nseg = (c + 127) // 128
+    csum = torch.full((m * nseg,), float('nan'), device=DEV)
+    ops.bn_apply_quant_levels(x, m, c, mean, rstd, gamma, beta_bn, 1, slot, 32, None, apl, hdr, csum)
+    torch.cuda.synchronize()
+    assert int(hdr.cpu().numpy().view(ops.ACT_HDR)[0]['nplanes']) == 2
+    xa = (apl.hi.double() + apl.lo.double()).cpu().view(n, h, w, c)
+    act = ops.tc_act(apl, hdr, csum, nseg)
+    g = torch.Generator().manual_seed(sum(case) + 5)
+    lv = torch.randint(0, 256, (r, s, c, k), generator=g).float()
+    alpha, beta = weight_scales(k, wrange, g)
+    qw = (alpha.double() * float(np.float32(1.0) / np.float32(255.0))) * lv.double() + beta.double()
+    wl = (lv - 128.0).permute(3, 0, 1, 2).reshape(k, r * s * c).to(torch.bfloat16).contiguous().to(DEV)
+    bias, res = torch.randn(k, generator=g), torch.randn(n, p, q, k, generator=g)
+    ref = torch.relu(_ref_conv(xa, qw, case) + bias.double()) + res.double()
+    A, B = alpha.to(DEV), beta.to(DEV)             # tc_wt holds raw pointers: keep the tensors alive
+    Y = torch.full((n, p, q, k), float('nan'), device=DEV)
+    ops.conv2d_tc_fwd_ex(d, act, ops.tc_wt(wl, None, A, B, True, 8), bias.to(DEV), True, Y, res.to(DEV))
+    torch.cuda.synchronize()
+    plan = ops.conv2d_tc_last_plan()
+    assert plan['feed'] == 1 and plan['aff'] == 2 and plan['na'] == 2 and plan['nb'] == 1, plan
+    assert (Y.double().cpu() - ref).abs().max().item() <= 2e-5 * ref.abs().max().item()
+    # weight gradient: x (split, under the 2-plane header) (x) split dy
+    dy = torch.randn(n, p, q, k, generator=g)
+    wd = torch.zeros(k, c, r, s, dtype=torch.float64, requires_grad=True)
+    F.conv2d(F.pad(xa.permute(0, 3, 1, 2), (p0, p1, p0, p1)), wd, stride=st).backward(dy.double().permute(0, 3, 1, 2))
+    refw = wd.grad.permute(2, 3, 1, 0)
+    dyp = ops.Planes(dy.numel(), DEV)
+    ops.split_bf16(dy.to(DEV), dyp)
+    ws = torch.empty(max(ops.conv2d_tc_wgrad_planes_workspace_floats(d), 4), device=DEV)
+    DW = torch.full((r, s, c, k), float('nan'), device=DEV)
+    ops.conv2d_tc_wgrad_ex(d, act, ops.tc_act(dyp), ws, DW)
+    torch.cuda.synchronize()
+    assert ops.conv2d_tc_last_plan()['aff'] == 1
     assert (DW.double().cpu() - refw).abs().max().item() <= 2e-5 * refw.abs().max().item()
 
 

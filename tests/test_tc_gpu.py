@@ -107,7 +107,9 @@ def test_conv_tc_fwd_dgrad(case):
     assert err <= 2e-5, 'dgrad err %.3e' % err
     ops.conv2d_tc_dgrad(d, DY, tw, True, DX)
     assert (DX.cpu().double() - 2 * dx_ref).abs().max().item() <= 4e-5 * dx_ref.abs().max().item()
-    # pre-split operand planes: the same kernels fed by cp.async instead of convert-on-the-fly -> identical bits
+    # pre-split operand planes: identical bits to convert-on-the-fly.  The planes call runs the TMA-fed kernel where
+    # the gathered channel count is a multiple of 64 and the cp.async planes kernel otherwise; both add the same products
+    # in the same order (tests/test_tc_variants_gpu.py checks the feeds against each other at every tile width)
     xp, dyp = ops.Planes(X.numel(), torch.device(DEV)), ops.Planes(DY.numel(), torch.device(DEV))
     ops.split_bf16(X, xp)
     ops.split_bf16(DY, dyp)
