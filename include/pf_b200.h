@@ -433,6 +433,26 @@ int pf_dwconv_dgrad(const pf_conv_desc* d, const float* dy_dev, const float* w_d
 int64_t pf_dwconv_wgrad_workspace_bytes(const pf_conv_desc* d);
 int pf_dwconv_wgrad(const pf_conv_desc* d, const float* x_dev, const float* dy_dev, float* ws_dev, float* dw_dev,
                     void* stream);
+/* which kernel the most recent pf_dwconv_fwd / _dgrad / _wgrad call launched (one of the PF_DW_* below; 0 before the
+ * first launch), chosen on the host from the shape and PF_DW_ROWS, so that tests can tell which dispatch target a call
+ * exercised.  One process-wide record, not synchronised: read it from the thread that launched. */
+enum {
+  PF_DW_FWD_ROWS = 1,        /* 3x3 stride 1, 4 output rows per thread */
+  PF_DW_FWD_3X3_S1,
+  PF_DW_FWD_3X3_S2,
+  PF_DW_FWD_GENERIC,
+  PF_DW_DGRAD_ROWS,
+  PF_DW_DGRAD_3X3_S1,
+  PF_DW_DGRAD_BLOCK_P0,      /* 3x3 stride 2, 2 x 2 input pixels per thread, pad 0 */
+  PF_DW_DGRAD_BLOCK_P1,      /* the same, pad 1 */
+  PF_DW_DGRAD_3X3_S2,
+  PF_DW_DGRAD_GENERIC,
+  PF_DW_WGRAD_ROWS,
+  PF_DW_WGRAD_3X3_S1,
+  PF_DW_WGRAD_3X3_S2,
+  PF_DW_WGRAD_GENERIC
+};
+int pf_dwconv_last_variant(void);
 
 /* ---------------------------------------------------------------------------------------------
  * a13 The HBM-bound layers between the convolutions (pf_nn.cu); tensors viewed as [m, c], c % 4 == 0.

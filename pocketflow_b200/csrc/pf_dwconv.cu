@@ -544,14 +544,12 @@ dw3x3s2_dgrad_block_kernel(const float* __restrict__ dy, const float* __restrict
   }
 }
 
-inline bool dw_rows_enabled() {           // PF_DW_ROWS=0: the one-output-per-thread kernels everywhere
-  static int on = -1;
-  if (on < 0) {
-    const char* v = getenv("PF_DW_ROWS");
-    on = !(v && v[0] == '0');
-  }
-  return on == 1;
+inline bool dw_rows_enabled() {           // PF_DW_ROWS=0: the one-output-per-thread kernels everywhere (read per launch)
+  const char* v = getenv("PF_DW_ROWS");
+  return !(v && v[0] == '0');
 }
+
+int g_last_variant = 0;                   // pf_dwconv_last_variant: PF_DW_* of the most recent launch, 0 = none yet
 inline bool dw_rows(const DwGeom& g) {   // the row-blocked stride-1 kernels
   return dw_rows_enabled() && g.sh == 1 && g.sw == 1 && g.P >= kRB && g.H >= kRB;
 }
@@ -601,12 +599,20 @@ int pf_dwconv_fwd(const pf_conv_desc* d, const float* x_dev, const float* w_dev,
   if (rc) return rc;
   PF_REQUIRE(x_dev && w_dev && y_dev, "pf_dwconv_fwd: null pointer");
   const unsigned grid = dw_grid((int64_t)g.N * g.P * g.Q * (g.C >> 2));
-  if (dw_is3x3(g) && dw_rows(g))
+  if (dw_is3x3(g) && dw_rows(g)) {
+    g_last_variant = PF_DW_FWD_ROWS;
     dw3x3s1_fwd_rows_kernel<<<dw_grid((int64_t)g.N * ((g.P + kRB - 1) / kRB) * g.Q * (g.C >> 2)), NT, 0, (cudaStream_t)stream>>>(
         x_dev, w_dev, g, y_dev);
-  else if (dw_is3x3(g) && g.sh == 1) dw3x3_fwd_kernel<1><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
-  else if (dw_is3x3(g)) dw3x3_fwd_kernel<2><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
-  else dw_fwd_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
+  } else if (dw_is3x3(g) && g.sh == 1) {
+    g_last_variant = PF_DW_FWD_3X3_S1;
+    dw3x3_fwd_kernel<1><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
+  } else if (dw_is3x3(g)) {
+    g_last_variant = PF_DW_FWD_3X3_S2;
+    dw3x3_fwd_kernel<2><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
+  } else {
+    g_last_variant = PF_DW_FWD_GENERIC;
+    dw_fwd_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, w_dev, g, y_dev);
+  }
   PF_CHECK_LAUNCH("pf_dwconv_fwd");
   return PF_OK;
 }
@@ -618,16 +624,25 @@ int pf_dwconv_dgrad(const pf_conv_desc* d, const float* dy_dev, const float* w_d
   if (rc) return rc;
   PF_REQUIRE(dy_dev && w_dev && dx_dev, "pf_dwconv_dgrad: null pointer");
   const unsigned grid = dw_grid((int64_t)g.N * g.H * g.W * (g.C >> 2));
-  if (dw_is3x3(g) && dw_rows(g))
+  if (dw_is3x3(g) && dw_rows(g)) {
+    g_last_variant = PF_DW_DGRAD_ROWS;
     dw3x3s1_dgrad_rows_kernel<<<dw_grid((int64_t)g.N * ((g.H + kRB - 1) / kRB) * g.W * (g.C >> 2)), NT, 0, (cudaStream_t)stream>>>(
         dy_dev, w_dev, g, accumulate, dx_dev);
-  else if (dw_is3x3(g) && g.sh == 1) dw3x3_dgrad_kernel<1><<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
-  else if (dw_is3x3(g) && g.pt == g.pl && g.pt <= 1 && dw_rows_enabled()) {
+  } else if (dw_is3x3(g) && g.sh == 1) {
+    g_last_variant = PF_DW_DGRAD_3X3_S1;
+    dw3x3_dgrad_kernel<1><<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
+  } else if (dw_is3x3(g) && g.pt == g.pl && g.pt <= 1 && dw_rows_enabled()) {
     const unsigned gb = dw_grid((int64_t)g.N * ((g.H + 1) / 2) * ((g.W + 1) / 2) * (g.C >> 2));
+    g_last_variant = g.pt == 0 ? PF_DW_DGRAD_BLOCK_P0 : PF_DW_DGRAD_BLOCK_P1;
     if (g.pt == 0) dw3x3s2_dgrad_block_kernel<0><<<gb, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
     else dw3x3s2_dgrad_block_kernel<1><<<gb, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
-  } else if (dw_is3x3(g)) dw3x3_dgrad_kernel<2><<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
-  else dw_dgrad_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
+  } else if (dw_is3x3(g)) {
+    g_last_variant = PF_DW_DGRAD_3X3_S2;
+    dw3x3_dgrad_kernel<2><<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
+  } else {
+    g_last_variant = PF_DW_DGRAD_GENERIC;
+    dw_dgrad_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(dy_dev, w_dev, g, accumulate, dx_dev);
+  }
   PF_CHECK_LAUNCH("pf_dwconv_dgrad");
   return PF_OK;
 }
@@ -654,15 +669,25 @@ int pf_dwconv_wgrad(const pf_conv_desc* d, const float* x_dev, const float* dy_d
     // same number of splits, over (image, row block, column) items instead of pixels
     const int nitems = g.N * ((g.P + kRB - 1) / kRB) * g.Q;
     const int ips = (nitems + splits - 1) / splits;
+    g_last_variant = PF_DW_WGRAD_ROWS;
     dw3x3s1_wgrad_rows_kernel<<<grid, NT, 0, st>>>(x_dev, dy_dev, g, ips, ws_dev);
-  } else if (dw_is3x3(g) && g.sh == 1) dw3x3_wgrad_partial_kernel<1><<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
-  else if (dw_is3x3(g)) dw3x3_wgrad_partial_kernel<2><<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
-  else dw_wgrad_partial_kernel<<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
+  } else if (dw_is3x3(g) && g.sh == 1) {
+    g_last_variant = PF_DW_WGRAD_3X3_S1;
+    dw3x3_wgrad_partial_kernel<1><<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
+  } else if (dw_is3x3(g)) {
+    g_last_variant = PF_DW_WGRAD_3X3_S2;
+    dw3x3_wgrad_partial_kernel<2><<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
+  } else {
+    g_last_variant = PF_DW_WGRAD_GENERIC;
+    dw_wgrad_partial_kernel<<<grid, NT, 0, st>>>(x_dev, dy_dev, g, pps, ws_dev);
+  }
   PF_CHECK_LAUNCH("pf_dwconv_wgrad/partial");
   const int n = g.R * g.S * g.C;
   dw_wgrad_final_kernel<<<(n + NT - 1) / NT, NT, 0, st>>>(ws_dev, n, splits, dw_dev);
   PF_CHECK_LAUNCH("pf_dwconv_wgrad/final");
   return PF_OK;
 }
+
+int pf_dwconv_last_variant(void) { return g_last_variant; }
 
 }  // extern "C"

@@ -812,12 +812,9 @@ softmax_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, in
 }
 
 // grid whose stride (gridDim*NT float4s) is a multiple of C/4, so that threads keep their channels
-inline int bn_grid_cap() {
-  static const int cap = [] {
-    const char* v = getenv("PF_BN_GRIDCAP");
-    return (v && *v) ? atoi(v) : 8;
-  }();
-  return cap;
+inline int bn_grid_cap() {                // PF_BN_GRIDCAP, read per launch
+  const char* v = getenv("PF_BN_GRIDCAP");
+  return (v && *v) ? atoi(v) : 8;
 }
 inline unsigned chan_grid(int64_t nvec, int C) {
   int64_t want = (nvec + NT - 1) / NT;

@@ -919,6 +919,18 @@ def dwconv_wgrad(d, x, dy, ws, dw):
                'pf_dwconv_wgrad')
 
 
+# pf_dwconv_last_variant codes (include/pf_b200.h: PF_DW_*), 1-based
+DW_VARIANTS = ('fwd rows', 'fwd 3x3 s1', 'fwd 3x3 s2', 'fwd generic',
+               'dgrad rows', 'dgrad 3x3 s1', 'dgrad block p0', 'dgrad block p1', 'dgrad 3x3 s2', 'dgrad generic',
+               'wgrad rows', 'wgrad 3x3 s1', 'wgrad 3x3 s2', 'wgrad generic')
+
+
+def dwconv_last_variant():
+    """Name of the kernel the most recent depthwise launch ran (DW_VARIANTS), None before the first one."""
+    v = int(_lib.load().pf_dwconv_last_variant())
+    return DW_VARIANTS[v - 1] if v else None
+
+
 def preprocess_images(crops_u8, desc, out, mean=(123.68, 116.78, 103.94)):
     """ILSVRC-12 preprocessing of a packed mini-batch on the device (pf_preprocess_images): crops_u8 = uint8 CUDA buffer
     holding every decoded crop back to back, desc = uint8 CUDA view of n pf_img_desc records

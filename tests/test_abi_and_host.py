@@ -34,6 +34,15 @@ def test_library_exports_every_declared_symbol():
     assert L.pf_abi_version() == 1
 
 
+def test_depthwise_variant_names_follow_the_header_enum():
+    src = open(os.path.join(ROOT, 'include', 'pf_b200.h')).read()
+    names = re.findall(r'\b(PF_DW_[A-Z0-9_]+)\s*[,=\s]', src[src.index('enum {\n  PF_DW_'):])
+    names = names[:names.index('PF_DW_WGRAD_GENERIC') + 1]
+    want = ['PF_DW_' + v.upper().replace(' ', '_') for v in ops.DW_VARIANTS]
+    assert names == want, (names, want)
+    assert ops.dwconv_last_variant() is None or ops.dwconv_last_variant() in ops.DW_VARIANTS
+
+
 def test_missing_library_fails_loudly(monkeypatch):
     monkeypatch.setattr(lib, '_lib', None)
     monkeypatch.setattr(lib, 'LIB_PATH', '/nonexistent/libpf_b200.so')

@@ -106,8 +106,9 @@ class Recorder:
     NAMES = ('conv2d_tc_fwd', 'conv2d_tc_fwd_planes', 'conv2d_tc_fwd_ex', 'conv2d_tc_dgrad', 'conv2d_tc_dgrad_planes',
              'conv2d_tc_dgrad_ex', 'conv2d_tc_wgrad', 'conv2d_tc_wgrad_planes', 'conv2d_tc_wgrad_ex')
 
-    def __init__(self, monkeypatch):
+    def __init__(self, monkeypatch, min_calls):
         self.plans, self.checked, self.worst, self.calls, self.max_tiles = {}, set(), {}, 0, 0
+        self.min_calls = min_calls
         self.over = []                 # checks above the DESIGN §6 bar: (key, error, error of an fp32 GEMM)
         orig_act, orig_wt = ops.tc_act, ops.tc_wt
 
@@ -252,15 +253,37 @@ class Recorder:
             got = dw.reshape(-1)[:ref.numel()].view(ref.shape)
         return ref, got, False
 
+    def finish(self, label, secs, peak_gb):
+        print('%s: %d tensor-core calls, %d checked against float64; worst errors %s; %d distinct plans, '
+              'at most %d tiles in one launch; %.0f s, peak %.1f GB' % (
+                  label, self.calls, len(self.checked), {k: '%.2e' % v for k, v in sorted(self.worst.items())},
+                  len(self.plans), self.max_tiles, secs, peak_gb))
+        for key, err, err32, errm in self.over:
+            print('  above the bar: %s %s: %.2e of max|ref| (an fp32 GEMM of the same operands: %.2e); %.2e of max '
+                  'sum of |terms|' % (key[0], key[1:], err, err32, errm))
+        # DESIGN.md §6 bars hold for every forward and dgrad call.  The weight gradients reduce over every pixel of the
+        # batch (6272 at ResNet-50's last stage, batch 128) of BN-backward gradients, which are zero-mean per channel:
+        # the sum cancels, and the tensor-core accumulation then loses more than an fp32 GEMM does (DESIGN.md §4).
+        # There the bar is 2e-5 of the largest sum of |terms|, which does not depend on the cancellation.
+        bad = [(k, e, m) for k, e, _, m in self.over if not (k[0].startswith('conv2d_tc_wgrad') and m <= 2e-5)]
+        assert not bad, bad
+        assert self.calls >= self.min_calls and len(self.checked) >= 3
+        assert self.max_tiles >= 3 * torch.cuda.get_device_properties(0).multi_processor_count
+        outside = {k: v for k, v in self.plans.items() if k not in REQUIRED}
+        assert not outside, 'plans the variant sweep does not reach: %s' % {
+            str(dict(zip(KEY_FIELDS, k))): v for k, v in outside.items()}
 
-def run_workload(workload, batch, monkeypatch, min_calls):
+
+def run_workload(workload, batch, monkeypatch, recorder):
+    """One eager step of a bench workload at `batch` under PF_POISON=1, with recorder(monkeypatch) wrapping entry
+    points of `ops` from just before the step; then recorder.finish(label, seconds, peak GB) prints and asserts."""
     import bench
     monkeypatch.setenv('PF_POISON', '1')
     t0 = time.time()
     torch.cuda.reset_peak_memory_stats()
     lrn = bench.build_learner(workload, 1, batch)
     ex = lrn.sess_train
-    rec = Recorder(monkeypatch)
+    rec = recorder(monkeypatch)
     images, labels = lrn.iterator_train.next_batch()
     ex.buf[lrn.images].copy_(images)
     ex.buf[lrn.labels].copy_(labels)
@@ -268,34 +291,17 @@ def run_workload(workload, batch, monkeypatch, min_calls):
     torch.cuda.synchronize()
     losses = ex.fetch_losses()
     assert np.isfinite(losses['loss']), losses
-    print('%s at batch %d: %d tensor-core calls, %d checked against float64; worst errors %s; %d distinct plans, '
-          'at most %d tiles in one launch; %.0f s, peak %.1f GB' % (
-              workload, batch, rec.calls, len(rec.checked), {k: '%.2e' % v for k, v in sorted(rec.worst.items())},
-              len(rec.plans), rec.max_tiles, time.time() - t0, torch.cuda.max_memory_allocated() / 2 ** 30))
-    for key, err, err32, errm in rec.over:
-        print('  above the bar: %s %s: %.2e of max|ref| (an fp32 GEMM of the same operands: %.2e); %.2e of max sum of '
-              '|terms|' % (key[0], key[1:], err, err32, errm))
-    # DESIGN.md §6 bars hold for every forward and dgrad call.  The weight gradients reduce over every pixel of the
-    # batch (6272 at ResNet-50's last stage, batch 128) of BN-backward gradients, which are zero-mean per channel: the
-    # sum cancels, and the tensor-core accumulation then loses more than an fp32 GEMM does (DESIGN.md §4).  There the
-    # bar is 2e-5 of the largest sum of |terms|, which does not depend on the cancellation.
-    bad = [(k, e, m) for k, e, _, m in rec.over if not (k[0].startswith('conv2d_tc_wgrad') and m <= 2e-5)]
-    assert not bad, bad
-    assert rec.calls >= min_calls and len(rec.checked) >= 3
-    assert rec.max_tiles >= 3 * torch.cuda.get_device_properties(0).multi_processor_count
-    outside = {k: v for k, v in rec.plans.items() if k not in REQUIRED}
-    assert not outside, 'plans the variant sweep does not reach: %s' % {
-        str(dict(zip(KEY_FIELDS, k))): v for k, v in outside.items()}
-    plans = dict(rec.plans)
-    del lrn, ex, rec
-    gc.collect()
-    torch.cuda.empty_cache()
-    return plans
+    try:
+        rec.finish('%s at batch %d' % (workload, batch), time.time() - t0, torch.cuda.max_memory_allocated() / 2 ** 30)
+    finally:
+        del lrn, ex, rec
+        gc.collect()
+        torch.cuda.empty_cache()
 
 
 def test_resnet50_uq8_bench_layers_at_batch_128(monkeypatch):
-    run_workload('resnet50_uq8_dst_b128', 128, monkeypatch, 100)
+    run_workload('resnet50_uq8_dst_b128', 128, monkeypatch, lambda mp: Recorder(mp, 100))
 
 
 def test_mobilenet_cpg50_bench_layers_at_batch_256(monkeypatch):
-    run_workload('mobilenet_cpg50_b256', 256, monkeypatch, 30)
+    run_workload('mobilenet_cpg50_b256', 256, monkeypatch, lambda mp: Recorder(mp, 30))
