@@ -564,6 +564,38 @@ int pf_cpg_channel_mask(const float* norms_dev, int rs, int cin, int cout, float
 int pf_mul(const float* a_dev, const float* b_dev, int64_t n, float* out_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * f5  Channel selection of the remastered channel-pruning learner (pf_cpr.cu).
+ *     Replaces the numpy float64 / small-TF-graph work of ChannelPrunedRmtLearner.__choose_channels
+ *     (learners/channel_pruning_rmt/learner.py:546-842); kernels W are [R,S,Cin,Cout] row-major, rs = R*S,
+ *     K = rs*Cin; patch rows are HWIO-ordered, so X * reshape(W, [K, Cout]) is the conv:
+ *   pf_cpr_sample   rows_dev int32 [n_rows, 4] = (n, oh, ow, dst) (16-byte aligned; dst < 0: skip the row):
+ *                   X[dst, (r*S+s)*Cin + c] = x[n, oh*sh - pad_t + r, ow*sw - pad_l + s, c] (0 outside the image),
+ *                   Y[dst, k] = y[n, oh, ow, k] - bias[k]   (:679-703; bias_dev may be NULL).  The input is x_dev
+ *                   when non-NULL, else hi + lo of the split-bf16 planes x_hi_dev / x_lo_dev.  Exact (a gather).
+ *   pf_cpr_gram     over the n_idx rows idx_dev of X / Y (:751-769):
+ *                     F[(j,o), c] = sum_t X[idx[j], t*Cin + c] * W[t, c, o]  (float64),  y[(j,o)] = Y[idx[j], o]
+ *                     G = F^T F, b = F^T y, nrm = ||G||_F;  g_dev = (Cin+1)^2 + 1 doubles:
+ *                     g[i*(Cin+1) + j] = G[i][j] / nrm, g[i*(Cin+1) + Cin] = b[i] / nrm (i, j < Cin),
+ *                     g[(Cin+1)^2] = nrm;  gf_dev [Cin*Cin] / bf_dev [Cin] = the same in float32.
+ *                   F is formed chunk_rows rows of X at a time in ws_dev (pf_cpr_gram_ws_doubles doubles).
+ *                   CUDA-core FP64, fixed summation order (deterministic).
+ *   pf_cpr_ista     iters steps of m <- prox(m - lr*(G m - b), gamma*lr) in float32 from m0 (:449-452, :780-781),
+ *                   one cooperative launch; m_dev [Cin] = result, nnz_dev[0] = its count of non-zeros;
+ *                   ws_dev: 2*Cin floats.  Deterministic (fixed-order row sums).
+ *   pf_cpr_mask_channels  a[row, t, c, k] *= (|m[c]| > 0) for a of shape [rows, rs, Cin, inner]   (:817-820, :839)
+ * ------------------------------------------------------------------------------------------- */
+int pf_cpr_sample(const pf_conv_desc* d, const float* x_dev, const void* x_hi_dev, const void* x_lo_dev,
+                  const float* y_dev, const float* bias_dev, const int32_t* rows_dev, int n_rows, float* X_dev,
+                  float* Y_dev, void* stream);
+int64_t pf_cpr_gram_ws_doubles(int cin, int cout, int64_t chunk_rows);
+int pf_cpr_gram(const float* X_dev, const float* Y_dev, const int32_t* idx_dev, int n_idx, const float* w_dev, int rs,
+                int cin, int cout, double* ws_dev, int64_t chunk_rows, double* g_dev, float* gf_dev, float* bf_dev,
+                void* stream);
+int pf_cpr_ista(const float* g_dev, const float* b_dev, const float* m0_dev, int cin, float lr, float gamma, int iters,
+                float* m_dev, float* ws_dev, int32_t* nnz_dev, void* stream);
+int pf_cpr_mask_channels(float* a_dev, int64_t rows, int rs, int cin, int inner, const float* m_dev, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * a10 The collective of the data-parallel step (pf_comm.cu).  Replaces mgw.DistributedOptimizer's per-variable
  *     Horovod all-reduces and mgw.broadcast_global_variables (utils/multi_gpu_wrapper.py:82-98; call sites
  *     learners/uniform_quantization/learner.py:245-247, :271): ONE in-place ncclAllReduce (sum, fp32) over the flat

@@ -14,13 +14,16 @@ def create_learner(sm_writer, model_helper):
     elif FLAGS.learner == 'chn-pruned-gpu':
         from .channel_pruning_gpu.learner import ChannelPrunedGpuLearner
         learner = ChannelPrunedGpuLearner(sm_writer, model_helper)
+    elif FLAGS.learner == 'chn-pruned-rmt':
+        from .channel_pruning_rmt.learner import ChannelPrunedRmtLearner
+        learner = ChannelPrunedRmtLearner(sm_writer, model_helper)
     elif FLAGS.learner == 'uniform':
         from .uniform_quantization.learner import UniformQuantLearner
         learner = UniformQuantLearner(sm_writer, model_helper)
     elif FLAGS.learner == 'non-uniform':
         from .nonuniform_quantization.learner import NonUniformQuantLearner
         learner = NonUniformQuantLearner(sm_writer, model_helper)
-    elif FLAGS.learner in ('channel', 'chn-pruned-rmt', 'dis-chn-pruned', 'uniform-tf'):
+    elif FLAGS.learner in ('channel', 'dis-chn-pruned', 'uniform-tf'):
         raise ValueError('learner %s is outside the hot-path scope of this build (SURVEY.md §8)' % FLAGS.learner)
     else:
         raise ValueError('unrecognized learner\'s name: ' + FLAGS.learner)

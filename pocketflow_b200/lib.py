@@ -109,6 +109,11 @@ SIGNATURES = {
     'pf_cpg_prox_apply': (c_i32, [c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     'pf_cpg_channel_mask': (c_i32, [c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]),
     'pf_mul': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_vp]),
+    'pf_cpr_sample': (c_i32, [c_vp] * 7 + [c_i32, c_vp, c_vp, c_vp]),
+    'pf_cpr_gram_ws_doubles': (c_i64, [c_i32, c_i32, c_i64]),
+    'pf_cpr_gram': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    'pf_cpr_ista': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_f32, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    'pf_cpr_mask_channels': (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp]),
 }
 
 

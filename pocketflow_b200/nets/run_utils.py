@@ -11,6 +11,7 @@ from ..learners.learner_utils import create_learner
 from ..learners.full_precision import learner as _fp  # noqa: F401
 from ..learners.weight_sparsification import learner as _ws  # noqa: F401
 from ..learners.channel_pruning_gpu import learner as _cpg  # noqa: F401
+from ..learners.channel_pruning_rmt import learner as _cpr  # noqa: F401
 from ..learners.uniform_quantization import learner as _uq  # noqa: F401
 from ..learners.nonuniform_quantization import learner as _nuq  # noqa: F401
 

@@ -1005,3 +1005,127 @@ def cpg_channel_mask(w, mask, norms=None):
 def mul(a, b, out):
     _check_f32(a, b, out)
     _lib.check(_lib.load().pf_mul(_p(a), _p(b), a.numel(), _p(out), _stream()), 'pf_mul')
+
+
+# ----------------------------------------------------------------------------- f5 remastered channel selection (pf_cpr.cu)
+def cpr_sample(d, x, y, rows, X, Y, planes=None, bias=None):
+    """Gather pruned-model input patches into rows of X [*, R*S*Cin] (HWIO order) and conv outputs into rows of Y
+    [*, Cout] (channel_pruning_rmt/learner.py:679-703).  rows: int32 CUDA tensor [n, 4] = (n, oh, ow, dst row; < 0
+    skips the row).  The input is `x` (fp32 NHWC) or, when x is None, hi + lo of `planes` (an ops.Planes).  `bias`:
+    subtracted from the output (a conv whose bias is fused into its epilogue)."""
+    _check_f32(x, y, X, Y, bias)
+    if rows.dtype != torch.int32 or not rows.is_cuda or not rows.is_contiguous() or rows.dim() != 2 or rows.shape[1] != 4:
+        raise ValueError('cpr_sample: rows must be a contiguous int32 CUDA tensor [n, 4]')
+    _lib.check(_lib.load().pf_cpr_sample(ctypes.byref(d), _p(x), _p(planes.hi) if planes is not None else None,
+                                         _p(planes.lo) if planes is not None else None, _p(y), _p(bias), _p(rows),
+                                         rows.shape[0], _p(X), _p(Y), _stream()), 'pf_cpr_sample')
+
+
+def cpr_gram_ws_doubles(cin, cout, chunk_rows):
+    return int(_lib.load().pf_cpr_gram_ws_doubles(int(cin), int(cout), int(chunk_rows)))
+
+
+def cpr_gram_chunk_rows(cin, cout, n_idx, budget_bytes=1 << 30):
+    """rows of X per chunk of the float64 feature matrix so that it stays within `budget_bytes`"""
+    return int(max(1, min(n_idx, budget_bytes // (8 * (cin + 1) * cout))))
+
+
+def cpr_gram(X, Y, idx, w, g, gf, bf, ws=None, chunk_rows=None):
+    """G = F^T F, b = F^T y over the rows idx of X / Y, normalised by ||G||_F (channel_pruning_rmt/learner.py:751-769).
+    g: float64 [(Cin+1)^2 + 1] (G | b columns, then the norm); gf / bf: float32 G [Cin, Cin] / b [Cin]."""
+    rs, cin, cout = _rs_cin_cout(w)
+    _check_f32(X, Y, w, gf, bf)
+    if idx.dtype != torch.int32 or g.dtype != torch.float64 or g.numel() < (cin + 1) ** 2 + 1:
+        raise ValueError('cpr_gram: idx must be int32 and g float64 [(Cin+1)^2 + 1]')
+    if chunk_rows is None:
+        chunk_rows = cpr_gram_chunk_rows(cin, cout, idx.numel())
+    need = cpr_gram_ws_doubles(cin, cout, chunk_rows)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.float64, device=X.device)
+    _lib.check(_lib.load().pf_cpr_gram(_p(X), _p(Y), _p(idx), idx.numel(), _p(w), rs, cin, cout, _p(ws), int(chunk_rows),
+                                       _p(g), _p(gf), _p(bf), _stream()), 'pf_cpr_gram')
+    return ws
+
+
+def cpr_ista(gf, bf, m0, lr, gamma, iters, m, ws, nnz):
+    """iters ISTA steps at one gamma in one launch (channel_pruning_rmt/learner.py:449-452, :780-781); m = result,
+    nnz (int32 [1]) = its count of non-zeros; ws: 2*Cin floats.  gamma / lr are rounded to float32 as the LASSO graph's
+    placeholder / constant are."""
+    _check_f32(gf, bf, m0, m, ws)
+    cin = m0.numel()
+    if gf.numel() != cin * cin or bf.numel() != cin or m.numel() != cin or ws.numel() < 2 * cin or nnz.dtype != torch.int32:
+        raise ValueError('cpr_ista: shape mismatch')
+    _lib.check(_lib.load().pf_cpr_ista(_p(gf), _p(bf), _p(m0), cin, float(np.float32(lr)), float(np.float32(gamma)),
+                                       int(iters), _p(m), _p(ws), _p(nnz), _stream()), 'pf_cpr_ista')
+
+
+def cpr_mask_channels(a, m, rs, cin, inner):
+    """a[row, t, c, k] *= (|m[c]| > 0), a viewed as [rows, rs, cin, inner] (channel_pruning_rmt/learner.py:817-820)"""
+    _check_f32(a, m)
+    per = rs * cin * inner
+    if a.numel() % per or m.numel() != cin:
+        raise ValueError('cpr_mask_channels: shape mismatch')
+    _lib.check(_lib.load().pf_cpr_mask_channels(_p(a), a.numel() // per, rs, cin, inner, _p(m), _stream()),
+               'pf_cpr_mask_channels')
+
+
+class CprLstsq:
+    """The least-squares refit of one layer (channel_pruning_rmt/learner.py:470-523, :814-842): min_W ||X W - Y||^2 /
+    (2N) + wd ||W||^2 / 2 by `iters` Adam steps from the current kernel.  X W is a 1x1 conv over N "pixels" of
+    K = R*S*Cin channels and X^T (X W - Y) is its weight gradient, so the conv kernels do the GEMMs: tensor-core
+    (split-bf16) where `conv_path` is 'tc' and the pass's shape rule holds (fwd: K, Cout multiples of 16; wgrad: also
+    Cout a multiple of 64), exact fp32 otherwise.  The update is pf_adam_step with
+    hp = (lr, beta1^t, beta2^t), the powers as float32 pow as tf.pow(beta, train_step) (:504-505).  Deviation: its
+    moment update is TF's m += (g - m)(1 - beta1) instead of the reference's beta1 m + (1 - beta1) g (:499-500) —
+    equal up to rounding."""
+
+    def __init__(self, X, Y, conv_path='tc'):
+        n, k = X.shape
+        cout = Y.shape[1]
+        self.X, self.Y, self.n = X, Y, n
+        self.d = conv_desc(n, 1, 1, k, cout, 1, 1, 1, 1, 1, 1, 0, 0)
+        self.tc_fwd = conv_path == 'tc' and conv2d_tc_supported(self.d)
+        self.tc_wgrad = conv_path == 'tc' and conv2d_tc_wgrad_supported(self.d)
+        dev = X.device
+        self.P = torch.empty(n, cout, dtype=torch.float32, device=dev)
+        self.R = torch.empty(n, cout, dtype=torch.float32, device=dev)
+        self.g = torch.empty(k * cout, dtype=torch.float32, device=dev)
+        self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.l2ws = torch.empty(L2_PARTIALS, dtype=torch.float32, device=dev)
+        self.tw = TcWeights(self.d, dev, need_dgrad=False) if self.tc_fwd else None
+        ws = conv2d_tc_wgrad_workspace_floats(self.d) if self.tc_wgrad else conv2d_wgrad_workspace_floats(self.d)
+        self.ws = torch.empty(max(ws, 4), dtype=torch.float32, device=dev)
+
+    def residual(self, w):
+        """R = X W - Y; returns loss = ||R||^2 / 2 (device [1])"""
+        if self.tc_fwd:
+            self.tw.prepare(w)
+            conv2d_tc_fwd(self.d, self.X, self.tw, None, False, self.P)
+        else:
+            conv2d_fwd(self.d, self.X, w, None, False, self.P)
+        cpg_diff_l2(self.P, self.Y, self.R, self.loss, self.l2ws)
+        return self.loss
+
+    def run(self, w, iters, lr, wd, beta1=0.9, beta2=0.999, eps=1e-8):
+        """w: [R, S, Cin, Cout] fp32 (updated in place).  Returns (loss before, loss after) / N: the reference's loss_reg."""
+        m, v = torch.zeros_like(w), torch.zeros_like(w)
+        b1, b2 = np.float32(beta1), np.float32(beta2)
+        t = np.arange(1, iters + 1, dtype=np.float32)
+        hp = np.zeros((max(iters, 1), 4), dtype=np.float32)
+        hp[:iters, 0] = np.float32(lr)
+        hp[:iters, 1] = np.power(b1, t)
+        hp[:iters, 2] = np.power(b2, t)
+        hp = torch.from_numpy(hp).to(w.device)
+        inv_n = float(np.float32(1.0) / np.float32(self.n))
+        first = float(self.residual(w).item()) / self.n
+        for i in range(iters):
+            if i:
+                self.residual(w)
+            if self.tc_wgrad:
+                conv2d_tc_wgrad(self.d, self.X, self.R, self.ws, self.g)
+            else:
+                conv2d_wgrad(self.d, self.X, self.R, self.ws, self.g)
+            adam_step(w.reshape(-1), m.reshape(-1), v.reshape(-1), self.g, hp[i], beta1, beta2, eps, wd=wd,
+                      grad_scale=inv_n)
+        last = float(self.residual(w).item()) / self.n
+        return first, last
