@@ -501,6 +501,26 @@ int pf_bn_bwd_planes(const float* dy_dev, const float* x_dev, int64_t m, int c, 
                      const float* rstd_dev, const float* gamma_dev, const float* beta_dev, int act,
                      float* dgamma_dev, float* dbeta_dev, float* dx_dev, int accumulate, void* dx_hi_dev,
                      void* dx_lo_dev, float* ws_dev, void* stream);
+/* linear bottleneck + residual (MobileNet-v2, conv_blocks.py:289-313): y = bn(x) + res, BN without activation, in one
+ * pass — the training form with batch statistics (mean / rstd of pf_bn_train_stats), the _eval form with moving
+ * statistics (rstd formed in the kernel as in pf_bn_apply_eval).  Writes the fp32 sum and / or its split-bf16 planes
+ * (the operand of the next block's expand conv); at least one output.  The add is one __fadd_rn after the BN op
+ * chain: bit-identical to pf_bn_apply + pf_add.  8 B/element read, 4 (fp32) and / or 4 (planes) written. */
+int pf_bn_apply_add(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
+                    const float* gamma_dev, const float* beta_dev, const float* res_dev, float* y_dev, void* y_hi_dev,
+                    void* y_lo_dev, void* stream);
+int pf_bn_apply_add_eval(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
+                         float eps, const float* gamma_dev, const float* beta_dev, const float* res_dev, float* y_dev,
+                         void* y_hi_dev, void* y_lo_dev, void* stream);
+/* dropout (slim.dropout, mobilenet.py:369; TF 1.x nn_ops.dropout): y = (x / keep) * floor(keep + u), u in [0, 1) from
+ * Philox4x32-10 keyed by (seed, rank) with counter (element index / 4 [64 bits], step [low 32 bits], stream_id);
+ * mask_dev[i] <- floor(keep + u) (0 / 1).  stream_id tells the Dropout ops of one graph apart (each passes its own
+ * state).  state_dev[0] is the step, state_dev[1] scratch (both 0 initially): the launch reads the step and advances it
+ * by one, so a replayed CUDA graph draws a fresh mask each time.  Backward: dx (+)= (dy * mask) / keep. */
+int pf_dropout_fwd(const float* x_dev, int64_t n, float keep_prob, uint32_t seed, uint32_t rank, uint32_t stream_id,
+                   uint64_t* state_dev, float* y_dev, uint8_t* mask_dev, void* stream);
+int pf_dropout_bwd(const float* dy_dev, const uint8_t* mask_dev, int64_t n, float keep_prob, int accumulate, float* dx_dev,
+                   void* stream);
 /* out (+)= a (+ b): residual add (resnet_model.py:199,314) / gradient fan-out; b_dev may be NULL */
 int pf_add(const float* a_dev, const float* b_dev, int64_t n, int accumulate, float* out_dev, void* stream);
 /* dst[i][j] = sum_b src[b*m+i][b*n+j] (src is (g*m) x (g*n) row-major): folds the diagonal blocks of a weight gradient that

@@ -194,12 +194,16 @@ __device__ __forceinline__ float bn_act(float x, float mu, float rs, float ga, f
 }
 
 // y = act(bn(x)); optionally accumulates the per-tensor min/max of y (ordered-uint slots)
+// RES: y = bn(x) + res — a linear-bottleneck BN (no activation) feeding a residual Add (MobileNet-v2,
+// conv_blocks.py:289-313) in one pass; the add is one more correctly rounded step after the BN chain, so the result is
+// bit-identical to BN apply followed by pf_add.  8 B/element read (x, res) instead of 4 + 8 + 8 for the three passes.
+template <bool RES>
 __global__ void __launch_bounds__(NT)
 bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* __restrict__ mean,
                 const float* __restrict__ rstd, const float* __restrict__ gamma,
                 const float* __restrict__ beta, int act, float* __restrict__ y,
                 uint32_t* __restrict__ minmax_enc, void* __restrict__ y_hi, void* __restrict__ y_lo,
-                const uint32_t* __restrict__ q_range, int q_bits, float var_eps) {
+                const uint32_t* __restrict__ q_range, int q_bits, float var_eps, const float* __restrict__ res) {
   // var_eps >= 0: `rstd` holds the (moving) VARIANCE and rstd = rsqrt(var + eps) is formed here (inference mode;
   // same two roundings as bn_eval_prepare_kernel, one launch less per layer)
   __shared__ float s_mn[NT / 32], s_mx[NT / 32];
@@ -224,6 +228,10 @@ bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* 
     v.y = bn_act(v.y, mu.y, rs.y, ga.y, be.y, act);
     v.z = bn_act(v.z, mu.z, rs.z, ga.z, be.z, act);
     v.w = bn_act(v.w, mu.w, rs.w, ga.w, be.w, act);
+    if (RES) {
+      const float4 r = pf_ld_stream(res + (idx << 2));
+      v.x = __fadd_rn(v.x, r.x); v.y = __fadd_rn(v.y, r.y); v.z = __fadd_rn(v.z, r.z); v.w = __fadd_rn(v.w, r.w);
+    }
     if (q_range) {
       v.x = pf_fake_quant(v.x, q_alpha, q_beta, q_k, q_ra, q_rk);
       v.y = pf_fake_quant(v.y, q_alpha, q_beta, q_k, q_ra, q_rk);
@@ -906,7 +914,7 @@ int pf_bn_eval_prepare(const float* moving_var_dev, int c, float eps, float* rst
 static int bn_apply_impl(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
                          const float* gamma_dev, const float* beta_dev, int act, float* y_dev, void* y_hi_dev,
                          void* y_lo_dev, uint32_t* minmax_enc_dev, const uint32_t* q_range_dev, int q_bits, void* stream,
-                         float var_eps = -1.f) {
+                         float var_eps = -1.f, const float* res_dev = nullptr) {
   PF_REQUIRE(m > 0 && c > 0 && (c & 3) == 0, "pf_bn_apply: bad shape (C must be a multiple of 4)");
   PF_REQUIRE(act >= 0 && act <= 2, "pf_bn_apply: act must be 0 (none), 1 (relu) or 2 (relu6)");
   PF_REQUIRE(x_dev && mean_dev && rstd_dev && gamma_dev && beta_dev, "pf_bn_apply: null pointer");
@@ -914,9 +922,15 @@ static int bn_apply_impl(const float* x_dev, int64_t m, int c, const float* mean
   PF_REQUIRE((y_hi_dev == nullptr) == (y_lo_dev == nullptr), "pf_bn_apply: planes come in pairs");
   PF_REQUIRE((((uintptr_t)y_hi_dev | (uintptr_t)y_lo_dev) & 7) == 0, "pf_bn_apply: planes must be 8-byte aligned");
   const int64_t total = m * c;
-  bn_apply_kernel<<<chan_grid(total >> 2, c), NT, 0, (cudaStream_t)stream>>>(x_dev, total, c, mean_dev, rstd_dev, gamma_dev,
-                                                                     beta_dev, act, y_dev, minmax_enc_dev, y_hi_dev, y_lo_dev,
-                                                                     q_range_dev, q_bits, var_eps);
+  const unsigned grid = chan_grid(total >> 2, c);
+  if (res_dev)
+    bn_apply_kernel<true><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, total, c, mean_dev, rstd_dev, gamma_dev, beta_dev, act,
+                                                                 y_dev, minmax_enc_dev, y_hi_dev, y_lo_dev, q_range_dev, q_bits,
+                                                                 var_eps, res_dev);
+  else
+    bn_apply_kernel<false><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, total, c, mean_dev, rstd_dev, gamma_dev, beta_dev, act,
+                                                                  y_dev, minmax_enc_dev, y_hi_dev, y_lo_dev, q_range_dev, q_bits,
+                                                                  var_eps, nullptr);
   PF_CHECK_LAUNCH("pf_bn_apply");
   return PF_OK;
 }
@@ -973,6 +987,26 @@ int pf_bn_apply_quant_levels(const float* x_dev, int64_t m, int c, const float* 
                                                                         range_enc_dev, bits, hdr_dev, csum_dev, nseg);
   PF_CHECK_LAUNCH("pf_bn_apply_quant_levels");
   return PF_OK;
+}
+
+int pf_bn_apply_add(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
+                    const float* gamma_dev, const float* beta_dev, const float* res_dev, float* y_dev, void* y_hi_dev,
+                    void* y_lo_dev, void* stream) {
+  PF_REQUIRE(res_dev != nullptr, "pf_bn_apply_add: null residual");
+  PF_REQUIRE((((uintptr_t)res_dev | (uintptr_t)x_dev | (uintptr_t)y_dev) & 15) == 0, "pf_bn_apply_add: fp32 tensors must be 16-byte aligned");
+  return bn_apply_impl(x_dev, m, c, mean_dev, rstd_dev, gamma_dev, beta_dev, 0, y_dev, y_hi_dev, y_lo_dev, nullptr, nullptr, 0,
+                       stream, -1.f, res_dev);
+}
+
+int pf_bn_apply_add_eval(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
+                         float eps, const float* gamma_dev, const float* beta_dev, const float* res_dev, float* y_dev,
+                         void* y_hi_dev, void* y_lo_dev, void* stream) {
+  PF_REQUIRE(eps >= 0.f, "pf_bn_apply_add_eval: eps < 0");
+  PF_REQUIRE(res_dev != nullptr, "pf_bn_apply_add_eval: null residual");
+  PF_REQUIRE((((uintptr_t)res_dev | (uintptr_t)x_dev | (uintptr_t)y_dev) & 15) == 0,
+             "pf_bn_apply_add_eval: fp32 tensors must be 16-byte aligned");
+  return bn_apply_impl(x_dev, m, c, moving_mean_dev, moving_var_dev, gamma_dev, beta_dev, 0, y_dev, y_hi_dev, y_lo_dev, nullptr,
+                       nullptr, 0, stream, eps, res_dev);
 }
 
 int pf_bn_apply(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,

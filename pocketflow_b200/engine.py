@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
 
 F32 = np.float32
 MATMUL_TYPES = ('Conv2D', 'MatMul', 'DepthwiseConv2dNative')
@@ -151,6 +152,7 @@ class Executor:
         # CUDA-core kernels elsewhere; 'fp32': exact-fp32 everywhere (the on-device reference)
         import os as _os
         self.conv_path = conv_path or _os.environ.get('PF_CONV_PATH', 'tc')
+        self.seed = int(seed)
         self.ops = self._reachable_ops(logits)
         variables = []
         for op in self.ops:
@@ -280,13 +282,27 @@ class Executor:
                         raise ValueError('training the codebooks needs `clusters` variables on the quantized ops')
                     self.wq = ops.CodebookWeightQuantizer(srcs, dsts, wq['bits'])
         self.qvars = {op: op.vars['kernel'] for op in self.wq_ops}
+        # ---- dropout (slim.dropout): per training-mode Dropout op a mask, a Philox stream index (its position among the
+        # graph's Dropout ops) and a device-side step counter (row of drop_state) that the forward kernel advances, so a
+        # replayed CUDA graph draws a fresh mask each step; an inference-mode Dropout is the identity (an alias)
+        self.dropout, self.drop_stream = {}, {}
+        for op in self.ops:
+            if op.type == 'Dropout' and op.attrs['training']:
+                mask = torch.empty(op.output.numel, dtype=torch.uint8, device=dev)
+                if poison:
+                    mask.fill_(0xff)
+                self.drop_stream[op] = len(self.dropout)
+                self.dropout[op] = mask
+        self.drop_state = torch.zeros(len(self.dropout), 2, dtype=torch.int64, device=dev) if self.dropout else None
+        self.drop_key = (self.seed, mgw.rank())
+        self._drop_on = False          # set per forward(): masks only in training-mode passes
         # ---- tensors
         for op in self.ops:
             t = op.output
             if op.type == 'Placeholder':
                 self.buf[t] = E(t.shape)
                 self.buf[t].zero_()
-            elif op.type in ('Reshape', 'Identity'):
+            elif self._passthrough(op):
                 self.alias[t] = op.inputs[0]
             elif op in self.fused_into:
                 self.alias[t] = op.inputs[0]
@@ -406,6 +422,23 @@ class Executor:
                     self.add_fused.add(op)
                     self.buf[x_t] = self.buf[op.output]       # the conv output IS the add output
                     break
+        # ---- linear bottleneck: a BatchNorm without activation whose only consumer is a residual Add (MobileNet-v2's
+        # projection, conv_blocks.py:289-313) writes bn(x) + shortcut straight into the Add's buffer (and / or the
+        # Add's operand planes, below) — one pass instead of BN apply + add + split
+        self.bn_add = {}           # BN op -> (add op, other input tensor)
+        fuse_bn_add = os.environ.get('PF_FUSE_BN_ADD', '1') != '0'
+        for op in self.ops:
+            if op.type != 'Add' or op in self.add_fused or not fuse_bn_add:
+                continue
+            for i, x_t in enumerate(op.inputs):
+                src, other = x_t.op, op.inputs[1 - i]
+                if src.type == 'FusedBatchNorm' and src not in self.fused_act and x_t not in self.alias \
+                        and self._consumers(x_t) == [op] and other is not x_t \
+                        and self.g.ops.index(other.op) < self.g.ops.index(src):
+                    self.bn_add[src] = (op, other)
+                    self.add_fused.add(op)
+                    self.buf[x_t] = self.buf[op.output]       # the BN output IS the add output
+                    break
         # ---- split-bf16 operand planes (tensor-core path): the BN-apply / activation-quantizer that produces a conv
         # input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
         # the fp32 copy is only written when some other consumer needs it
@@ -414,7 +447,7 @@ class Executor:
         for op in self.ops:
             if op in self.tc and op not in self.im2col:
                 r = self._root(op.inputs[0])
-                if r is not None and r.op.type == 'FusedBatchNorm' and r.numel % 8 == 0:
+                if r is not None and (r.op.type == 'FusedBatchNorm' or r.op in self._add_of_bn()) and r.numel % 8 == 0:
                     if r.op not in self.xplanes:
                         self.xplanes[r.op] = ops.Planes(r.numel, dev)
                         self.bn_need_f32[r.op] = False
@@ -564,7 +597,7 @@ class Executor:
             # writer and the conv the only reader, the fp32 copy is dropped and the planes live in its memory.
             grad_writers = {}
             for op in self.ops:
-                if op.type in ('Placeholder', 'Reshape', 'Identity') or op in self.fused_into:
+                if op.type == 'Placeholder' or self._passthrough(op) or op in self.fused_into:
                     continue
                 ins = op.inputs if op.type == 'Add' else op.inputs[:1]
                 for x_t in ins:
@@ -669,8 +702,17 @@ class Executor:
             if op in self.aq_out:
                 return self.aq_out[op].view(shape)
             t = self.alias[t]
+        if t.op in self.dropout and not self._drop_on:
+            return self.T(t.op.inputs[0]).view(shape)         # inference-mode pass: dropout is the identity
         b = self.buf[t]
         return b if b.shape == shape else b.view(shape)
+
+    def _passthrough(self, op):
+        """ops that launch nothing and whose output (and gradient) buffer is their input's"""
+        return op.type in ('Reshape', 'Identity') or (op.type == 'Dropout' and op not in self.dropout)
+
+    def _add_of_bn(self):
+        return {a for a, _ in self.bn_add.values()}
 
     def _root(self, t):
         """The tensor whose buffer holds t (following Reshape / fused-activation aliases); None when t is
@@ -741,6 +783,7 @@ class Executor:
         if self.static_weights and not self._static_ready:
             self.prepare_static_weights()
         self._lv_on = bool(training and (self.act_lv or self.w_lv))
+        self._drop_on = bool(training)
         if self.tc_batch is not None:
             with self.timed('conv_prep'):
                 self.tc_batch.prepare(levels=self._lv_on)
@@ -750,7 +793,7 @@ class Executor:
                 return None
             prev = op
             ty = op.type
-            if ty in ('Placeholder', 'Reshape', 'Identity'):
+            if ty == 'Placeholder' or self._passthrough(op):
                 continue
             if ty in ('Conv2D', 'MatMul'):
                 bias = st.view(op.vars['bias']) if 'bias' in op.vars else None
@@ -802,6 +845,26 @@ class Executor:
             elif ty == 'DepthwiseConv2dNative':
                 with self.timed('dwconv'):
                     ops.dwconv_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), self.buf[op.output])
+            elif ty == 'FusedBatchNorm' and op in self.bn_add:
+                x, y = self.T(op.inputs[0]), self.buf[op.output]
+                c = y.shape[-1]
+                m = y.numel() // c
+                b = self.bn[op]
+                gamma, beta = st.view(op.vars['gamma']), st.view(op.vars['beta'])
+                mm, mv = st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance'])
+                add_op, other = self.bn_add[op]
+                pl = self.xplanes.get(add_op)
+                y_out = y if (pl is None or self.bn_need_f32[add_op]) else None
+                if op.attrs['training'] and training:
+                    with self.timed('bn_stats'):
+                        ops.bn_train_stats(x, m, c, op.attrs['epsilon'],
+                                           op.attrs['momentum'] if self.update_moving_stats else 1.0, b['mean'],
+                                           b['var'], b['rstd'], mm, mv, self.bn_ws)
+                    with self.timed('bn_apply'):
+                        ops.bn_apply_add(x, m, c, b['mean'], b['rstd'], gamma, beta, self.T(other), y_out, pl)
+                else:
+                    with self.timed('bn_apply'):
+                        ops.bn_apply_add_eval(x, m, c, mm, mv, op.attrs['epsilon'], gamma, beta, self.T(other), y_out, pl)
             elif ty == 'FusedBatchNorm':
                 x, y = self.T(op.inputs[0]), self.buf[op.output]
                 c = y.shape[-1]
@@ -861,9 +924,15 @@ class Executor:
                 n, h, w, c = x.shape
                 with self.timed('pool'):
                     ops.global_avgpool_fwd(self.T(x), n, h * w, c, self.buf[op.output])
+            elif ty == 'Dropout':
+                if training:
+                    with self.timed('dropout'):
+                        i = self.drop_stream[op]
+                        ops.dropout_fwd(self.T(op.inputs[0]), op.attrs['keep_prob'], self.drop_key[0], self.drop_key[1],
+                                        self.drop_state[i], self.buf[op.output], self.dropout[op], stream_id=i)
             elif ty == 'Add':
                 if op in self.add_fused:
-                    continue                               # computed by the producing conv's epilogue
+                    continue                               # computed by the producing conv's / BN's epilogue
                 with self.timed('add_fwd'):
                     ops.add(self.T(op.inputs[0]), self.T(op.inputs[1]), self.buf[op.output])
             elif ty == 'Softmax':
@@ -957,7 +1026,7 @@ class Executor:
             gy = self.grad_of(op.output)
             if gy is None:
                 continue
-            if ty in ('Reshape', 'Identity') or op in self.fused_into:
+            if self._passthrough(op) or op in self.fused_into:
                 continue                                   # gradient buffer is shared with the input
             if ty in ('Conv2D', 'MatMul'):
                 d = self.desc[op]
@@ -1058,6 +1127,10 @@ class Executor:
                 gx, acc = self.grad_target(x_t)
                 with self.timed('pool'):
                     ops.maxpool_bwd(self.desc[op], gy, self.pool_argmax[op], gx, acc)
+            elif ty == 'Dropout':
+                gx, acc = self.grad_target(op.inputs[0])
+                with self.timed('dropout'):
+                    ops.dropout_bwd(gy, self.dropout[op], op.attrs['keep_prob'], gx, acc)
             elif ty == 'Mean':
                 x_t = op.inputs[0]
                 n, h, w, c = x_t.shape

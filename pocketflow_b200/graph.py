@@ -305,6 +305,7 @@ def truncated_normal_initializer(stddev):
             x[bad] = rng.standard_normal(size=int(bad.sum()))
             bad = np.abs(x) > 2
         return (x * stddev).astype(np.float32)
+    init.stddev = stddev
     return init
 
 
@@ -329,6 +330,14 @@ def softmax(inputs, name=None):
 def identity(inputs, name):
     g = get_default_graph()
     return g.add_op('Identity', name, [inputs], {}, {}, inputs.shape).output
+
+
+def dropout(inputs, keep_prob, is_training, name=None):
+    """slim.dropout: y = (x / keep_prob) * floor(keep_prob + u), u ~ U[0, 1), in a training-mode forward pass; the
+    identity otherwise (and always when is_training is False)."""
+    g = get_default_graph()
+    return g.add_op('Dropout', name or 'Dropout', [inputs], {},
+                    dict(keep_prob=float(keep_prob), training=bool(is_training)), inputs.shape).output
 
 
 # ------------------------------------------------------------------------------ losses / metrics

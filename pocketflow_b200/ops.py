@@ -594,6 +594,37 @@ def bn_bwd(dy, x, m, c, mean, rstd, gamma, beta, act, dgamma, dbeta, dx, accumul
                                                 _p(planes.lo), _p(ws), _stream()), 'pf_bn_bwd_planes')
 
 
+def bn_apply_add(x, m, c, mean, rstd, gamma, beta, res, y=None, planes=None):
+    """y = bn(x) + res (linear bottleneck + residual, training-mode statistics), to fp32 and / or operand planes"""
+    _lib.check(_lib.load().pf_bn_apply_add(_p(x), m, c, _p(mean), _p(rstd), _p(gamma), _p(beta), _p(res), _p(y),
+                                           _p(planes.hi if planes is not None else None),
+                                           _p(planes.lo if planes is not None else None), _stream()), 'pf_bn_apply_add')
+
+
+def bn_apply_add_eval(x, m, c, mov_mean, mov_var, eps, gamma, beta, res, y=None, planes=None):
+    """y = bn(x) + res with the moving statistics (inference mode), to fp32 and / or operand planes"""
+    _lib.check(_lib.load().pf_bn_apply_add_eval(_p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma), _p(beta),
+                                                _p(res), _p(y), _p(planes.hi if planes is not None else None),
+                                                _p(planes.lo if planes is not None else None), _stream()),
+               'pf_bn_apply_add_eval')
+
+
+def dropout_fwd(x, keep_prob, seed, rank, state, y, mask, stream_id=0):
+    """slim.dropout in a training pass: y = (x / keep) * mask, mask = floor(keep + u) (uint8), u from Philox4x32-10 keyed
+    by (seed, rank) at the step held in `state` (int64 [2] on the device, advanced by the launch) of stream `stream_id`
+    (one per Dropout op of a graph)"""
+    assert state.dtype == torch.int64 and state.numel() >= 2 and mask.dtype == torch.uint8 and mask.numel() >= x.numel()
+    _lib.check(_lib.load().pf_dropout_fwd(_p(x), x.numel(), float(keep_prob), int(seed) & 0xffffffff,
+                                          int(rank) & 0xffffffff, int(stream_id) & 0xffffffff, _p(state), _p(y), _p(mask),
+                                          _stream()), 'pf_dropout_fwd')
+
+
+def dropout_bwd(dy, mask, keep_prob, dx, accumulate=False):
+    """dx (+)= (dy * mask) / keep"""
+    _lib.check(_lib.load().pf_dropout_bwd(_p(dy), _p(mask), dy.numel(), float(keep_prob), int(bool(accumulate)), _p(dx),
+                                          _stream()), 'pf_dropout_bwd')
+
+
 def add(a, b, out, accumulate=False):
     _lib.check(_lib.load().pf_add(_p(a), _p(b), a.numel(), int(bool(accumulate)), _p(out), _stream()), 'pf_add')
 
