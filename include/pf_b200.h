@@ -227,6 +227,32 @@ int pf_nuq_cluster_grad(const pf_uq_seg* gsegs_dev, int n_seg, const pf_work* wo
                         const float* scales_dev, float* partial_ws_dev, float* grad_base_dev,
                         const int64_t* cluster_off_dev, void* stream);
 
+/* f5  Bucketed codebooks (NonUniformQuantization.__bucket_quantize, utils.py:196-243).  segs as for the bucketed
+ *     pf_uq_weight_minmax (ncols = nb buckets, bucket of flat element i = i % nb, split padding = copies of the last
+ *     element), scales from pf_uq_weight_minmax + pf_uq_weight_scales on those segs.  The codebook of bucket b of
+ *     tensor seg is column b of a [K, nb] matrix: c[j, b] = clusters_base[cluster_off[seg] + j * nb + b], K >= 2^bits.
+ *     Quantize / gradient work: kind-1 tiles (columns [c0, c0 + ncol_tile), rows [start, start + count)) with
+ *     ncol_tile <= min(256, 8192 / 2^bits); the tile's codebooks are staged in shared memory.  Only the real elements
+ *     (flat index < numel) are quantized, indexed and differentiated. */
+#define PF_NUQ_BUCKET_MAX_ROWS 16384
+int pf_nuq_bucket_quant(const pf_uq_seg* segs_dev, const pf_work* work_dev, int n_work, const float* scales_dev,
+                        int n_buckets, const float* clusters_base_dev, const int64_t* cluster_off_dev,
+                        uint8_t* idx_out_dev, const int64_t* idx_base_dev, void* stream);
+/* c[j, b] = (sorted_b[pos[seg*256 + j]] - beta_b) / alpha_b for j < 2^bits, 0 for 2^bits <= j < K: exact order
+ *     statistics of every bucket (its padded rows included).  work: one item per bucket, seg, c0 = bucket,
+ *     count = rows of the bucket (<= PF_NUQ_BUCKET_MAX_ROWS = max_rows bound), ncol_tile = K.  pos: ascending
+ *     positions, 256 per seg. */
+int pf_nuq_bucket_quantile_init(const pf_uq_seg* segs_dev, const pf_work* work_dev, int n_work, int max_rows,
+                                const int32_t* pos_dev, const float* scales_dev, int n_buckets,
+                                float* clusters_base_dev, const int64_t* cluster_off_dev, void* stream);
+/* dL/dc[j, b] = alpha_b * sum_{i in b, i < numel, idx_i = j} g_i.  work = the quantize tiles, each with
+ *     reserved = float offset of its 2^bits * ncol_tile partials in partial_ws_dev; tiles_dev: one item per column
+ *     tile, start / count = its range of `work` (row order), c0 / ncol_tile as there.  Deterministic. */
+int pf_nuq_bucket_cluster_grad(const pf_uq_seg* gsegs_dev, const pf_work* work_dev, int n_work,
+                               const pf_work* tiles_dev, int n_tiles, const uint8_t* idx_dev,
+                               const int64_t* idx_base_dev, const float* scales_dev, float* partial_ws_dev,
+                               float* grad_base_dev, const int64_t* cluster_off_dev, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * a4  Convolution / dense layers, exact-fp32 CUDA-core path (pf_conv.cu).
  *     Replaces tf.nn.conv2d / tf.matmul re-created on the quantized weight

@@ -274,13 +274,17 @@ class Executor:
                 # live in the parameter store), else a private table of the quantizer
                 cvars = [op.vars.get('clusters') for op in self.wq_ops]
                 self.train_clusters = bool(wq.get('train_clusters', False)) and self.train
+                # bucketed codebooks (utils.py:196-243): one [2^bits, nb] codebook matrix per tensor
+                bkw = dict(use_buckets=True, bucket_type=wq.get('bucket_type', 'split'),
+                           bucket_size=wq.get('bucket_size', 256)) if wq.get('use_buckets', False) else {}
                 if all(c is not None for c in cvars):
                     self.wq = ops.CodebookWeightQuantizer(srcs, dsts, wq['bits'], keep_index=self.train_clusters,
-                                                          cluster_views=[st.view(c) for c in cvars], cluster_base=st.P)
+                                                          cluster_views=[st.view(c) for c in cvars], cluster_base=st.P,
+                                                          **bkw)
                 else:
                     if self.train_clusters:
                         raise ValueError('training the codebooks needs `clusters` variables on the quantized ops')
-                    self.wq = ops.CodebookWeightQuantizer(srcs, dsts, wq['bits'])
+                    self.wq = ops.CodebookWeightQuantizer(srcs, dsts, wq['bits'], **bkw)
         self.qvars = {op: op.vars['kernel'] for op in self.wq_ops}
         # ---- dropout (slim.dropout): per training-mode Dropout op a mask, a Philox stream index (its position among the
         # graph's Dropout ops) and a device-side step counter (row of drop_state) that the forward kernel advances, so a

@@ -13,7 +13,7 @@ from ...utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
 from ...utils.lrn_rate_utils import piecewise_constant
 from ..abstract_learner import AbstractLearner, latest_checkpoint, load_checkpoint, save_checkpoint
 from ..distillation_helper import DistillationHelper
-from .utils import NonUniformQuantization
+from .utils import NonUniformQuantization, check_bucket_args
 from .bit_optimizer import BitOptimizer
 
 DEFINE_string('nuql_opt_mode', 'weights', 'the variables to optimize: [clusters, weights, both]')
@@ -58,6 +58,8 @@ def setup_bnds_decay_rates(model_name, dataset_name):
 class NonUniformQuantLearner(AbstractLearner):
     # pylint: disable=too-many-instance-attributes
     def __init__(self, sm_writer, model_helper):
+        if FLAGS.nuql_use_buckets:      # before anything is built or allocated
+            check_bucket_args(FLAGS.nuql_init_style, FLAGS.nuql_bucket_type, FLAGS.nuql_bucket_size)
         super(NonUniformQuantLearner, self).__init__(sm_writer, model_helper)
         # learner.py:254-268 tests for 'cluster' / 'both' / 'weights' (the flag's help text says 'clusters'; that
         # spelling ends in the reference's ValueError too)
@@ -131,7 +133,17 @@ class NonUniformQuantLearner(AbstractLearner):
             self.feed(ex, self.eval_iterator())
             ex.forward_eval_loss()
             out.append(ex.fetch_losses()['loss'])
+        if FLAGS.nuql_use_buckets:
+            self.__show_bucket_storage(self.bucket_storage)
         return float(np.mean(out))
+
+    def __show_bucket_storage(self, bucket_storage):
+        """learner.py:470-476, 497-503: the weight storage counts nuql_equivalent_bits per weight under the RL agent."""
+        weight_storage = sum(self.statistics['num_weights']) * (FLAGS.nuql_equivalent_bits if FLAGS.nuql_enbl_rl_agent
+                                                                else FLAGS.nuql_weight_bits)
+        print('bucket storage: %d bit / %.3f kb | weight storage: %d bit / %.3f kb | ratio: %.3f'
+              % (bucket_storage, bucket_storage / (8. * 1024.), weight_storage, weight_storage / (8. * 1024.),
+                 bucket_storage * 1. / weight_storage))
 
     # ------------------------------------------------------------------ what the RL bit search drives
     def rl_restore(self):
@@ -203,6 +215,7 @@ class NonUniformQuantLearner(AbstractLearner):
                 self.optimal_w_bit_list, self.optimal_a_bit_list = w_bits, a_bits
                 nq.insert_quant_op_for_weights({op.name: b for op, b in zip(matmul_ops, w_bits)})
                 nq.insert_quant_op_for_activations({op.name: b for op, b in zip(act_ops, a_bits)})
+                self.bucket_storage = nq.bucket_storage       # bits of the per-bucket alpha / beta (0 without buckets)
                 # "Strictly speaking, clusters should be not included for regularization" (learner.py:219-220): they are
                 loss, metrics = self.calc_loss(labels, logits, self.trainable_vars)
                 if FLAGS.enbl_dst:

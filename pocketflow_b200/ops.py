@@ -73,6 +73,49 @@ def minmax_works(segs):
     return np.array(rows, dtype=WORK) if rows else np.zeros(0, dtype=WORK)
 
 
+NUQ_BUCKET_SMEM_FLOATS = 8192   # codebook floats of one bucketed-quantize tile (pf_nuq.cu kBucketSmemFloats)
+NUQ_BUCKET_MAX_ROWS = 16384     # PF_NUQ_BUCKET_MAX_ROWS: largest bucket the quantile init sorts in shared memory
+
+
+def nuq_bucket_tile_width(bits):
+    """Columns (buckets) per tile of the bucketed codebook kernels: the tile's [2^bits, width] codebooks fit in
+    NUQ_BUCKET_SMEM_FLOATS, and one thread per column fits in a 256-thread CTA."""
+    return min(256, NUQ_BUCKET_SMEM_FLOATS >> int(bits))
+
+
+def nuq_bucket_works(segs):
+    """Work tables of the bucketed codebook kernels over the [padded/nb, nb] views: (tiles, finals, partial floats).
+    tiles: kind-1 items, columns [c0, c0+ncol_tile) x a row range, reserved = float offset of the tile's 2^bits x
+    ncol_tile gradient partials; finals: one item per column tile, start/count = its range of `tiles`."""
+    rows, finals, poff = [], [], 0
+    for s, seg in enumerate(segs):
+        nb, padded, bits = int(seg['ncols']), int(seg['padded']), int(seg['bits'])
+        k, tw = 1 << bits, nuq_bucket_tile_width(bits)
+        nrows = padded // nb
+        rows_per = max(2 * CHUNK // tw, 4 * k)
+        for c0 in range(0, nb, tw):
+            tc = min(tw, nb - c0)
+            first = len(rows)
+            for r0 in range(0, nrows, rows_per):
+                rows.append((s, 1, r0, min(rows_per, nrows - r0), c0, tc, poff))
+                poff += k * tc
+            finals.append((s, 1, first, len(rows) - first, c0, tc, 0))
+    if poff >= 2 ** 31:
+        raise ValueError('too many codebook-gradient partials for one launch')
+    mk = lambda r: np.array(r, dtype=WORK) if r else np.zeros(0, dtype=WORK)
+    return mk(rows), mk(finals), poff
+
+
+def nuq_bucket_quantile_positions(rows, bits):
+    """Ascending sort positions of centroids j < 2^bits of a bucket of `rows` elements: percentile(x_n,
+    (j+1)*100/(k+1), axis=0) with the 'nearest' rule (utils.py:349-366), padded to 256 entries."""
+    k = 1 << int(bits)
+    pos = np.zeros(256, np.int32)
+    for j in range(k):
+        pos[j] = rows - 1 - percentile_rank_desc(rows, (j + 1) * 100 / (k + 1))
+    return pos
+
+
 def percentile_rank_desc(n, q):
     """Index into the descending sort gathered by tf.contrib.distributions.percentile
     (interpolation='nearest'): clip(int32(rint((n-1)*(1-q/100))), 0, n-1) in float64."""
@@ -386,12 +429,22 @@ class CodebookWeightQuantizer:
 
     The codebooks are either a private [tensors, 256] table (`clusters`), or — `cluster_views` — 1-D views of ONE flat
     buffer `cluster_base` that the caller owns: the reference's trainable `clusters` variables (utils.py:297), which then
-    sit among the model's parameters (optimizer, weight decay, checkpoints, broadcast all apply to them)."""
+    sit among the model's parameters (optimizer, weight decay, checkpoints, broadcast all apply to them).
 
-    def __init__(self, srcs, dsts, bits, keep_index=False, cluster_views=None, cluster_base=None):
+    use_buckets: one range and one codebook per bucket — NonUniformQuantization.__bucket_quantize (utils.py:196-243),
+    the 'channel' / 'split' layouts of uq_bucket_layout.  The codebooks of a tensor with nb buckets are then a [K, nb]
+    matrix (column b = bucket b, K >= 2^bits rows): cluster_views of K * nb floats, or a private [256, nb] table per
+    tensor (codebooks())."""
+
+    def __init__(self, srcs, dsts, bits, keep_index=False, cluster_views=None, cluster_base=None,
+                 use_buckets=False, bucket_type='split', bucket_size=256):
         self.L = _lib.load()
         _check_f32(*srcs)
         _check_f32(*dsts)
+        self.use_buckets = bool(use_buckets)
+        if self.use_buckets:
+            self._init_buckets(srcs, dsts, bits, keep_index, cluster_views, cluster_base, bucket_type, bucket_size)
+            return
         self.uq = UniformWeightQuantizer(srcs, dsts, bits)       # per-layer ranges + tables
         if any(b > 8 for b in self.uq.bits):
             raise ValueError('codebook bit-widths must be <= 8')
@@ -422,10 +475,85 @@ class CodebookWeightQuantizer:
             self.idx_offsets = offs
         self._grad_tables = None
 
+    def _init_buckets(self, srcs, dsts, bits, keep_index, cluster_views, cluster_base, bucket_type, bucket_size):
+        if bucket_type == 'split' and int(bucket_size) <= 0:
+            raise ValueError('split buckets need a positive bucket size (got %d)' % int(bucket_size))
+        self.uq = UniformWeightQuantizer(srcs, dsts, bits, True, bucket_type, bucket_size)   # per-bucket ranges
+        if any(b > 8 for b in self.uq.bits):
+            raise ValueError('codebook bit-widths must be <= 8')
+        self.srcs, self.dsts = list(srcs), list(dsts)
+        self.device = self.uq.device
+        self.nb = [int(s['ncols']) for s in self.uq.segs]
+        self.rows = [int(s['padded']) // int(s['ncols']) for s in self.uq.segs]
+        if any(r > NUQ_BUCKET_MAX_ROWS for r in self.rows):
+            raise ValueError('a bucket holds %d elements; the bucketed quantile init supports up to %d'
+                             % (max(self.rows), NUQ_BUCKET_MAX_ROWS))
+        self.cluster_views = None
+        if cluster_views is not None:
+            _check_f32(cluster_base, *cluster_views)
+            offs, krows = [], []
+            for v, b, nb in zip(cluster_views, self.uq.bits, self.nb):
+                off = (v.data_ptr() - cluster_base.data_ptr()) // 4
+                if v.numel() % nb or v.numel() < (1 << b) * nb or off < 0 or off + v.numel() > cluster_base.numel():
+                    raise ValueError('bucketed codebook views must hold [K >= 2^bits, nb] floats inside cluster_base')
+                offs.append(off)
+                krows.append(v.numel() // nb)
+            self.cluster_views, self.cluster_base = list(cluster_views), cluster_base
+            self.clusters = None
+        else:
+            offs, krows, tot = [], [], 0
+            for nb in self.nb:
+                offs.append(tot)
+                krows.append(256)
+                tot += (256 * nb + 3) // 4 * 4
+            self.clusters = torch.zeros(max(tot, 4), dtype=torch.float32, device=self.device)
+            self.cluster_base = self.clusters
+        self.cluster_krows, self.cluster_offsets = krows, offs
+        self.cluster_off = torch.tensor(offs, dtype=torch.int64, device=self.device)
+        self.idx = None
+        if keep_index:
+            ioffs, tot = [], 0
+            for s in srcs:
+                ioffs.append(tot)
+                tot += (s.numel() + 15) // 16 * 16
+            self.idx = torch.zeros(tot, dtype=torch.uint8, device=self.device)
+            self.idx_base = torch.tensor(ioffs, dtype=torch.int64, device=self.device)
+            self.idx_offsets = ioffs
+        qi = [(s, 2, 0, r, b, k, 0) for s, (nb, r, k) in enumerate(zip(self.nb, self.rows, krows)) for b in range(nb)]
+        self.work_qi = np.array(qi, dtype=WORK) if qi else np.zeros(0, dtype=WORK)
+        self.work_qi_dev = _upload(self.work_qi, self.device)
+        self._bucket_tables()
+
+    def _bucket_tables(self):
+        """Tables that depend on the bit-widths: the tiles (their width is 8192 / 2^bits at most) and the quantile
+        positions."""
+        self.work_b, self.work_fin, n_partial = nuq_bucket_works(self.uq.segs)
+        self.work_b_dev = _upload(self.work_b, self.device)
+        self.work_fin_dev = _upload(self.work_fin, self.device)
+        self.partial = torch.empty(max(n_partial, 1), dtype=torch.float32, device=self.device)
+        pos = np.stack([nuq_bucket_quantile_positions(r, b) for r, b in zip(self.rows, self.uq.bits)]) \
+            if self.rows else np.zeros((1, 256), np.int32)
+        self.qpos_dev = torch.from_numpy(pos.reshape(-1).astype(np.int32)).to(self.device)
+        self._grad_tables = None
+
+    def codebooks(self):
+        """[K, nb] views of the codebooks (column b = bucket b's 2^bits centroids in its first rows)."""
+        if self.cluster_views is not None:
+            return [v.view(-1, nb) for v, nb in zip(self.cluster_views, self.nb)]
+        return [self.clusters[o:o + k * nb].view(k, nb)
+                for o, k, nb in zip(self.cluster_offsets, self.cluster_krows, self.nb)]
+
+    def bucket_storage_bits(self):
+        """alpha and beta of every bucket, 32 bits each (utils.py:487-494)."""
+        return self.uq.bucket_storage_bits()
+
     def quantile_values(self):
         """clusters_j = percentile(x_n, (j+1)*100/(k+1)) (utils.py:349-366), [tensors][k] as numpy.  x -> x_n is
         monotone non-decreasing in fp32, so the order statistic is selected on the raw weights (exact radix select)
-        and normalised afterwards with the same fp32 ops."""
+        and normalised afterwards with the same fp32 ops.  With buckets: [tensors] of [2^bits, nb] arrays."""
+        if self.use_buckets:
+            self.quantile_init()
+            return [c[:1 << b].cpu().numpy() for c, b in zip(self.codebooks(), self.uq.bits)]
         self.uq.minmax()
         queries = []
         for i, s in enumerate(self.srcs):
@@ -449,12 +577,27 @@ class CodebookWeightQuantizer:
         bits = [int(b) for b in (bits if hasattr(bits, '__len__') else [bits] * len(self.srcs))]
         if any(b < 1 or b > 8 for b in bits):
             raise ValueError('codebook bit-widths must be in [1, 8]')
+        if self.use_buckets:
+            if any(k < (1 << b) for k, b in zip(self.cluster_krows, bits)):
+                raise ValueError('a codebook variable has fewer than 2^bits rows')
+            self.uq.set_bits(bits)
+            self._bucket_tables()
+            return
         if self.cluster_views is not None and any(v.numel() < (1 << b) for v, b in zip(self.cluster_views, bits)):
             raise ValueError('a codebook variable is smaller than 2^bits')
         self.uq.set_bits(bits)
         self._grad_tables = None
 
     def quantile_init(self):
+        if self.use_buckets:
+            # per-bucket ranges, then every bucket's order statistics in one launch
+            self.uq.minmax()
+            if len(self.work_qi):
+                _lib.check(self.L.pf_nuq_bucket_quantile_init(
+                    _p(self.uq.segs_dev), _p(self.work_qi_dev), len(self.work_qi), max(self.rows), _p(self.qpos_dev),
+                    _p(self.uq.scales), self.uq.n_buckets, _p(self.cluster_base), _p(self.cluster_off), _stream()),
+                    'pf_nuq_bucket_quantile_init')
+            return
         vals = self.quantile_values()
         if self.cluster_views is not None:
             for v, c in zip(self.cluster_views, vals):
@@ -469,6 +612,12 @@ class CodebookWeightQuantizer:
     def forward(self):
         self.uq.minmax()
         idx_base = _p(self.idx_base) if self.idx is not None else None
+        if self.use_buckets:
+            _lib.check(self.L.pf_nuq_bucket_quant(_p(self.uq.segs_dev), _p(self.work_b_dev), len(self.work_b),
+                                                  _p(self.uq.scales), self.uq.n_buckets, _p(self.cluster_base),
+                                                  _p(self.cluster_off), _p(self.idx), idx_base, _stream()),
+                       'pf_nuq_bucket_quant')
+            return
         if self.cluster_views is not None:
             _lib.check(self.L.pf_nuq_weight_quant_ex(_p(self.uq.segs_dev), _p(self.uq.work_q_dev), len(self.uq.work_q),
                                                      _p(self.uq.scales), self.uq.n_buckets, _p(self.cluster_base),
@@ -487,6 +636,18 @@ class CodebookWeightQuantizer:
             raise ValueError('cluster_grad needs keep_index=True and cluster_views')
         _check_f32(grad_base, *grads)
         ptrs = [g.data_ptr() for g in grads]
+        if self.use_buckets:
+            # dL/dc[j, b] = alpha_b * sum over bucket b's real elements with idx = j
+            if self._grad_tables is None or self._grad_tables[0] != ptrs:
+                gs = self.uq.segs.copy()
+                gs['src'] = ptrs
+                gs['dst'] = ptrs
+                self._grad_tables = (ptrs, _upload(gs, self.device))
+            _lib.check(self.L.pf_nuq_bucket_cluster_grad(
+                _p(self._grad_tables[1]), _p(self.work_b_dev), len(self.work_b), _p(self.work_fin_dev),
+                len(self.work_fin), _p(self.idx), _p(self.idx_base), _p(self.uq.scales), _p(self.partial),
+                _p(grad_base), _p(self.cluster_off), _stream()), 'pf_nuq_bucket_cluster_grad')
+            return
         if self._grad_tables is None or self._grad_tables[0] != ptrs:
             gs = self.uq.segs.copy()
             gs['src'] = ptrs
