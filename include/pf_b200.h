@@ -538,6 +538,20 @@ int pf_bn_apply_add(const float* x_dev, int64_t m, int c, const float* mean_dev,
 int pf_bn_apply_add_eval(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
                          float eps, const float* gamma_dev, const float* beta_dev, const float* res_dev, float* y_dev,
                          void* y_hi_dev, void* y_lo_dev, void* stream);
+/* channel gathers of the compact (channel-pruned) inference graph, pocketflow_b200/compact.py: NHWC viewed as
+ * [m, cin] -> [m, cout], y[:, j] = x[:, idx[j]], and 0 where idx[j] < 0 (zero padding channels); cout % 4 == 0,
+ * idx_dev 16-byte aligned.
+ *   pf_gather_channels       input fp32 (x_dev) OR split-bf16 planes (x_hi_dev / x_lo_dev); output fp32 and / or
+ *                            planes.  fp32 -> planes is the split of pf_split_bf16; planes -> planes copies the bits;
+ *                            planes -> fp32 is hi + lo.
+ *   pf_bn_apply_eval_gather  y = gather(act(bn(x))) with the moving statistics, bit-identical to pf_bn_apply_eval at
+ *                            full width followed by pf_gather_channels (mean / var / gamma / beta have cin entries). */
+int pf_gather_channels(const float* x_dev, const void* x_hi_dev, const void* x_lo_dev, int64_t m, int cin, int cout,
+                       const int32_t* idx_dev, float* y_dev, void* y_hi_dev, void* y_lo_dev, void* stream);
+int pf_bn_apply_eval_gather(const float* x_dev, int64_t m, int cin, const float* moving_mean_dev,
+                            const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev, int act,
+                            int cout, const int32_t* idx_dev, float* y_dev, void* y_hi_dev, void* y_lo_dev,
+                            void* stream);
 /* dropout (slim.dropout, mobilenet.py:369; TF 1.x nn_ops.dropout): y = (x / keep) * floor(keep + u), u in [0, 1) from
  * Philox4x32-10 keyed by (seed, rank) with counter (element index / 4 [64 bits], step [low 32 bits], stream_id);
  * mask_dev[i] <- floor(keep + u) (0 / 1).  stream_id tells the Dropout ops of one graph apart (each passes its own

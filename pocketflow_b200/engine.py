@@ -451,7 +451,8 @@ class Executor:
         for op in self.ops:
             if op in self.tc and op not in self.im2col:
                 r = self._root(op.inputs[0])
-                if r is not None and (r.op.type == 'FusedBatchNorm' or r.op in self._add_of_bn()) and r.numel % 8 == 0:
+                if r is not None and (r.op.type in ('FusedBatchNorm', 'GatherChannels') or r.op in self._add_of_bn()) \
+                        and r.numel % 8 == 0:
                     if r.op not in self.xplanes:
                         self.xplanes[r.op] = ops.Planes(r.numel, dev)
                         self.bn_need_f32[r.op] = False
@@ -465,6 +466,21 @@ class Executor:
                         continue
                     if not (c in self.tc and c not in self.im2col and (not self.train or c in self.tc_wgrad)):
                         self.bn_need_f32[bn_op] = True
+        # ---- channel gathers of a compact (channel-pruned) graph, compact.py: a GatherChannels op writes its
+        # consumer's operand planes (above); when it is the only reader of an inference-mode BN (+ activation), the BN
+        # apply writes the gathered tensor itself and the full-width BN output is never materialised
+        self.gather_idx, self.bn_gather = {}, {}
+        for op in self.ops:
+            if op.type != 'GatherChannels':
+                continue
+            self.gather_idx[op] = torch.from_numpy(np.ascontiguousarray(op.attrs['index'], np.int32)).to(dev)
+            t = op.inputs[0]
+            bn = t.op.inputs[0].op if t.op in self.fused_into else t.op
+            if bn.type == 'FusedBatchNorm' and not bn.attrs['training'] and bn not in self.bn_add \
+                    and bn not in self.xplanes and self._consumers(t) == [op] \
+                    and (t.op is bn or self._consumers(bn.output) == [t.op]) and t.op not in self.aq_index:
+                self.bn_gather[bn] = op
+        self.gather_fused = set(self.bn_gather.values())
         # ---- integer-level operands (TMA-fed kernels, SURVEY §7 hard part 1b): a <= 8-bit fake-quantized tensor is
         # exactly scale * level, and the levels are exact in bf16 — one operand plane instead of hi + lo, one MMA per
         # k-slice instead of three (two against a split gradient).  Activation side: the fused BN + ReLU + fake-quant
@@ -869,6 +885,24 @@ class Executor:
                 else:
                     with self.timed('bn_apply'):
                         ops.bn_apply_add_eval(x, m, c, mm, mv, op.attrs['epsilon'], gamma, beta, self.T(other), y_out, pl)
+            elif ty == 'FusedBatchNorm' and op in self.bn_gather:
+                gop = self.bn_gather[op]
+                x = self.T(op.inputs[0])
+                c = x.shape[-1]
+                pl = self.xplanes.get(gop)
+                with self.timed('bn_apply'):
+                    ops.bn_apply_eval_gather(x, x.numel() // c, c, st.view(op.vars['moving_mean']),
+                                             st.view(op.vars['moving_variance']), op.attrs['epsilon'],
+                                             st.view(op.vars['gamma']), st.view(op.vars['beta']),
+                                             self.fused_act.get(op, 0), self.gather_idx[gop],
+                                             self.buf[gop.output] if pl is None or self.bn_need_f32[gop] else None, pl)
+            elif ty == 'GatherChannels':
+                if op in self.gather_fused:
+                    continue                               # written by the producing BN apply
+                pl = self.xplanes.get(op)
+                with self.timed('gather'):
+                    ops.gather_channels(self.T(op.inputs[0]), self.gather_idx[op],
+                                        self.buf[op.output] if pl is None or self.bn_need_f32[op] else None, pl)
             elif ty == 'FusedBatchNorm':
                 x, y = self.T(op.inputs[0]), self.buf[op.output]
                 c = y.shape[-1]

@@ -770,6 +770,33 @@ def bn_apply_add_eval(x, m, c, mov_mean, mov_var, eps, gamma, beta, res, y=None,
                'pf_bn_apply_add_eval')
 
 
+def gather_channels(x, idx, y=None, planes=None, x_planes=None):
+    """y[..., j] = x[..., idx[j]] (0 where idx[j] < 0) over the last (channel) axis, to fp32 `y` and / or operand
+    `planes`.  The input is `x` (fp32) or, when x is None, `x_planes` = (Planes, rows m, channels cin)."""
+    cout = idx.numel()
+    if x is not None:
+        cin = x.shape[-1]
+        m = x.numel() // cin
+        xh = xl = None
+    else:
+        (xp, m, cin) = x_planes
+        xh, xl = xp.hi, xp.lo
+    _lib.check(_lib.load().pf_gather_channels(_p(x), _p(xh), _p(xl), m, cin, cout, _p(idx), _p(y),
+                                              _p(planes.hi if planes is not None else None),
+                                              _p(planes.lo if planes is not None else None), _stream()),
+               'pf_gather_channels')
+
+
+def bn_apply_eval_gather(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, idx, y=None, planes=None):
+    """gather(act(bn(x))) with the moving statistics in one launch: x is [m, c], the result [m, idx.numel()] goes to
+    fp32 `y` and / or operand `planes`"""
+    _lib.check(_lib.load().pf_bn_apply_eval_gather(_p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma),
+                                                   _p(beta), int(act), idx.numel(), _p(idx), _p(y),
+                                                   _p(planes.hi if planes is not None else None),
+                                                   _p(planes.lo if planes is not None else None), _stream()),
+               'pf_bn_apply_eval_gather')
+
+
 def dropout_fwd(x, keep_prob, seed, rank, state, y, mask, stream_id=0):
     """slim.dropout in a training pass: y = (x / keep) * mask, mask = floor(keep + u) (uint8), u from Philox4x32-10 keyed
     by (seed, rank) at the step held in `state` (int64 [2] on the device, advanced by the launch) of stream `stream_id`
