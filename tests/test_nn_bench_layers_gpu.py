@@ -7,13 +7,24 @@ PF_POISON=1, and one eager step runs with entry points of `ops` wrapped.  Each c
   * the first call of each (entry point, geometry, form, flags) is compared on exactly the operands it was given, with
     "prior" outputs (accumulate targets, moving statistics, range slots) cloned before the call:
       - batch-norm statistics: mean within 1e-6 of |mean| + std, var 1e-5 relative, rstd within one ulp of
-        fp32(1 / sqrt(fl(var + eps))), moving statistics 1e-6 of float64 from the prior, the range slot bit-exact;
+        fp32(1 / sqrt(fl(var + eps))), moving statistics 1e-6 of float64 from the prior (the mean at the scale
+        |prior| momentum + (|mean| + std)(1 - momentum), and bit-exact as the fp32 chain of the batch mean), the range
+        slot bit-exact;
       - BN apply, fake-quant, planes, levels and range slots: bit-exact against the fp32 op chain
         ((x - mean) * rstd) * gamma + beta and the quantizer's op chain (test_nn_variants_gpu);
       - BN backward: mask from that fp32 chain, dgamma / dbeta within 1e-6 of the sum of |terms| per channel, dx 1e-5
         of max|ref| on the fed fp32 statistics, planes == split(fp32 dx);
       - depthwise fwd / dgrad 1e-5 of max|ref|; wgrad against max|ref|, the sum of |terms| and an fp32 reference;
       - max-pool: y and argmax (first maximum) bit-exact, dx 1e-6; the rest float64 at 1e-5 or bit-exact.
+The weight-sparse and codebook workloads also run what their learners do besides the step (run_workload's `after`):
+      - mask rebuild: masks, weights (as uint32: -0.0 counts), backups and thresholds bit-exact against
+        oracle.ws_build_mask at the ratios passed in;
+      - codebook forward: quantized weights (and kept indices, ties to the first centroid) bit-exact against
+        oracle.nonuniform_quantize with the device codebook; quantile init: every codebook bit-exact against
+        oracle.nuq_quantile_init of the normalised tensor, entries past 2^bits zero; order statistics (pf_select_desc)
+        bit-exact against a sort; codebook gradient within 1e-6 of each centroid's sum of |terms| of float64
+        oracle.nuq_grads, and the same bits on a second call.
+      Each of them must cover every tensor its object holds.
 Every public callable of `ops` is wrapped: the test fails when the step calls one that is neither a tensor-core entry
 point (test_tc_bench_layers_gpu), nor checked here, nor in EXEMPT with its reason."""
 import os
@@ -32,7 +43,7 @@ if ROOT not in sys.path:
 from oracle import pf_oracle as O  # noqa: E402
 from pocketflow_b200 import ops  # noqa: E402
 from test_nn_variants_gpu import bn_chain, fq_chain, pool_dx_ref, pool_ref, split_planes  # noqa: E402
-from test_tc_bench_layers_gpu import Recorder as TcRecorder, conv64, geom, run_workload  # noqa: E402
+from test_tc_bench_layers_gpu import Recorder as TcRecorder, after_step, conv64, geom, run_workload  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0')
@@ -56,11 +67,15 @@ EXEMPT = {
     'dwconv_wgrad_workspace_floats': 'host-side query',
     'decode_ordered': 'host-side decoding',
     'flat_works': 'host-side work table',
+    'percentile_rank_desc': 'host-side rank arithmetic',
+    'ws_rank_desc': 'host-side rank arithmetic',
+    'UniformWeightQuantizer.ranges': 'host-side copy of the range slots',
     'minmax_reset': 'fills the range slots with the empty range; every slot it resets is checked where it is consumed',
     'launch_count': 'host-side counter',
     'launch_count_reset': 'host-side counter',
     'UniformWeightQuantizer.reset_ranges': 'part of UniformWeightQuantizer.forward, whose output is checked',
-    'UniformWeightQuantizer.minmax': 'part of UniformWeightQuantizer.forward, whose output is checked',
+    'UniformWeightQuantizer.minmax': 'part of UniformWeightQuantizer.forward and of the codebook forward and '
+                                     'quantile init, whose outputs are checked',
     'UniformWeightQuantizer.quantize': 'part of UniformWeightQuantizer.forward, whose output is checked',
 }
 CLASSES = ('UniformWeightQuantizer', 'CodebookWeightQuantizer', 'MaskBuilder', 'TcWeights', 'TcWeightsBatch',
@@ -110,10 +125,12 @@ def relerr(got, ref, scale=None):
 class NnRecorder:
     """wraps every public callable of `ops`; see the module docstring"""
 
-    def __init__(self, monkeypatch):
+    def __init__(self, monkeypatch, expect=None):
+        """expect: {check tag: tensors it must cover, or None where the tag only has to appear}"""
         self.checked, self.worst, self.calls, self.called, self.fail = set(), {}, 0, set(), []
         self.wgrad_notes = []
         self.oracle_done, self.quant_seen = False, False
+        self.expect, self.covered, self._codebooks = dict(expect or {}), {}, {}
         for name in dir(ops):
             obj = getattr(ops, name)
             if name.startswith('_') or isinstance(obj, type) or not callable(obj) or \
@@ -148,10 +165,16 @@ class NnRecorder:
         if not err <= bar:
             self.fail.append((tag, err, bar))
 
-    def _exact(self, tag, ok):
+    def _exact(self, tag, ok, where=None):
         self.worst.setdefault(tag, 0.0)
         if not ok:
-            self.fail.append((tag, 'not bit-exact', None))
+            self.fail.append((tag, 'not bit-exact', where))
+
+    def _per_tensor(self, results):
+        """results: {tag: [bit-exact per tensor]}; one entry per tag, naming the tensors that differ"""
+        for tag, oks in results.items():
+            bad = [i for i, ok in enumerate(oks) if not ok]
+            self._exact(tag, not bad, 'tensors %s of %d' % (bad, len(oks)) if bad else None)
 
     # ---------------------------------------------------------------------------------------------- batch-norm
     def _stats(self, fn, name, x, m, c, eps, mom, mean, var, rstd, mm, mv, gamma=None, beta=None, act=0, slot=None,
@@ -178,9 +201,16 @@ class NnRecorder:
         ulp = (torch.nextafter(r32, torch.full_like(r32, float('inf'))) - r32).double()
         self._exact('bn stats rstd (1 ulp)', bool(((rstd.double() - r64).abs() <= ulp).all()))
         if prior is not None:
-            om = 1.0 - float(np.float32(mom))
-            e = max(relerr(mm, prior[0].double() * float(np.float32(mom)) + m64 * om),
-                    relerr(mv, prior[1].double() * float(np.float32(mom)) + xd.var(0, unbiased=True) * om))
+            # moving mean: the fp32 op chain of the batch mean it was given (checked above), bit for bit; and against
+            # float64 per channel at the mean's own scale carried through the update, |prior| mom + (|mean| + std) om
+            # (a bar of max|moving mean| fails where every batch mean is small beside its std: ResNet-20 at batch 256)
+            mo, om32 = np.float32(mom), np.float32(1) - np.float32(mom)
+            self._exact('bn stats moving mean (fp32 chain)',
+                        np.array_equal(mm.cpu().numpy(), prior[0].cpu().numpy() * mo + mean.cpu().numpy() * om32))
+            om = 1.0 - float(mo)
+            scale = prior[0].double().abs() * float(mo) + (m64.abs() + v64.sqrt()) * om
+            e = max(((mm.double() - (prior[0].double() * float(mo) + m64 * om)).abs() / scale.clamp_min(1e-30)).max()
+                    .item(), relerr(mv, prior[1].double() * float(mo) + xd.var(0, unbiased=True) * om))
             self._note('bn stats moving', e, 1e-6)
         if pslot is not None:
             y = bn_chain(x.reshape(-1)[:m * c].view(m, c), mean, rstd, gamma, beta, act)
@@ -641,6 +671,140 @@ class NnRecorder:
             ref = O.uq_ste_grad(g, a, q.bits[i]).reshape(pre[i].shape)
             self._exact('weight quantizer STE', np.array_equal(grads[i].cpu().numpy(), ref))
 
+    # ---------------------------------------------------------------------------------------------- codebooks
+    def _cover(self, tag, n, held):
+        """one run of a per-tensor check: n tensors compared of the `held` its object holds"""
+        self.covered.setdefault(tag, []).append((n, held))
+
+    @staticmethod
+    def _codebook(q, i):
+        """the whole device codebook of tensor i: its store-resident `clusters` variable, or its private table row"""
+        return q.cluster_views[i] if q.cluster_views is not None else q.clusters[i]
+
+    def _quantile_ref(self, q, i):
+        """oracle.nuq_quantile_init of tensor i's normalised weights from ONE sort: the elements at the oracle's
+        percentile_index positions of the descending order (16 full sorts of a 2.36M tensor per kernel would dominate
+        the run; the shortcut is cross-checked against the oracle itself in the quantile-init check)"""
+        key = (id(q), i)
+        if key not in self._codebooks:
+            xn = O.uq_scale(q.srcs[i].cpu().numpy().reshape(-1), None)[0]
+            k = 1 << q.uq.bits[i]
+            desc = np.sort(xn)[::-1]
+            self._codebooks[key] = desc[[O.percentile_index(xn.size, (j + 1) * 100 / (k + 1)) for j in range(k)]]
+        return self._codebooks[key]
+
+    def _c_select_desc(self, fn, tensors, queries):
+        out = fn(tensors, queries)
+        if self._first(('select_desc', tuple(t.numel() for t in tensors), tuple(queries))):
+            got, desc, ok = out.cpu().numpy(), {}, True
+            for qi, (ti, rank) in enumerate(queries):
+                if ti not in desc:
+                    desc[ti] = np.sort(tensors[ti].cpu().numpy().reshape(-1))[::-1]
+                ok = ok and got[qi] == desc[ti][rank]
+            self._exact('order statistics (select_desc)', ok)
+        return out
+
+    def _m_CodebookWeightQuantizer_quantile_values(self, fn, q):
+        vals = fn(q)
+        if self._first(('CodebookWeightQuantizer.quantile_values', id(q))):
+            assert not q.use_buckets, 'bucketed codebooks are not benchmarked (test_nuq_buckets_gpu checks them)'
+            oks = [np.array_equal(v.view(np.uint32), self._quantile_ref(q, i).view(np.uint32))
+                   for i, v in enumerate(vals)]
+            self._per_tensor({'codebook quantile values': oks})
+            self._cover('codebook quantile values', len(oks), len(q.srcs))
+        return vals
+
+    def _m_CodebookWeightQuantizer_quantile_init(self, fn, q):
+        fn(q)
+        if not self._first(('CodebookWeightQuantizer.quantile_init', id(q))):
+            return
+        torch.cuda.synchronize()
+        assert not q.use_buckets, 'bucketed codebooks are not benchmarked (test_nuq_buckets_gpu checks them)'
+        res = {'codebook quantile init': [], 'codebook quantile init: entries past 2^bits zero': []}
+        for i in range(len(q.srcs)):
+            k = 1 << q.uq.bits[i]
+            cb = self._codebook(q, i).cpu().numpy().view(np.uint32)
+            res['codebook quantile init'].append(np.array_equal(cb[:k], self._quantile_ref(q, i).view(np.uint32)))
+            res['codebook quantile init: entries past 2^bits zero'].append(not cb[k:].any())
+        self._per_tensor(res)
+        self._cover('codebook quantile init', len(res['codebook quantile init']), len(q.srcs))
+        sizes = [s.numel() for s in q.srcs]
+        for i in sorted({int(np.argmin(sizes)), int(np.argmax(sizes))}):
+            xn = O.uq_scale(q.srcs[i].cpu().numpy(), None)[0]
+            self._exact('codebook quantile init: one sort == oracle (smallest, largest tensor)',
+                        np.array_equal(self._quantile_ref(q, i), O.nuq_quantile_init(xn, 1 << q.uq.bits[i])))
+        self._codebooks = {key: v for key, v in self._codebooks.items() if key[0] != id(q)}
+
+    def _m_CodebookWeightQuantizer_forward(self, fn, q):
+        fn(q)
+        if not self._first(('CodebookWeightQuantizer.forward', id(q))):
+            return
+        torch.cuda.synchronize()
+        assert not q.use_buckets, 'bucketed codebooks are not benchmarked (test_nuq_buckets_gpu checks them)'
+        res = {'codebook forward': []}
+        for i, (src, dst) in enumerate(zip(q.srcs, q.dsts)):
+            bits = q.uq.bits[i]
+            ref, _, idx = O.nonuniform_quantize(src.cpu().numpy(), bits,
+                                                clusters=self._codebook(q, i)[:1 << bits].cpu().numpy())
+            res['codebook forward'].append(np.array_equal(dst.cpu().numpy().view(np.uint32), ref.view(np.uint32)))
+            if q.idx is not None:           # ties go to the first centroid (tf.argmin)
+                o = q.idx_offsets[i]
+                res.setdefault('codebook forward kept index', []).append(
+                    np.array_equal(q.idx[o:o + src.numel()].cpu().numpy(), idx.reshape(-1).astype(np.uint8)))
+        self._per_tensor(res)
+        self._cover('codebook forward', len(res['codebook forward']), len(q.srcs))
+
+    def _m_CodebookWeightQuantizer_cluster_grad(self, fn, q, grads, grad_base):
+        first = self._first(('CodebookWeightQuantizer.cluster_grad', id(q)))
+        fn(q, grads, grad_base)
+        if not first:
+            return
+        torch.cuda.synchronize()
+        assert not q.use_buckets, 'bucketed codebooks are not benchmarked (test_nuq_buckets_gpu checks them)'
+        outs = [grad_base[int(o):int(o) + (1 << b)].clone() for o, b in zip(q.cluster_off.cpu().numpy(), q.uq.bits)]
+        scales = q.uq.scales.cpu().numpy()
+        worst, n = 0.0, 0
+        for i, g in enumerate(grads):
+            k, gn = 1 << q.uq.bits[i], g.cpu().numpy().reshape(-1)
+            idx = q.idx[q.idx_offsets[i]:q.idx_offsets[i] + gn.size].cpu().numpy().astype(np.int64)
+            alpha = scales[int(q.uq.segs[i]['bucket0'])]
+            ref = O.nuq_grads(gn, idx, k, alpha)[1].astype(np.float64)
+            mag = np.bincount(idx, weights=np.abs((gn * alpha).astype(np.float32).astype(np.float64)), minlength=k)
+            err = np.abs(outs[i].cpu().numpy().astype(np.float64) - ref) / np.maximum(mag, 1e-30)
+            worst = max(worst, err.max())
+            n += 1
+        self._note('codebook gradient / sum|terms|', worst, 1e-6)
+        self._cover('codebook gradient', n, len(q.srcs))
+        fn(q, grads, grad_base)            # the reduction runs in a fixed order: a second call gives the same bits
+        torch.cuda.synchronize()
+        self._exact('codebook gradient run to run', all(
+            torch.equal(grad_base[int(o):int(o) + t.numel()].view(torch.int32), t.view(torch.int32))
+            for o, t in zip(q.cluster_off.cpu().numpy(), outs)))
+
+    # ---------------------------------------------------------------------------------------------- masks
+    def _m_MaskBuilder_build(self, fn, mb, prune_ratios):
+        first = self._first(('MaskBuilder.build', id(mb), tuple(float(r) for r in prune_ratios)))
+        if first:
+            torch.cuda.synchronize()
+            pre = [(w.cpu().numpy(), b.cpu().numpy(), m.cpu().numpy()) for w, b, m in zip(mb.ws, mb.bkups, mb.masks)]
+        ranks = fn(mb, prune_ratios)
+        if not first:
+            return ranks
+        torch.cuda.synchronize()
+        u32 = lambda t: t.cpu().numpy().view(np.uint32)        # noqa: E731
+        res = {'mask rebuild mask': [], 'mask rebuild weights': [], 'mask rebuild backups': [],
+               'mask rebuild thresholds': []}
+        thr = u32(mb.thr)
+        for i, ((w0, b0, m0), r) in enumerate(zip(pre, prune_ratios)):
+            rw, rb, rm, rt = O.ws_build_mask(w0, b0, m0, r)
+            res['mask rebuild mask'].append(np.array_equal(u32(mb.masks[i]), rm.view(np.uint32)))
+            res['mask rebuild weights'].append(np.array_equal(u32(mb.ws[i]), rw.view(np.uint32)))
+            res['mask rebuild backups'].append(np.array_equal(u32(mb.bkups[i]), rb.view(np.uint32)))
+            res['mask rebuild thresholds'].append(thr[i] == np.float32(rt).view(np.uint32))
+        self._per_tensor(res)
+        self._cover('mask rebuild', len(res['mask rebuild mask']), len(mb.ws))
+        return ranks
+
     # ---------------------------------------------------------------------------------------------- tc operands
     def _check_tc_weights(self, tw, w, seg):
         """forward / dgrad copies of one kernel against the fp32 tensor they stand for (pf_conv2d_tc_prep_*)"""
@@ -787,17 +951,62 @@ class NnRecorder:
             label, self.calls, len(self.checked), {k: '%.2e' % v for k, v in sorted(self.worst.items())}, secs, peak_gb))
         for g, e, em, e32 in self.wgrad_notes:
             print('  dwconv wgrad %s: %.2e of max|ref|, %.2e of max sum|terms|, fp32 reference %.2e' % (g, e, em, e32))
+        for tag, runs in sorted(self.covered.items()):
+            print('  %s: %s tensors' % (tag, ', '.join('%d of %d' % r for r in runs)))
         checked_here = {n[3:] for n in dir(self) if n.startswith('_c_')} | \
             {n[3:].replace('_', '.', 1) for n in dir(self) if n.startswith('_m_')}
         unknown = self.called - checked_here - set(TcRecorder.NAMES) - set(EXEMPT)
+        for what, v in (('unchecked entry points', sorted(unknown)), ('failed checks', self.fail)):
+            if v:
+                print('  %s: %s' % (what, v))
         assert not unknown, 'the step calls entry points that are neither checked nor exempt: %s' % sorted(unknown)
         assert not self.fail, self.fail
+        # every per-tensor check covered every tensor its object holds, and each check the plan calls for ran
+        assert all(n == held for runs in self.covered.values() for n, held in runs), self.covered
+        missing = {t: n for t, n in self.expect.items()
+                   if (t not in self.worst if n is None else
+                       not self.covered.get(t) or any(r[0] != n for r in self.covered[t]))}
+        assert not missing, ('checks the plan calls for that did not run (over every tensor)', missing, self.covered)
         # one activation tensor per workload through the numpy oracle itself (when the workload quantizes activations)
         assert self.oracle_done or not self.quant_seen, 'no activation tensor went through the numpy oracle'
         assert len(self.checked) >= 10
 
 
-@pytest.mark.parametrize('workload,batch', [('resnet50_uq8_dst_b128', 128), ('mobilenet_cpg50_b256', 256),
-                                            ('lenet_uq8_b128', 128)])
-def test_bench_layers_besides_the_tc_convs(workload, batch, monkeypatch):
-    run_workload(workload, batch, monkeypatch, NnRecorder)
+def expected_checks(workload, lrn):
+    """the checks the learner's plan calls for: {tag: tensors each run must cover, or None where the tag only has to
+    appear} — the weight-sparse mask rebuild over every maskable variable, the codebook checks over every quantized
+    kernel, and the producer of each first layer that computes its own operand (the stem's folded weight gradient
+    included)"""
+    import bench
+    ex = lrn.sess_train
+    want = {}
+    if bench.WORKLOADS[workload][2] == 'weight-sparse':
+        want['mask rebuild'] = len(ex.maskable)
+    if isinstance(ex.wq, ops.CodebookWeightQuantizer):
+        for tag in ('codebook forward', 'codebook quantile values', 'codebook quantile init'):
+            want[tag] = len(ex.wq_ops)
+        if ex.train_clusters:
+            want['codebook gradient'] = len(ex.wq_ops)
+    for e in (ex, ex.teacher):
+        for im in (e.im2col.values() if e is not None else ()):
+            if im['compute']:
+                want['s2d_planes' if im['mode'] == 's2d' else ('im2col_planes' if im['planes'] else 'im2col')] = None
+            if e.train and 'pair' in im:
+                want['fold_diag_blocks / sum|terms|'] = None
+    return want
+
+
+# (workload, batch, flag overrides): the benchmarked workloads at their batch, and the codebook learner also in the
+# 'both' optimisation mode, where the codebook gradient runs
+RUNS = [('resnet50_uq8_dst_b128', 128, None), ('mobilenet_cpg50_b256', 256, None), ('lenet_uq8_b128', 128, None),
+        ('resnet50_ws50_dst_b128', 128, None), ('resnet50_nuq4_dst_b128', 128, None),
+        ('resnet50_nuq4_dst_b128', 128, {'nuql_opt_mode': 'both'}), ('resnet20_uq8_dst_b256', 256, None),
+        ('resnet20_ws50_dst_b256', 256, None)]
+
+
+@pytest.mark.parametrize('workload,batch,flags', [
+    pytest.param(w, b, f, id='%s-%d' % (w, b) + ''.join('-%s' % v for _, v in sorted((f or {}).items())))
+    for w, b, f in RUNS])
+def test_bench_layers_besides_the_tc_convs(workload, batch, flags, monkeypatch):
+    run_workload(workload, batch, monkeypatch, lambda mp, lrn: NnRecorder(mp, expected_checks(workload, lrn)),
+                 flags=flags, after=after_step(workload))

@@ -1,10 +1,10 @@
 """Every tensor-core convolution of one training step of the benchmarked workloads, at the benchmarked batch, against
 float64.
 
-bench.py measures resnet50_uq8_dst_b128 at batch 128 (DESIGN.md §8); the other step tests run ResNet-50 at batch 2,
-where no CTA of the persistent kernels ever sees a second tile.  Here the learner is built at the benchmarked batch
-under PF_POISON=1 (activation and scratch buffers start as NaN) and one eager step runs with the tensor-core entry
-points of `ops` wrapped: each call is passed through unchanged, then
+bench.py measures its workloads at batch 128 (ResNet-50) and 256 (ResNet-20, MobileNet) (DESIGN.md §8); the other step
+tests run ResNet-50 at batch 2, where no CTA of the persistent kernels ever sees a second tile.  Here the learner of a
+workload is built at the benchmarked batch under PF_POISON=1 (activation and scratch buffers start as NaN) and one
+eager step runs with the tensor-core entry points of `ops` wrapped: each call is passed through unchanged, then
   * its output must be finite, and its launch plan (pf_conv2d_tc_last_plan) is collected;
   * the first call of each (entry point, geometry, operand form, epilogue) is compared with a float64 convolution of
     exactly the operands it was fed — split planes as hi + lo, activation levels as scale x level, weight levels as
@@ -106,9 +106,10 @@ class Recorder:
     NAMES = ('conv2d_tc_fwd', 'conv2d_tc_fwd_planes', 'conv2d_tc_fwd_ex', 'conv2d_tc_dgrad', 'conv2d_tc_dgrad_planes',
              'conv2d_tc_dgrad_ex', 'conv2d_tc_wgrad', 'conv2d_tc_wgrad_planes', 'conv2d_tc_wgrad_ex')
 
-    def __init__(self, monkeypatch, min_calls):
+    def __init__(self, monkeypatch, min_calls, fwd_geoms=()):
+        """fwd_geoms: geometries that must each make a forward call"""
         self.plans, self.checked, self.worst, self.calls, self.max_tiles = {}, set(), {}, 0, 0
-        self.min_calls = min_calls
+        self.min_calls, self.fwd_geoms, self.fwd_seen = min_calls, set(fwd_geoms), set()
         self.over = []                 # checks above the DESIGN §6 bar: (key, error, error of an fp32 GEMM)
         orig_act, orig_wt = ops.tc_act, ops.tc_wt
 
@@ -138,6 +139,8 @@ class Recorder:
             plan = ops.conv2d_tc_last_plan()
             self.plans.setdefault(plan_key(plan), '%s %s' % (name, geom(d)))
             self.calls += 1
+            if pass_ == 0:
+                self.fwd_seen.add(geom(d))
             self.max_tiles = max(self.max_tiles, plan['tiles'])
             out = args[4] if pass_ == 0 else args[3]
             if out is not None:
@@ -258,6 +261,8 @@ class Recorder:
               'at most %d tiles in one launch; %.0f s, peak %.1f GB' % (
                   label, self.calls, len(self.checked), {k: '%.2e' % v for k, v in sorted(self.worst.items())},
                   len(self.plans), self.max_tiles, secs, peak_gb))
+        for k, first in sorted(self.plans.items()):
+            print('  plan %s: first %s' % (' '.join('%s=%s' % f for f in zip(KEY_FIELDS, k)), first))
         for key, err, err32, errm in self.over:
             print('  above the bar: %s %s: %.2e of max|ref| (an fp32 GEMM of the same operands: %.2e); %.2e of max '
                   'sum of |terms|' % (key[0], key[1:], err, err32, errm))
@@ -268,22 +273,60 @@ class Recorder:
         bad = [(k, e, m) for k, e, _, m in self.over if not (k[0].startswith('conv2d_tc_wgrad') and m <= 2e-5)]
         assert not bad, bad
         assert self.calls >= self.min_calls and len(self.checked) >= 3
+        assert not self.fwd_geoms - self.fwd_seen, ('planned tensor-core convolutions that made no forward call',
+                                                    sorted(self.fwd_geoms - self.fwd_seen))
         assert self.max_tiles >= 3 * torch.cuda.get_device_properties(0).multi_processor_count
         outside = {k: v for k, v in self.plans.items() if k not in REQUIRED}
         assert not outside, 'plans the variant sweep does not reach: %s' % {
             str(dict(zip(KEY_FIELDS, k))): v for k, v in outside.items()}
 
 
-def run_workload(workload, batch, monkeypatch, recorder):
-    """One eager step of a bench workload at `batch` under PF_POISON=1, with recorder(monkeypatch) wrapping entry
-    points of `ops` from just before the step; then recorder.finish(label, seconds, peak GB) prints and asserts."""
+def tc_recorder(monkeypatch, lrn):
+    """a Recorder expecting what the executors planned: every convolution they put on the tensor cores, student and
+    teacher, makes at least one forward call, at its own geometry (the first layer's lowered one)"""
+    geoms = []
+    for ex in (lrn.sess_train, lrn.sess_train.teacher):
+        for op in (set(ex.tc) | set(ex.im2col) if ex is not None else ()):
+            geoms.append(geom(ex.im2col[op]['d1'] if op in ex.im2col else ex.desc[op]))
+    return Recorder(monkeypatch, len(geoms), set(geoms))
+
+
+def ws_prune(lrn):
+    """two mask rebuilds inside the pruning window (steps 6 and 8 of 20): the second finds the weights the first pruned
+    at zero under a zero mask, so their backups must be kept"""
+    lrn.nb_iters_train = 20
+    for step in (6, 8):
+        lrn.sess_train.step_count = step
+        lrn.prune()
+
+
+def after_step(workload):
+    """what runs after the step besides it, by learner: the weight-sparse mask rebuild, and the codebook quantile init
+    (which the learner first ran at construction, before any entry point was wrapped)"""
+    import bench
+    learner = bench.WORKLOADS[workload][2]
+    if learner == 'weight-sparse':
+        return ws_prune
+    if learner == 'non-uniform':
+        return lambda lrn: lrn.cluster_init()
+    return None
+
+
+def run_workload(workload, batch, monkeypatch, recorder, flags=None, after=None):
+    """One eager step of a bench workload at `batch` under PF_POISON=1, with recorder(monkeypatch, learner) wrapping
+    entry points of `ops` from just before the step; after(learner), if given, runs next with the recorder still
+    installed; then recorder.finish(label, seconds, peak GB) prints and asserts.  flags: overrides of the workload's
+    flags."""
     import bench
     monkeypatch.setenv('PF_POISON', '1')
+    if flags:
+        net, size, learner, over, descr = bench.WORKLOADS[workload]
+        monkeypatch.setitem(bench.WORKLOADS, workload, (net, size, learner, dict(over, **flags), descr))
     t0 = time.time()
     torch.cuda.reset_peak_memory_stats()
     lrn = bench.build_learner(workload, 1, batch)
     ex = lrn.sess_train
-    rec = recorder(monkeypatch)
+    rec = recorder(monkeypatch, lrn)
     images, labels = lrn.iterator_train.next_batch()
     ex.buf[lrn.images].copy_(images)
     ex.buf[lrn.labels].copy_(labels)
@@ -291,8 +334,12 @@ def run_workload(workload, batch, monkeypatch, recorder):
     torch.cuda.synchronize()
     losses = ex.fetch_losses()
     assert np.isfinite(losses['loss']), losses
+    if after is not None:
+        after(lrn)
+        torch.cuda.synchronize()
+    label = '%s at batch %d' % (workload, batch) + ''.join(' %s=%s' % kv for kv in sorted((flags or {}).items()))
     try:
-        rec.finish('%s at batch %d' % (workload, batch), time.time() - t0, torch.cuda.max_memory_allocated() / 2 ** 30)
+        rec.finish(label, time.time() - t0, torch.cuda.max_memory_allocated() / 2 ** 30)
     finally:
         del lrn, ex, rec
         gc.collect()
@@ -300,8 +347,14 @@ def run_workload(workload, batch, monkeypatch, recorder):
 
 
 def test_resnet50_uq8_bench_layers_at_batch_128(monkeypatch):
-    run_workload('resnet50_uq8_dst_b128', 128, monkeypatch, lambda mp: Recorder(mp, 100))
+    run_workload('resnet50_uq8_dst_b128', 128, monkeypatch, tc_recorder)
 
 
 def test_mobilenet_cpg50_bench_layers_at_batch_256(monkeypatch):
-    run_workload('mobilenet_cpg50_b256', 256, monkeypatch, lambda mp: Recorder(mp, 30))
+    run_workload('mobilenet_cpg50_b256', 256, monkeypatch, tc_recorder)
+
+
+@pytest.mark.parametrize('workload,batch', [('resnet50_ws50_dst_b128', 128), ('resnet50_nuq4_dst_b128', 128),
+                                            ('resnet20_uq8_dst_b256', 256), ('resnet20_ws50_dst_b256', 256)])
+def test_bench_tc_convs(workload, batch, monkeypatch):
+    run_workload(workload, batch, monkeypatch, tc_recorder, after=after_step(workload))
