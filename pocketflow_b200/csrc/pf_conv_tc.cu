@@ -315,7 +315,7 @@ conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __res
         if (PLANES) fence_proxy_async_smem();   // cp.async writes -> visible to the tensor core (async proxy)
         const uint32_t a_hi = smem_u32(smem_a + (size_t)s * 2 * a_bytes) + (uint32_t)wg * 64 * 128, a_lo = a_hi + a_bytes;
         const uint32_t bh = smem_u32(smem_b + (size_t)(p.b_stationary ? ks : (int)s) * 2 * b_bytes), bl = bh + b_bytes;
-        wg_mma_stage<BN, 0>(acc, a_hi, a_lo, bh, bl, 2, 2, 32, 32, 16, 1024, 16, 1024);
+        wg_mma_stage<BN, 0, 2, 2>(acc, a_hi, a_lo, bh, bl, 32, 32, 16, 1024, 16, 1024);
         wgmma_wait<1>(acc);                      // the previous stage's MMAs have completed: release it
         if (ks > 0) {
           __syncwarp();
@@ -492,7 +492,7 @@ conv_tc_wgrad_persist_kernel(const __nv_bfloat16* __restrict__ x_hi, const __nv_
         const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
         const uint32_t a_hi = base + (uint32_t)wg * 1024u, a_lo = a_hi + a_bytes, bh = base + 2 * a_bytes, bl = bh + b_bytes;
         // MN-major: LBO = stride between 64-wide MN blocks, SBO = stride between 8-pixel groups; 16 pixels per MMA
-        wg_mma_stage<BN, 1>(acc, a_hi, a_lo, bh, bl, 2, 2, 2 * sbo_a, 2 * sbo_b, 1024, sbo_a, 1024, sbo_b);
+        wg_mma_stage<BN, 1, 2, 2>(acc, a_hi, a_lo, bh, bl, 2 * sbo_a, 2 * sbo_b, 1024, sbo_a, 1024, sbo_b);
         wgmma_wait<1>(acc);
         if (ks > 0) {
           __syncwarp();

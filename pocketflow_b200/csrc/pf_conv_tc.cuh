@@ -42,11 +42,13 @@ inline int env_int(const char* name, int dflt) {
 int tc_geom(const pf_conv_desc* d, TcGeom* g, const char* who);
 
 // ---------------------------------------------------------------------------------------------------------
-// Main loop and epilogue warps.  Warps 0-7 of every tensor-core kernel are two warpgroups: warpgroup g issues the
-// wgmma of GEMM rows [64 g, 64 g + 64) of the 128 x BN tile into registers; at the end of a tile both write their
-// accumulators into one fp32 tile in shared memory (row pitch BN + 4 floats), and the same 8 warps then run the
-// epilogue from there: warp w owns rows [32 (w % 4), 32 (w % 4) + 32) and every other 32-column chunk starting at
-// chunk w / 4.  The producers (cp.async warps or the TMA thread) keep filling the next tile's stages meanwhile.
+// Main loop and epilogue warps.  Warps 0-7 of every tensor-core kernel are two warpgroups.  In the cooperative kernels
+// (cp.async-fed, TMA wgrad) warpgroup g issues the wgmma of GEMM rows [64 g, 64 g + 64) of the 128 x BN tile into
+// registers; at the end of a tile both write their accumulators into one fp32 tile in shared memory (row pitch BN + 4
+// floats), and the same 8 warps then run the epilogue from there: warp w owns rows [32 (w % 4), 32 (w % 4) + 32) and
+// every other 32-column chunk starting at chunk w / 4.  The producers (cp.async warps or the TMA thread) keep filling
+// the next tile's stages meanwhile.  The TMA fwd / dgrad kernel is a ping-pong instead (pf_conv_tma.cu): each
+// warpgroup owns whole tiles and runs their epilogue alone, under the other warpgroup's MMAs.
 constexpr int kMmaWarps = 8;
 constexpr int kMaxBN = 128;                                    // 64 accumulator registers per thread and warpgroup
 __host__ __device__ constexpr int acc_pitch(int BN) { return BN + 4; }
@@ -54,23 +56,31 @@ __host__ __device__ constexpr int acc_tile_bytes(int BN) { return TM * acc_pitch
 // accumulator tile + per-warp row-offset and J tables
 __host__ __device__ constexpr int epi_fixed_bytes(int BN) { return 1024 + acc_tile_bytes(BN) + kMmaWarps * 32 * (8 + 4) + 256; }
 
+// The MMAs of one 16-wide k-slice of one m64 row block:  A0 B0 (+ A0 B1 when NB == 2) (+ A1 B0 when NA == 2)  of the
+// bf16 planes (hi / lo, or integer levels).  The plane counts are template parameters: a run-time test between two
+// wgmmas makes ptxas end the chain there and re-arm the accumulator registers with an injected warpgroup.arrive (C7519).
+template <int BN, int TMN, int NA, int NB>
+__device__ __forceinline__ void wg_mma_kslice(float (&acc)[BN / 2], uint64_t da0, uint64_t da1, uint64_t db0,
+                                              uint64_t db1) {
+  Wgmma<BN>::template mma<TMN, TMN>(acc, da0, db0);
+  if (NB == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, da0, db1);
+  if (NA == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, da1, db0);
+}
+
 // One k-stage of MMAs of warpgroup `wg` (wtid = thread index inside the warpgroup is implied): per 16-wide k-slice
-// the products  A0 B0 (+ A0 B1 when nb == 2) (+ A1 B0 when na == 2)  of the bf16 planes (hi / lo, or integer levels).
-// a0 / a1 / b0 / b1 are the shared-memory addresses of the planes; a_kstep / b_kstep the byte step of one 16-wide
-// k-slice; lbo / sbo the descriptor strides.
-template <int BN, int TMN>
+// the plane products of wg_mma_kslice.  a0 / a1 / b0 / b1 are the shared-memory addresses of the planes; a_kstep /
+// b_kstep the byte step of one 16-wide k-slice; lbo / sbo the descriptor strides.
+template <int BN, int TMN, int NA, int NB>
 __device__ __forceinline__ void wg_mma_stage(float (&acc)[BN / 2], uint32_t a0, uint32_t a1, uint32_t b0, uint32_t b1,
-                                             int na, int nb, uint32_t a_kstep, uint32_t b_kstep, uint32_t lbo_a,
-                                             uint32_t sbo_a, uint32_t lbo_b, uint32_t sbo_b) {
+                                             uint32_t a_kstep, uint32_t b_kstep, uint32_t lbo_a, uint32_t sbo_a,
+                                             uint32_t lbo_b, uint32_t sbo_b) {
   wgmma_fence();
 #pragma unroll
-  for (int kk = 0; kk < BK / 16; ++kk) {
-    const uint64_t da0 = make_smem_desc(a0 + kk * a_kstep, lbo_a, sbo_a);
-    const uint64_t db0 = make_smem_desc(b0 + kk * b_kstep, lbo_b, sbo_b);
-    Wgmma<BN>::template mma<TMN, TMN>(acc, da0, db0);
-    if (nb == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, da0, make_smem_desc(b1 + kk * b_kstep, lbo_b, sbo_b));
-    if (na == 2) Wgmma<BN>::template mma<TMN, TMN>(acc, make_smem_desc(a1 + kk * a_kstep, lbo_a, sbo_a), db0);
-  }
+  for (int kk = 0; kk < BK / 16; ++kk)
+    wg_mma_kslice<BN, TMN, NA, NB>(acc, make_smem_desc(a0 + kk * a_kstep, lbo_a, sbo_a),
+                                   make_smem_desc(a1 + kk * a_kstep, lbo_a, sbo_a),
+                                   make_smem_desc(b0 + kk * b_kstep, lbo_b, sbo_b),
+                                   make_smem_desc(b1 + kk * b_kstep, lbo_b, sbo_b));
   wgmma_commit();
 }
 
@@ -233,6 +243,21 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
   if (EXTRA == 2) asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// the epilogue of one warp over 32 rows of the accumulator tile starting at `acc`, 32-column chunks c_begin,
+// c_begin + c_step, ...: picks the residual / accumulate path (none, registers, cp.async ring of depth 2 or 4)
+template <int AFF>
+__device__ __forceinline__ void epilogue_rows(const float* acc, int c_begin, int c_step, long long my_row_off,
+                                              long long* rowoff, float* __restrict__ out, const float* __restrict__ extra,
+                                              const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
+                                              int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
+                                              const float* aff_tab, int ring_depth) {
+  const int pitch = acc_pitch(BN);
+  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else if (extra && ring) epilogue_tile_t<2, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else if (extra) epilogue_tile_t<1, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  else epilogue_tile_t<0, AFF>(acc, pitch, my_row_off, rowoff, out, nullptr, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+}
+
 // the epilogue of warp `ew` (0..7) of the MMA warps: rows 32 (ew % 4) .., chunks ew / 4, ew / 4 + 2, ...
 template <int AFF>
 __device__ __forceinline__ void epilogue_tile_a(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
@@ -240,13 +265,8 @@ __device__ __forceinline__ void epilogue_tile_a(const float* acc_s, int ew, long
                                                 const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
                                                 int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
                                                 const float* aff_tab = nullptr, int ring_depth = kRingDepth) {
-  const int pitch = acc_pitch(BN);
-  const float* acc = acc_s + (size_t)(32 * (ew & 3)) * pitch;
-  const int c_begin = 32 * (ew >> 2), c_step = 64;
-  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra && ring) epilogue_tile_t<2, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra) epilogue_tile_t<1, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else epilogue_tile_t<0, AFF>(acc, pitch, my_row_off, rowoff, out, nullptr, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  epilogue_rows<AFF>(acc_s + (size_t)(32 * (ew & 3)) * acc_pitch(BN), 32 * (ew >> 2), 64, my_row_off, rowoff, out,
+                     extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, aff_tab, ring_depth);
 }
 __device__ __forceinline__ void epilogue_tile(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
                                               float* __restrict__ out, const float* __restrict__ extra,

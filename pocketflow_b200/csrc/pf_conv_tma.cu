@@ -6,9 +6,9 @@
 //   * the NHWC operand (x in fwd / wgrad, dy in dgrad) is fetched by ONE im2col-mode TMA load per k-stage and plane
 //     (128 filter-window positions x 64 channels of one tap; the padding is TMA's out-of-bounds zero fill), the
 //     K-major weight matrix / the dy matrix by tiled TMA loads — one elected thread issues them, completion is counted
-//     in bytes on the stage's mbarrier.  No LSU instruction touches an operand; producer warps are gone
-//     (9 warps: two MMA + epilogue warpgroups and the TMA warp instead of 16), stages are as deep as shared memory
-//     allows (up to 8);
+//     in bytes on the stage's mbarrier.  No LSU instruction touches an operand; producer warps are gone (fwd / dgrad:
+//     two ping-pong consumer warpgroups and a producer warpgroup; wgrad: two MMA + epilogue warpgroups and the TMA
+//     warp), stages are as deep as shared memory allows (up to 8);
 //   * an operand that is a <= 8-bit fake-quantized tensor arrives as its INTEGER LEVELS (exact in bf16): one plane
 //     instead of hi + lo.  MMAs per k-slice: levels x levels 1, levels x split 2, split x split 3; the per-channel
 //     scale, and the rank-1 term that the weight offset contributes, are applied by the epilogue (pf_conv_tc.cuh).
@@ -21,7 +21,7 @@ namespace pfconv {
 using namespace pftma;
 
 constexpr int kTmaMaxStages = 8;
-constexpr int kTmaThreads = (kMmaWarps + 1) * 32;     // warps 0-7: MMA warpgroups + epilogue, warp 8: TMA producer
+constexpr int kTmaThreads = (kMmaWarps + 1) * 32;     // wgrad: warps 0-7 MMA warpgroups + epilogue, warp 8 TMA producer
 constexpr uint32_t kATileBytes = TM * 128;
 
 struct TmaP {
@@ -41,16 +41,154 @@ struct TmaP {
 
 // ---------------------------------------------------------------------------------------------------------
 // fwd / dgrad (unit stride): D[M x Ng] = A[M x K] * B[Ng x K]^T, both operands K-major, 128 x BN output tiles,
-// persistent CTAs (the TMA loads of tile i+1 run under the epilogue of tile i).
+// persistent CTAs, ping-pong consumers.  The TMA thread fills the stage ring for the CTA's tiles in order; consumer
+// warpgroup w owns the CTA's tiles 2 j + w (j = 0, 1, ...) whole: two m64 wgmmas per k-slice and plane product, into
+// two accumulator halves.  Two turns pass between the warpgroups, each through a pair of mbarriers:
+//   * the mainloop turn: a warpgroup waits on the stage ring only after the other has issued its last tile's MMAs, so
+//     the ring is consumed in the order it is filled (a consumer that ran ahead could take the parity of a stage's
+//     earlier fill for the one it wants) and the two warpgroups' MMAs do not interleave;
+//   * the epilogue turn: one fp32 staging tile serves both; a warpgroup owns it from its accumulator store to its last
+//     read in the epilogue.
+// So while one warpgroup runs a tile's epilogue (bias, ReLU, residual or accumulate, the levels' rank-1 term, 64 KB of
+// fp32 stores at BN = 128), the other runs the next tile's MMAs.  Warpgroup 0 takes its first turns without waiting;
+// every later turn waits for the other warpgroup's release of the previous one, which keeps the handoff correct for
+// any number of tiles per CTA (with one tile, warpgroup 1 never waits and its releases are never read).
+constexpr int kPingPongWarps = 4;        // arrivals per turn release and per stage release: one per consumer warp
+// warps 0-7: the two consumer warpgroups; warps 8-11: the producer warpgroup (one thread issues the TMA loads).  A
+// consumer holds a whole 128 x BN accumulator (128 registers at BN = 128), more than the 168 registers per thread
+// that 384 resident threads leave; the producer warpgroup gives up all but 40 of its registers and the consumers
+// raise theirs to 232 (128 x 40 + 256 x 232 <= 64 K).
+constexpr int kPingPongThreads = (kMmaWarps + 4) * 32;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
+template <int AFF, int BN, int NA, int NB>
+__device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, uint32_t stage_bytes,
+                                                  uint32_t n_stages, uint64_t* full_bar, uint64_t* empty_bar,
+                                                  uint64_t* ml_bar, uint64_t* epi_bar, int* tab_n0, float* out,
+                                                  const float* bias, const float* residual) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, q = warp & 3, wtid = tid & 127;   // epilogue rows [32 q, 32 q + 32) of the tile
+  const uint32_t b_bytes = (uint32_t)BN * 128u;
+  float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
+  float* aff_tab = jrow_all + kMmaWarps * 32;               // AFF == 2: e1[256], e2[256] of the staged tile's columns
+  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : 0));
+  long long* rowoff = rowoff_all + warp * 32;
+  float* jrow = jrow_all + warp * 32;
+  uint8_t* ring = p.ring ? ring_all + (size_t)warp * p.ring * kRingSlotBytes : nullptr;
+  const float* extra = residual ? residual : (p.accumulate ? out : nullptr);
+  uint32_t it = (uint32_t)wg * (uint32_t)p.nk;              // stage-ring position of this warpgroup's next tile
+  for (int tile = blockIdx.x + wg * gridDim.x, j = 0; tile < p.total_tiles; tile += 2 * gridDim.x, ++j) {
+    const bool wait_turn = wg == 1 || j > 0;
+    const uint32_t turn_ph = (uint32_t)(wg == 1 ? j : j - 1) & 1u;
+    // ---- mainloop
+    if (wait_turn) mbar_wait_bounded(&ml_bar[wg], turn_ph);
+    float acc[2][BN / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+    uint32_t s = it % n_stages, ph = (it / n_stages) & 1u, prev = 0;
+    for (int ks = 0; ks < p.nk; ++ks) {
+      mbar_wait_bounded(&full_bar[s], ph);                               // TMA bytes have landed
+      const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), a1 = a0 + kATileBytes;
+      const uint32_t b0 = a0 + (uint32_t)NA * kATileBytes, b1 = b0 + b_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t db0 = make_smem_desc(b0 + kk * 32, 16, 1024), db1 = make_smem_desc(b1 + kk * 32, 16, 1024);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {                                    // rows [64 h, 64 h + 64): 8 KB per plane
+          const uint32_t ha = (uint32_t)h * 64 * 128 + kk * 32;
+          wg_mma_kslice<BN, 0, NA, NB>(acc[h], make_smem_desc(a0 + ha, 16, 1024), make_smem_desc(a1 + ha, 16, 1024),
+                                       db0, db1);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>(acc);                     // the previous stage's MMAs have completed: release it
+      if (ks > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = s;
+      if (++s == n_stages) { s = 0; ph ^= 1u; }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&ml_bar[wg ^ 1]);                          // every MMA of this tile is issued
+    wgmma_wait<0>(acc);
+    if (p.nk > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    it += 2u * (uint32_t)p.nk;
+    // ---- epilogue
+    const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
+    const int n0 = (tile - mt * p.n_tiles) * BN;
+    const int m = mt * TM + q * 32 + lane;
+    const long long off = m < p.M ? (long long)m * p.Ng : -1;
+    float my_j = 0.f;
+    if (AFF == 2 && p.csum && m < p.M) {
+      // sum of the stored activation levels under this row's filter window, from the per-pixel channel sums, before
+      // the epilogue turn (it needs no staging tile): the (tap, segment) terms are independent loads, issued four at a
+      // time (branch-free; the terms are integers below 2^24, so the order of the additions does not change the result)
+      const int img = (int)fdiv((uint32_t)m, p.d_hw);
+      const int rem = m - img * p.rows_hw;
+      const int y = (int)fdiv((uint32_t)rem, p.d_w), x = rem - y * p.rows_w;
+      const int ow0 = p.base_w + x * p.str_w, oh0 = p.base_h + y * p.str_h;
+      const int total = p.R * p.S * p.nseg;
+      const float* cbase = p.csum + (size_t)img * p.src_h * p.src_w * p.nseg;
+      auto term = [&](int u) -> float {
+        if (u >= total) return 0.f;
+        const int t = u / p.nseg, g = u - t * p.nseg;
+        const int r = (int)fdiv((uint32_t)t, p.d_s), s_ = t - r * p.S;
+        const int ih = oh0 + r, iw = ow0 + s_;
+        const bool ok = (unsigned)ih < (unsigned)p.src_h && (unsigned)iw < (unsigned)p.src_w;
+        return ok ? __ldg(cbase + ((size_t)ih * p.src_w + iw) * p.nseg + g) : 0.f;
+      };
+      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+      for (int u = 0; u < total; u += 4) {
+        const float v0 = term(u), v1 = term(u + 1), v2 = term(u + 2), v3 = term(u + 3);
+        a0 += v0; a1 += v1; a2 += v2; a3 += v3;
+      }
+      my_j = (a0 + a1) + (a2 + a3);
+    }
+    if (wait_turn) mbar_wait_bounded(&epi_bar[wg], turn_ph);            // the staging tile is this warpgroup's
+    wgmma_store_acc<BN>(acc[0], acc_s, acc_pitch(BN), 0, wtid);
+    wgmma_store_acc<BN>(acc[1], acc_s, acc_pitch(BN), 64, wtid);
+    const int tab_was = AFF == 2 ? *reinterpret_cast<volatile int*>(tab_n0) : 0;
+    if (AFF == 2 && tab_was != n0) {
+      // per-column constants of this tile's columns, when they differ from the staged table's (with one n-tile per
+      // row of tiles this runs once per CTA):  e1[c] = s_a * alpha_c / k_w ,  e2[c] = s_a * (centre * alpha_c / k_w + beta_c)
+      const float a_s = p.aff.a_scale ? __ldg(p.aff.a_scale) : 1.f;
+      for (int c = wtid; c < BN; c += 128) {
+        const bool cok = n0 + c < p.Ng;
+        const int bi = p.aff.per_channel ? n0 + c : 0;
+        const float al = cok ? __ldg(p.aff.w_alpha + bi) : 0.f, be = cok ? __ldg(p.aff.w_beta + bi) : 0.f;
+        const float sx = al * p.aff.w_rk;
+        aff_tab[c] = sx * a_s;
+        aff_tab[256 + c] = fmaf(p.aff.w_centre, sx, be) * a_s;
+      }
+    }
+    named_bar_sync(2 + wg, 128);                       // the staged tile (and table) are visible to the warpgroup
+    if (AFF == 2 && tab_was != n0 && wtid == 0) *reinterpret_cast<volatile int*>(tab_n0) = n0;
+    epilogue_rows<AFF>(acc_s + (size_t)(32 * q) * acc_pitch(BN), 0, 32, off, rowoff, out, extra, bias, p.relu, n0, BN,
+                       p.Ng, lane, ring, p.aff, my_j, jrow, AFF == 2 ? aff_tab : nullptr, p.ring);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&epi_bar[wg ^ 1]);                         // this warp's reads of the tile are done
+  }
+}
+
 template <int AFF, int BN>
-__global__ void __launch_bounds__(kTmaThreads, 1)
+__global__ void __launch_bounds__(kPingPongThreads, 1)
 conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
                 float* __restrict__ out, const float* __restrict__ bias, const float* __restrict__ residual,
                 const __grid_constant__ TmaP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages];
+  __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages], ml_bar[2], epi_bar[2];
+  __shared__ int tab_n0;                              // first column of the AFF == 2 table in shared memory (-1: none)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int na = p.na;
   if (p.a_hdr) na = (__ldg(&p.a_hdr->nplanes) == 2) ? 2 : 1;
@@ -58,31 +196,31 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
   const uint32_t b_bytes = (uint32_t)BN * 128u;
   const uint32_t stage_bytes = (uint32_t)na * kATileBytes + (uint32_t)nb * b_bytes;
   const uint32_t n_stages = min((uint32_t)kTmaMaxStages, (uint32_t)p.stage_budget / stage_bytes);
-  float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
-  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
-  float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
-  float* aff_tab = jrow_all + kMmaWarps * 32;               // AFF == 2: e1[256], e2[256] of the current tile columns
-  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : 0));
 
   if (tid == 0) {
     for (int s = 0; s < kTmaMaxStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kMmaWarps);
+      mbar_init(&empty_bar[s], kPingPongWarps);
     }
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&ml_bar[w], kPingPongWarps);
+      mbar_init(&epi_bar[w], kPingPongWarps);
+    }
+    tab_n0 = -1;
     fence_barrier_init();
   }
   __syncthreads();
-  const int first_tile = blockIdx.x, tile_step = gridDim.x;
 
-  if (warp == kMmaWarps) {
+  if (warp >= kMmaWarps) {
     // =================================== TMA producer (one thread) ===================================
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kMmaWarps && lane == 0) {
       prefetch_map(&tmA0);
       prefetch_map(&tmB0);
       if (na == 2) prefetch_map(&tmA1);
       if (nb == 2) prefetch_map(&tmB1);
       uint32_t s = 0, ph = 0;
-      for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
         const int n0 = (tile - mt * p.n_tiles) * BN;
         const int m0 = mt * TM;
@@ -108,90 +246,20 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
       }
     }
   } else {
-    // ============================ MMA warpgroups + epilogue (warps 0-7) ============================
-    const int wg = warp >> 2, q = warp & 3;  // MMA rows [64 wg, 64 wg + 64); epilogue rows [32 q, 32 q + 32)
-    const int ew = warp;
-    long long* rowoff = rowoff_all + ew * 32;
-    float* jrow = jrow_all + ew * 32;
-    const float* extra = residual ? residual : (p.accumulate ? out : nullptr);
-    int tab_n0 = -1;
-    uint32_t s = 0, ph = 0;
-    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
-      float acc[BN / 2];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      uint32_t prev = 0;
-      for (int ks = 0; ks < p.nk; ++ks) {
-        mbar_wait_bounded(&full_bar[s], ph);                             // TMA bytes have landed
-        const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)wg * 64 * 128, a1 = a0 + kATileBytes;
-        const uint32_t b0 = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)na * kATileBytes, b1 = b0 + b_bytes;
-        wg_mma_stage<BN, 0>(acc, a0, a1, b0, b1, na, nb, 32, 32, 16, 1024, 16, 1024);
-        wgmma_wait<1>(acc);                    // the previous stage's MMAs have completed: release it
-        if (ks > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
-        }
-        prev = s;
-        if (++s == n_stages) { s = 0; ph ^= 1u; }
-      }
-      wgmma_wait<0>(acc);
-      if (p.nk > 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      }
-      const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
-      const int n0 = (tile - mt * p.n_tiles) * BN;
-      const int m = mt * TM + q * 32 + lane;
-      const long long off = m < p.M ? (long long)m * p.Ng : -1;
-      if (AFF == 2 && n0 != tab_n0) {
-        // per-column constants of this tile's columns, once (every epilogue warp walks the same tile sequence, so the
-        // named barrier below is reached by all of them; with one n-tile per row of tiles this runs once per CTA):
-        //   e1[c] = s_a * alpha_c / k_w ,  e2[c] = s_a * (centre * alpha_c / k_w + beta_c)
-        const int nthr = kMmaWarps * 32;
-        asm volatile("bar.sync 1, %0;" ::"r"(nthr) : "memory");          // readers of the previous table are done
-        const float a_s = p.aff.a_scale ? __ldg(p.aff.a_scale) : 1.f;
-        for (int c = ew * 32 + lane; c < BN; c += nthr) {
-          const bool cok = n0 + c < p.Ng;
-          const int bi = p.aff.per_channel ? n0 + c : 0;
-          const float al = cok ? __ldg(p.aff.w_alpha + bi) : 0.f, be = cok ? __ldg(p.aff.w_beta + bi) : 0.f;
-          const float sx = al * p.aff.w_rk;
-          aff_tab[c] = sx * a_s;
-          aff_tab[256 + c] = fmaf(p.aff.w_centre, sx, be) * a_s;
-        }
-        asm volatile("bar.sync 1, %0;" ::"r"(nthr) : "memory");
-        tab_n0 = n0;
-      }
-      float my_j = 0.f;
-      if (AFF == 2 && p.csum && m < p.M) {
-        // sum of the stored activation levels under this row's filter window, from the per-pixel channel sums: the
-        // (tap, segment) terms are independent loads, issued four at a time (branch-free; the terms are integers below
-        // 2^24, so the order of the additions does not change the result)
-        const int img = (int)fdiv((uint32_t)m, p.d_hw);
-        const int rem = m - img * p.rows_hw;
-        const int y = (int)fdiv((uint32_t)rem, p.d_w), x = rem - y * p.rows_w;
-        const int ow0 = p.base_w + x * p.str_w, oh0 = p.base_h + y * p.str_h;
-        const int total = p.R * p.S * p.nseg;
-        const float* cbase = p.csum + (size_t)img * p.src_h * p.src_w * p.nseg;
-        auto term = [&](int u) -> float {
-          if (u >= total) return 0.f;
-          const int t = u / p.nseg, g = u - t * p.nseg;
-          const int r = (int)fdiv((uint32_t)t, p.d_s), s_ = t - r * p.S;
-          const int ih = oh0 + r, iw = ow0 + s_;
-          const bool ok = (unsigned)ih < (unsigned)p.src_h && (unsigned)iw < (unsigned)p.src_w;
-          return ok ? __ldg(cbase + ((size_t)ih * p.src_w + iw) * p.nseg + g) : 0.f;
-        };
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-        for (int u = 0; u < total; u += 4) {
-          const float v0 = term(u), v1 = term(u + 1), v2 = term(u + 2), v3 = term(u + 3);
-          a0 += v0; a1 += v1; a2 += v2; a3 += v3;
-        }
-        my_j = (a0 + a1) + (a2 + a3);
-      }
-      wg_tile_to_smem<BN>(acc, acc_s, tid);
-      epilogue_tile_a<AFF>(acc_s, ew, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
-                           p.ring ? ring_all + (size_t)ew * p.ring * kRingSlotBytes : nullptr, p.aff, my_j, jrow,
-                           AFF == 2 ? aff_tab : nullptr, p.ring);
+    // ==================== two ping-pong consumer warpgroups (warps 0-3, 4-7): MMAs + epilogue ====================
+    // the plane counts are fixed for the whole launch: one straight-line mainloop per combination
+    setmaxnreg_inc<kConsumerRegs>();
+#define PF_TMA_CONSUMER(NA_, NB_)                                                                                    \
+  conv_tma_consumer<AFF, BN, NA_, NB_>(p, smem, stage_bytes, n_stages, full_bar, empty_bar, ml_bar, epi_bar, &tab_n0, \
+                                       out, bias, residual)
+    if (na == 2) {
+      if (nb == 2) PF_TMA_CONSUMER(2, 2);
+      else PF_TMA_CONSUMER(2, 1);
+    } else {
+      if (nb == 2) PF_TMA_CONSUMER(1, 2);
+      else PF_TMA_CONSUMER(1, 1);
     }
+#undef PF_TMA_CONSUMER
   }
 }
 
@@ -302,10 +370,13 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
       }
     }
   } else {
-    // MMA warpgroups + epilogue: warpgroup wg multiplies kf rows [64 wg, 64 wg + 64) = MN block wg of the x tile
+    // MMA warpgroups + epilogue: warpgroup wg multiplies kf rows [64 wg, 64 wg + 64) = MN block wg of the x tile;
+    // the plane counts are fixed for the whole launch: one straight-line mainloop per combination
     const int wg = warp >> 2, q = warp & 3;
     long long* rowoff = rowoff_all + warp * 32;
     float* jrow = jrow_all + warp * 32;
+    auto consume = [&](auto na_c, auto nb_c) {
+    constexpr int NA = decltype(na_c)::value, NB = decltype(nb_c)::value;
     uint32_t s = 0, ph = 0;
     for (int u = blockIdx.x; u < p.total_units; u += gridDim.x) {
       const Unit un = decode(u);
@@ -317,10 +388,10 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
         mbar_wait_bounded(&full_bar[s], ph);
         const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
         const uint32_t a0 = base + (uint32_t)wg * kWgBlockBytes, a1 = a0 + a_bytes;
-        const uint32_t b0 = base + (uint32_t)na * a_bytes, b1 = b0 + b_bytes;
+        const uint32_t b0 = base + (uint32_t)NA * a_bytes, b1 = b0 + b_bytes;
         // MN-major: LBO = stride between 64-wide MN blocks (8 KB), SBO = stride between 8-pixel groups (1 KB);
         // one MMA consumes 16 pixels = 2 KB
-        wg_mma_stage<BN, 1>(acc, a0, a1, b0, b1, na, nb, 2048, 2048, kWgBlockBytes, 1024, kWgBlockBytes, 1024);
+        wg_mma_stage<BN, 1, NA, NB>(acc, a0, a1, b0, b1, 2048, 2048, kWgBlockBytes, 1024, kWgBlockBytes, 1024);
         wgmma_wait<1>(acc);
         if (ks > 0) {
           __syncwarp();
@@ -339,6 +410,16 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
       wg_tile_to_smem<BN>(acc, acc_s, tid);
       epilogue_tile_a<AFF>(acc_s, warp, off, rowoff, partial, nullptr, nullptr, 0, un.n0, BN, g.K, lane, nullptr, p.aff,
                            0.f, jrow);
+    }
+    };
+    using one = std::integral_constant<int, 1>;
+    using two = std::integral_constant<int, 2>;
+    if (na == 2) {
+      if (nb == 2) consume(two(), two());
+      else consume(two(), one());
+    } else {
+      if (nb == 2) consume(one(), two());
+      else consume(one(), one());
     }
   }
 }
@@ -485,7 +566,7 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     constexpr int B = decltype(bn)::value;
     auto kern = aff == 2 ? conv_tma_kernel<2, B> : (aff == 1 ? conv_tma_kernel<1, B> : conv_tma_kernel<0, B>);
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err == cudaSuccess) kern<<<grid, kTmaThreads, smem, st>>>(tA0, tA1, tB0, tB1, out, bias, residual, p);
+    if (err == cudaSuccess) kern<<<grid, kPingPongThreads, smem, st>>>(tA0, tA1, tB0, tB1, out, bias, residual, p);
   });
   PF_CUDA(err);
   PF_CHECK_LAUNCH(who);

@@ -64,6 +64,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ---- per-warpgroup register budgets (all 128 threads of a warpgroup execute these together): a warpgroup that
+// needs few registers hands them back to the pool, one that holds large accumulators takes them
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- wgmma descriptors
 // Shared-memory matrix descriptor: start address, LBO, SBO in 16-byte units; bits 62-63 layout type
 // 1 = SWIZZLE_128B (tile base 1024-byte aligned).
@@ -87,6 +94,15 @@ __device__ __forceinline__ void wgmma_wait(float (&d)[R]) {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// the same for an accumulator of H row blocks (one warpgroup owning several m64 blocks of a tile)
+template <int N, int H, int R>
+__device__ __forceinline__ void wgmma_wait(float (&d)[H][R]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+#pragma unroll
+  for (int h = 0; h < H; ++h)
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[h][i])::"memory");
 }
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 operands from shared memory, fp32 accumulator in registers.
