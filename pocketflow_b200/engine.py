@@ -27,6 +27,160 @@ def _align4(n):
     return (n + 3) // 4 * 4
 
 
+class _ConvLowering:
+    """How one Conv2D / MatMul runs, fixed at plan time; this class: the exact-fp32 CUDA-core kernels.
+    wgrad writes dL/dW into `dw`, or (None) into the plan's target; dy_buf: bf16 buffer to split an external gy into."""
+    side = False                     # the weight gradient may run on the side stream (both operands are planes)
+
+    def __init__(self, ex, op):
+        self.ex, self.op, self.d, self.x = ex, op, ex.desc[op], op.inputs[0]
+
+    def _epilogue(self):
+        """(bias, fused relu, output buffer) of the forward kernel"""
+        op, ex = self.op, self.ex
+        return ex.store.view(op.vars['bias']) if 'bias' in op.vars else None, op in ex.fused_act, ex.buf[op.output]
+
+    def _target(self, dw):
+        return dw if dw is not None else self.ex.store.view(self.op.vars['kernel'], self.ex.G)
+
+    def prepare_weights(self):
+        """refresh the tensor-core copy of the kernel (inference executors that own their parameters)"""
+
+    def forward(self):
+        with self.ex.timed('conv_fwd'):
+            ops.conv2d_fwd(self.d, self.ex.T(self.x), self.ex.kernel_of(self.op), *self._epilogue())
+
+    def wgrad(self, gy, ws, dw=None, dy_buf=None):
+        ops.conv2d_wgrad(self.d, self.ex.T(self.x), gy, ws, self._target(dw))
+
+    def dgrad(self, gy, gx, acc):
+        ops.conv2d_dgrad(self.d, gy, self.ex.kernel_of(self.op), self.ex.wt_ws, acc, gx)
+
+
+class _TcConv(_ConvLowering):
+    """Tensor-core conv: x from its producer's planes (integer levels in training passes where it writes them) or fp32;
+    with a tensor-core wgrad, dy from the BN backward's planes or split into the shared scratch, for wgrad and dgrad."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op)
+        self.tw, self.xp, self.w_lv = ex.tc[op], ex.planes_of(self.x), ex.w_lv.get(op)
+        self.x_lv = ex.act_lv.get(ex._root(self.x).op) if self.xp is not None else None
+        self.res = ex.fused_add[op][1] if op in ex.fused_add else None
+        self.tc_wgrad = op in ex.tc_wgrad
+        if self.tc_wgrad:
+            self.xw = ops.Planes(self.x.numel, ex.device, ex.x_scratch.buf) if self.xp is None else self.xp
+            self.dy_split = op not in ex.conv_dy_planes
+            self.dy = ops.Planes(op.output.numel, ex.device, ex.dy_scratch.buf) if self.dy_split \
+                else ex.conv_dy_planes[op]
+            self.part = ex.wg_part.get(op)
+            self.side = self.xp is not None and not self.dy_split
+
+    def _levels(self):
+        return self.ex._lv_on and self.x_lv is not None
+
+    def _x_act(self):
+        lv = self.x_lv
+        return ops.tc_act(self.xp, lv['hdr'], lv['csum'], lv['nseg'])
+
+    def _wt(self):
+        lv = self.w_lv
+        if lv is not None and self.ex.wq.bits[lv['index']] <= 8:
+            return ops.tc_wt(self.tw.f_hi, None, lv['alpha'], lv['beta'], lv['ncols'] > 1, self.ex.wq.bits[lv['index']])
+        return ops.tc_wt(self.tw.f_hi, self.tw.f_lo)
+
+    def prepare_weights(self):
+        self.tw.prepare(self.ex.kernel_of(self.op))
+
+    def forward(self):
+        ex = self.ex
+        res = ex.T(self.res) if self.res is not None else None
+        with ex.timed('conv_fwd'):
+            if self._levels():
+                ops.conv2d_tc_fwd_ex(self.d, self._x_act(), self._wt(), *self._epilogue(), res)
+            elif self.xp is not None:
+                ops.conv2d_tc_fwd_planes(self.d, self.xp, self.tw, *self._epilogue(), res)
+            else:
+                ops.conv2d_tc_fwd(self.d, ex.T(self.x), self.tw, *self._epilogue(), res)
+
+    def wgrad(self, gy, ws, dw=None, dy_buf=None):
+        if not self.tc_wgrad:
+            return super().wgrad(gy, ws, dw)
+        if self.xp is None:
+            ops.split_bf16(self.ex.T(self.x), self.xw)
+        dyp = self.dy if dy_buf is None else ops.Planes(self.op.output.numel, self.ex.device, dy_buf)
+        if dy_buf is not None or self.dy_split:
+            ops.split_bf16(gy, dyp)
+        if dw is None and self.part is not None:
+            ws = self.part                   # split-K partials, summed into the flat gradient after the backward pass
+        else:
+            dw = self._target(dw)
+        if self._levels():
+            ops.conv2d_tc_wgrad_ex(self.d, self._x_act(), ops.tc_act(dyp), ws, dw)
+        else:
+            ops.conv2d_tc_wgrad_planes(self.d, self.xw, dyp, ws, dw)
+
+    def dgrad(self, gy, gx, acc):
+        if self.tc_wgrad:
+            ops.conv2d_tc_dgrad_planes(self.d, self.dy, self.tw, acc, gx)
+        else:
+            ops.conv2d_tc_dgrad(self.d, gy, self.tw, acc, gx)
+
+
+class _StemConv(_ConvLowering):
+    """First layer (its input is the image: no dgrad): a tensor-core conv over the columns / space-to-depth planes of
+    ex.im2col[op], with the kernel re-arranged into that layout and its gradient mapped back."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op)
+        self.im = ex.im2col[op]
+        self.s2d = self.im['mode'] == 's2d'
+
+    def prepare_weights(self):
+        im, wk = self.im, self.ex.kernel_of(self.op)
+        if self.s2d:
+            ops.gather_rows(wk, im['fwd_map'], im['wpad'], wk.shape[-1])
+        else:
+            ops.add(wk.reshape(-1), None, im['wpad'][:wk.numel()])       # rows >= R*S*C stay zero
+        im['tw'].prepare(im['wpad'])
+
+    def forward(self):
+        ex, im = self.ex, self.im
+        with ex.timed('conv_prep'):
+            if im['compute']:
+                x = ex.T(self.x)
+                if self.s2d:
+                    ops.s2d_planes(x, *self.op.attrs['pad'], im['d1'].h, im['d1'].w, im['d1'].c, im['cols'])
+                else:
+                    (ops.im2col_planes if im['planes'] else ops.im2col)(self.d, x, im['kpad'], im['cols'])
+                if ex.cols_event is not None:
+                    ex.cols_event.record()
+            elif ex.cols_wait is not None:
+                torch.cuda.current_stream().wait_event(ex.cols_wait)
+            if not ex.static_weights:
+                self.prepare_weights()
+        with ex.timed('conv_fwd'):
+            fwd = ops.conv2d_tc_fwd_planes if im['planes'] else ops.conv2d_tc_fwd
+            fwd(im['d1'], im['cols'], im['tw'], *self._epilogue())
+
+    def wgrad(self, gy, ws, dw=None, dy_buf=None):
+        im, dw = self.im, self._target(dw)
+        if im['planes']:
+            dyp = ops.Planes(self.op.output.numel, self.ex.device, self.ex.dy_scratch.buf if dy_buf is None else dy_buf)
+            ops.split_bf16(gy, dyp)
+            if 'pair' in im:
+                pr = im['pair']
+                ops.conv2d_tc_wgrad_planes(pr['d'], im['cols'], dyp, ws, pr['dw'])
+                ops.fold_diag_blocks(pr['dw'], pr['g'], im['kpad'], im['d1'].k, im['dwpad'])
+            else:
+                ops.conv2d_tc_wgrad_planes(im['d1'], im['cols'], dyp, ws, im['dwpad'])
+        else:
+            ops.conv2d_wgrad(im['d1'], im['cols'], gy, ws, im['dwpad'])
+        if self.s2d:
+            ops.gather_rows(im['dwpad'], im['bwd_map'], dw, dw.shape[-1])
+        else:
+            ops.add(im['dwpad'][:dw.numel()], None, dw.reshape(-1))
+
+
 class ParamStore:
     """Flat storage for the trainable variables of one model scope (+ separate non-trainable store).
 
@@ -190,26 +344,13 @@ class Executor:
         """Parameters were (re)loaded: refresh the prepared weight copies now (a captured CUDA graph that contains
         this executor's forward does not re-run the preparation)."""
         self._static_ready = False
-        if hasattr(self, 'tc'):
+        if hasattr(self, 'conv'):
             self.prepare_static_weights()
 
     def prepare_static_weights(self):
-        for op in self.ops:
-            if op in self.im2col:
-                im, wk = self.im2col[op], self.kernel_of(op)
-                self._stem_weights(im, wk)
-            elif op in self.tc:
-                self.tc[op].prepare(self.kernel_of(op))
+        for lo in self.conv.values():
+            lo.prepare_weights()
         self._static_ready = True
-
-    def _stem_weights(self, im, wk):
-        """fp32 kernel of the first layer -> the (re-arranged / padded) matrix its tensor-core conv multiplies by"""
-        k = wk.shape[-1]
-        if im['mode'] == 's2d':
-            ops.gather_rows(wk, im['fwd_map'], im['wpad'], k)
-        else:
-            ops.add(wk.reshape(-1), None, im['wpad'][:wk.numel()])       # rows >= R*S*C stay zero
-        im['tw'].prepare(im['wpad'])
 
     # ------------------------------------------------------------------ planning
     def _reachable_ops(self, out):
@@ -322,6 +463,7 @@ class Executor:
         self.im2col = {}
         self.pool_argmax = {}
         max_ws, max_wt, max_bnws = 4, 4, 4
+        max_x = max_dy = 8             # the x / dy operands split into planes (shared scratch)
         self.desc = {}
         for op in self.ops:
             if op.type == 'FusedBatchNorm':
@@ -377,14 +519,14 @@ class Executor:
                         self.im2col[op]['bwd_map'] = torch.from_numpy(bwd_map).to(dev)
                     if self.train:
                         self.im2col[op]['dwpad'] = torch.zeros(kpad * k, dtype=torch.float32, device=dev)
+                        if as_planes:                      # dy is split into planes for the tensor-core wgrad
+                            max_dy = max(max_dy, n * p * q * k)
                         if pair is not None and mode == 'im2col':
                             pair['dw'] = torch.zeros(pair['g'] * kpad * pair['g'] * k, dtype=torch.float32, device=dev)
                             self.im2col[op]['pair'] = pair
                             max_ws = max(max_ws, ops.conv2d_tc_wgrad_planes_workspace_floats(pair['d']))
-                            self._stem_dy = max(getattr(self, '_stem_dy', 8), n * p * q * k)
                         if ops.conv2d_tc_wgrad_supported(d1):
                             max_ws = max(max_ws, ops.conv2d_tc_wgrad_planes_workspace_floats(d1))
-                            self._stem_dy = max(getattr(self, '_stem_dy', 8), n * p * q * k)
                         max_ws = max(max_ws, ops.conv2d_wgrad_workspace_floats(d1))
                 if self.conv_path == 'tc' and ops.conv2d_tc_supported(d):
                     self.tc[op] = ops.TcWeights(d, dev, need_dgrad=self.train and x.op.type != 'Placeholder')
@@ -447,7 +589,6 @@ class Executor:
         # input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
         # the fp32 copy is only written when some other consumer needs it
         self.xplanes, self.bn_need_f32 = {}, {}
-        max_x = max_dy = 8
         for op in self.ops:
             if op in self.tc and op not in self.im2col:
                 r = self._root(op.inputs[0])
@@ -658,7 +799,6 @@ class Executor:
                         red_items.append((self.wg_part[op], gk, splits))
             self._red_items = red_items
             self.wg_reduce = ops.TcWgradReduceBatch(red_items, dev) if red_items else None
-            max_dy = max(max_dy, getattr(self, '_stem_dy', 8))
             self.x_scratch = ops.Planes(max_x, dev)
             self.dy_scratch = ops.Planes(max_dy, dev)
             if self.maskable:
@@ -677,6 +817,9 @@ class Executor:
                 self._ste_grads = None
             self.beta1_power = F32(self.optimizer.get('beta1', 0.9))
             self.beta2_power = F32(self.optimizer.get('beta2', 0.999))
+        # ---- how each Conv2D / MatMul runs forward, backward and in layer_wgrad
+        self.conv = {op: (_StemConv if op in self.im2col else _TcConv if op in self.tc else _ConvLowering)(self, op)
+                     for op in self.ops if op.type in ('Conv2D', 'MatMul')}
 
     # ------------------------------------------------------------------ profiling (bench.py roofline)
     class _Timed:
@@ -747,27 +890,6 @@ class Executor:
         r = self._root(t)
         return self.xplanes.get(r.op) if r is not None else None
 
-    def _act_lv_of(self, t):
-        """level-operand record of the BN that produced tensor t's planes (None: plain split-bf16 planes)"""
-        r = self._root(t)
-        return self.act_lv.get(r.op) if r is not None else None
-
-    def _tc_act(self, t):
-        lv, xp = self._act_lv_of(t), self.planes_of(t)
-        return ops.tc_act(xp, lv['hdr'], lv['csum'], lv['nseg']) if lv is not None else ops.tc_act(xp)
-
-    def _tc_wt(self, op):
-        tw = self.tc[op]
-        lv = self.w_lv.get(op) if self._lv_on else None
-        if lv is not None and self.wq.bits[lv['index']] <= 8:
-            return ops.tc_wt(tw.f_hi, None, lv['alpha'], lv['beta'], lv['ncols'] > 1, self.wq.bits[lv['index']])
-        return ops.tc_wt(tw.f_hi, tw.f_lo)
-
-    def raw(self, t):
-        while t in self.alias:
-            t = self.alias[t]
-        return self.buf[t]
-
     def gkey(self, t):
         while t in self.galias:
             t = self.galias[t]
@@ -816,52 +938,7 @@ class Executor:
             if ty == 'Placeholder' or self._passthrough(op):
                 continue
             if ty in ('Conv2D', 'MatMul'):
-                bias = st.view(op.vars['bias']) if 'bias' in op.vars else None
-                if op in self.im2col:
-                    im = self.im2col[op]
-                    wk = self.kernel_of(op)
-                    with self.timed('conv_prep'):
-                        if im['compute']:
-                            if im['mode'] == 's2d':
-                                pt_, pl_ = op.attrs['pad']
-                                ops.s2d_planes(self.T(op.inputs[0]), pt_, pl_, im['d1'].h, im['d1'].w, im['d1'].c, im['cols'])
-                            elif im['planes']:
-                                ops.im2col_planes(self.desc[op], self.T(op.inputs[0]), im['kpad'], im['cols'])
-                            else:
-                                ops.im2col(self.desc[op], self.T(op.inputs[0]), im['kpad'], im['cols'])
-                            if self.cols_event is not None:
-                                self.cols_event.record()
-                        elif self.cols_wait is not None:
-                            torch.cuda.current_stream().wait_event(self.cols_wait)
-                        if not self.static_weights:
-                            self._stem_weights(im, wk)
-                    with self.timed('conv_fwd'):
-                        if im['planes']:
-                            ops.conv2d_tc_fwd_planes(im['d1'], im['cols'], im['tw'], bias, op in self.fused_act,
-                                                     self.buf[op.output])
-                        else:
-                            ops.conv2d_tc_fwd(im['d1'], im['cols'], im['tw'], bias, op in self.fused_act,
-                                              self.buf[op.output])
-                elif op in self.tc:
-                    if not self.static_weights and self.tc_batch is None:
-                        with self.timed('conv_prep'):
-                            self.tc[op].prepare(self.kernel_of(op))
-                    res = self.T(self.fused_add[op][1]) if op in self.fused_add else None
-                    xp = self.planes_of(op.inputs[0])
-                    with self.timed('conv_fwd'):
-                        if xp is not None and self._lv_on and self._act_lv_of(op.inputs[0]) is not None:
-                            ops.conv2d_tc_fwd_ex(self.desc[op], self._tc_act(op.inputs[0]), self._tc_wt(op), bias,
-                                                 op in self.fused_act, self.buf[op.output], res)
-                        elif xp is not None:
-                            ops.conv2d_tc_fwd_planes(self.desc[op], xp, self.tc[op], bias, op in self.fused_act,
-                                                     self.buf[op.output], res)
-                        else:
-                            ops.conv2d_tc_fwd(self.desc[op], self.T(op.inputs[0]), self.tc[op], bias,
-                                              op in self.fused_act, self.buf[op.output], res)
-                else:
-                    with self.timed('conv_fwd'):
-                        ops.conv2d_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), bias,
-                                       op in self.fused_act, self.buf[op.output])
+                self.conv[op].forward()
             elif ty == 'DepthwiseConv2dNative':
                 with self.timed('dwconv'):
                     ops.dwconv_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), self.buf[op.output])
@@ -1067,8 +1144,7 @@ class Executor:
             if self._passthrough(op) or op in self.fused_into:
                 continue                                   # gradient buffer is shared with the input
             if ty in ('Conv2D', 'MatMul'):
-                d = self.desc[op]
-                x_t = op.inputs[0]
+                lo, x_t = self.conv[op], op.inputs[0]
                 y = self.buf[op.output]
                 m, k = y.numel() // y.shape[-1], y.shape[-1]
                 if op in self.fused_act:
@@ -1078,65 +1154,18 @@ class Executor:
                 if 'bias' in op.vars:
                     ops.colsum(gy, m, k, st.view(op.vars['bias'], self.G))
                 with self.timed('conv_wgrad'):
-                    if op in self.im2col:
-                        im = self.im2col[op]
-                        gk = st.view(op.vars['kernel'], self.G)
-                        if im['planes']:
-                            gp = ops.Planes(op.output.numel, self.device, self.dy_scratch.buf)
-                            ops.split_bf16(gy, gp)
-                            self._stem_wgrad_planes(im, gp)
-                        elif ops.conv2d_tc_wgrad_supported(im['d1']):
-                            ops.conv2d_tc_wgrad(im['d1'], im['cols'], gy, self.wgrad_ws, im['dwpad'])
-                        else:
-                            ops.conv2d_wgrad(im['d1'], im['cols'], gy, self.wgrad_ws, im['dwpad'])
-                        if im['mode'] == 's2d':
-                            ops.gather_rows(im['dwpad'], im['bwd_map'], gk, gk.shape[-1])
-                        else:
-                            ops.add(im['dwpad'][:gk.numel()], None, gk.reshape(-1))
-                    elif op in self.tc_wgrad and self._side_active and self.planes_of(x_t) is not None \
-                            and self.conv_dy_planes.get(op) is not None:
-                        # both operands exist as planes: the weight gradient runs on the side stream, beside the
-                        # dgrad / BN-backward chain that continues on the main stream
-                        gp = self.conv_dy_planes[op]
+                    if lo.side and self._side_active:
+                        # the weight gradient runs on the side stream, beside the dgrad / BN-backward chain that
+                        # continues on the main stream
                         self.side2.wait_stream(torch.cuda.current_stream())
                         with torch.cuda.stream(self.side2):
-                            part = self.wg_part.get(op)
-                            dw = None if part is not None else st.view(op.vars['kernel'], self.G)
-                            if self._lv_on and self._act_lv_of(x_t) is not None:
-                                ops.conv2d_tc_wgrad_ex(d, self._tc_act(x_t), ops.tc_act(gp),
-                                                       part if part is not None else self.wgrad_ws2, dw)
-                            else:
-                                ops.conv2d_tc_wgrad_planes(d, self.planes_of(x_t), gp,
-                                                           part if part is not None else self.wgrad_ws2, dw)
-                    elif op in self.tc_wgrad:
-                        # operands in split-bf16 planes: native (written by BN-apply / BN-backward) or split here
-                        xp = self.planes_of(x_t)
-                        if xp is None:
-                            xp = ops.Planes(x_t.numel, self.device, self.x_scratch.buf)
-                            ops.split_bf16(self.T(x_t), xp)
-                        gp = self.conv_dy_planes.get(op)
-                        if gp is None:
-                            gp = ops.Planes(op.output.numel, self.device, self.dy_scratch.buf)
-                            ops.split_bf16(gy, gp)
-                        part = self.wg_part.get(op)
-                        dw = None if part is not None else st.view(op.vars['kernel'], self.G)
-                        if self._lv_on and self._act_lv_of(x_t) is not None:
-                            ops.conv2d_tc_wgrad_ex(d, self._tc_act(x_t), ops.tc_act(gp),
-                                                   part if part is not None else self.wgrad_ws, dw)
-                        else:
-                            ops.conv2d_tc_wgrad_planes(d, xp, gp, part if part is not None else self.wgrad_ws, dw)
+                            lo.wgrad(gy, self.wgrad_ws2)
                     else:
-                        gp = None
-                        ops.conv2d_wgrad(d, self.T(x_t), gy, self.wgrad_ws, st.view(op.vars['kernel'], self.G))
+                        lo.wgrad(gy, self.wgrad_ws)
                 if x_t.op.type != 'Placeholder':
                     gx, acc = self.grad_target(x_t)
                     with self.timed('conv_dgrad'):
-                        if op in self.tc_wgrad and op not in self.im2col:
-                            ops.conv2d_tc_dgrad_planes(d, gp, self.tc[op], acc, gx)
-                        elif op in self.tc:
-                            ops.conv2d_tc_dgrad(d, gy, self.tc[op], acc, gx)
-                        else:
-                            ops.conv2d_dgrad(d, gy, self.kernel_of(op), self.wt_ws, acc, gx)
+                        lo.dgrad(gy, gx, acc)
             elif ty == 'DepthwiseConv2dNative':
                 d = self.desc[op]
                 x_t = op.inputs[0]
@@ -1213,15 +1242,6 @@ class Executor:
             with self.timed('weight_quant'):
                 self.wq.cluster_grad([st.view(op.vars['kernel'], self.G) for op in self.wq_ops], self.G)
 
-    def _stem_wgrad_planes(self, im, gp):
-        """weight gradient of the first layer from its column planes and the dy planes, into im['dwpad']"""
-        if 'pair' in im:
-            pr = im['pair']
-            ops.conv2d_tc_wgrad_planes(pr['d'], im['cols'], gp, self.wgrad_ws, pr['dw'])
-            ops.fold_diag_blocks(pr['dw'], pr['g'], im['kpad'], im['d1'].k, im['dwpad'])
-        else:
-            ops.conv2d_tc_wgrad_planes(im['d1'], im['cols'], gp, self.wgrad_ws, im['dwpad'])
-
     @contextlib.contextmanager
     def standalone_forward(self):
         """forward() calls outside device_step (layer-wise regression passes): an executor that shares the first layer's
@@ -1241,39 +1261,12 @@ class Executor:
         forward() of this executor: the weight gradient of the layer-wise regression loss of the channel-pruning
         learner (learners/channel_pruning_gpu/learner.py:370, :391 — compute_gradients(reg_loss_i, [kernel_i])).
         Same kernels as the step's own backward; `dw` is an fp32 tensor of the kernel's shape."""
-        d, x_t = self.desc[op], op.inputs[0]
         # own dy planes: the step's dy_scratch is only sized for the layers whose gradient is split in a separate pass
         lw = getattr(self, '_lw_planes', None)
         if lw is None or lw.numel < op.output.numel:
             lw = self._lw_planes = ops.Planes(op.output.numel, self.device)
         with self.timed('conv_wgrad'):
-            if op in self.im2col:
-                im = self.im2col[op]
-                if im['planes']:
-                    gp = ops.Planes(op.output.numel, self.device, lw.buf)
-                    ops.split_bf16(gy, gp)
-                    self._stem_wgrad_planes(im, gp)
-                elif ops.conv2d_tc_wgrad_supported(im['d1']):
-                    ops.conv2d_tc_wgrad(im['d1'], im['cols'], gy, self.wgrad_ws, im['dwpad'])
-                else:
-                    ops.conv2d_wgrad(im['d1'], im['cols'], gy, self.wgrad_ws, im['dwpad'])
-                if im['mode'] == 's2d':
-                    ops.gather_rows(im['dwpad'], im['bwd_map'], dw, dw.shape[-1])
-                else:
-                    ops.add(im['dwpad'][:dw.numel()], None, dw.reshape(-1))
-            elif op in self.tc_wgrad:
-                xp = self.planes_of(x_t)
-                if xp is None:
-                    xp = ops.Planes(x_t.numel, self.device, self.x_scratch.buf)
-                    ops.split_bf16(self.T(x_t), xp)
-                gp = ops.Planes(op.output.numel, self.device, lw.buf)
-                ops.split_bf16(gy, gp)
-                if self._lv_on and self._act_lv_of(x_t) is not None:
-                    ops.conv2d_tc_wgrad_ex(d, self._tc_act(x_t), ops.tc_act(gp), self.wgrad_ws, dw)
-                else:
-                    ops.conv2d_tc_wgrad_planes(d, xp, gp, self.wgrad_ws, dw)
-            else:
-                ops.conv2d_wgrad(d, self.T(x_t), gy, self.wgrad_ws, dw)
+            self.conv[op].wgrad(gy, self.wgrad_ws, dw, lw.buf)
 
     def forward_eval_loss(self):
         """Evaluation pass: BN in inference mode, quantizers active, losses/metrics only."""

@@ -25,7 +25,8 @@ CASES = {
 }
 
 
-def build(net, flags, train=True):
+def build(net, flags, train=True, edit=None, **kw):
+    """edit(graph) -> extra Executor arguments (quantization specs); kw: further Executor arguments"""
     import importlib
 
     import torch
@@ -46,10 +47,12 @@ def build(net, flags, train=True):
             out = mh.forward_train(im) if train else mh.forward_eval(im)
             tv = [v for v in g.variables.values() if v.name.startswith('model/') and v.trainable]
             loss, _ = mh.calc_loss(lab, out, tv)
+    if edit is not None:
+        kw.update(edit(g))
     if not train:
-        return Executor(g, im, out, torch.device('cpu'), train=False)
+        return Executor(g, im, out, torch.device('cpu'), train=False, **kw)
     return Executor(g, im, out, torch.device('cpu'), train=True, loss=loss, labels=lab,
-                    optimizer=dict(kind='momentum', momentum=0.9))
+                    optimizer=dict(kind='momentum', momentum=0.9), **kw)
 
 
 def plan_record(ex):
