@@ -354,6 +354,28 @@ int pf_conv2d_tc_fwd_planes(const pf_conv_desc* d, const void* x_hi_dev, const v
                             float* y_dev, void* stream);
 int pf_conv2d_tc_dgrad_planes(const pf_conv_desc* d, const void* dy_hi_dev, const void* dy_lo_dev, const void* wd_hi_dev,
                               const void* wd_lo_dev, int accumulate, float* dx_dev, void* stream);
+/* Inference-mode batch norm of the conv's output, applied in the forward epilogue: after bias, ReLU and the residual
+ * add, the value stored to y_dev also goes through act(((v - mean) * rsqrt(var + eps)) * gamma + beta) with the op
+ * chain (and rounding) of pf_bn_apply_eval, and is stored as split-bf16 planes and / or fp32.  Bit-identical to the
+ * plain forward followed by pf_bn_apply_eval(y_dev, ...); y_dev itself is still written.  Every pointer is a device
+ * pointer: the four per-channel vectors ([Cout] each) and y 16-byte aligned, the planes 8-byte aligned. */
+typedef struct pf_tc_bn_out {
+  const float* mean;       /* moving mean */
+  const float* var;        /* moving variance */
+  const float* gamma;
+  const float* beta;
+  float eps;               /* >= 0 */
+  int32_t act;             /* 0 none, 1 ReLU, 2 ReLU6 */
+  float* y;                /* post-BN fp32 tensor, or NULL */
+  void* hi;                /* post-BN split-bf16 planes (layout of y_dev), or NULL; at least one of y / hi */
+  void* lo;
+} pf_tc_bn_out;
+int pf_conv2d_tc_fwd_bn(const pf_conv_desc* d, const float* x_dev, const void* w_hi_dev, const void* w_lo_dev,
+                        const float* bias_dev, int relu, const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn,
+                        void* stream);
+int pf_conv2d_tc_fwd_planes_bn(const pf_conv_desc* d, const void* x_hi_dev, const void* x_lo_dev, const void* w_hi_dev,
+                               const void* w_lo_dev, const float* bias_dev, int relu, const float* residual_dev,
+                               float* y_dev, const pf_tc_bn_out* bn, void* stream);
 /* dw_dev == NULL: leave the split-K partials [splits][R*S*Cin][Cout] in ws_dev (pf_conv2d_tc_wgrad_splits(d) of
  * them) for ONE deferred pf_conv2d_tc_wgrad_reduce_multi over every layer of the step */
 typedef struct pf_tc_reduce_seg {

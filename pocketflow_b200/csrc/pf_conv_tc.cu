@@ -85,13 +85,13 @@ __device__ __forceinline__ int tile_class(const TcP& p, int mt) {
   return ci;
 }
 
-template <int MODE, bool PLANES, int BN>
+template <int MODE, bool PLANES, int BN, bool BNO = false>
 __global__ void __launch_bounds__(kThreadsP, 1)
 conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __restrict__ a_hi_g,
                        const __nv_bfloat16* __restrict__ a_lo_g, const __nv_bfloat16* __restrict__ b_hi,
                        const __nv_bfloat16* __restrict__ b_lo, float* __restrict__ out,
                        const float* __restrict__ bias, const float* __restrict__ residual,
-                       const __grid_constant__ TcP p) {
+                       const __grid_constant__ TcP p, const __grid_constant__ pf_tc_bn_out bn) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const TcGeom& g = p.g;
@@ -344,9 +344,22 @@ conv_tc_persist_kernel(const float* __restrict__ src, const __nv_bfloat16* __res
           off = (((long long)n_ * g.H + (k.ph + y * g.sh)) * g.W + (k.pw + x * g.sw)) * g.C;
         }
       }
-      wg_tile_to_smem<BN>(acc, acc_s, tid);
-      epilogue_tile(acc_s, warp, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
-                    p.ring ? ring_all + (size_t)warp * kRingDepth * kRingSlotBytes : nullptr);
+      if (BNO) {
+        // wg_tile_to_smem, and between its barriers the folded batch norm's constants of the tile's columns, in the shared
+        // memory after the ring (the J table space of epi_fixed_bytes, which this kernel does not use otherwise)
+        float* bn_tab = reinterpret_cast<float*>(ring_all + (p.ring ? kMmaWarps * kRingDepth * kRingSlotBytes : 0));
+        named_bar_sync(1, kMmaWarps * 32);
+        wgmma_store_acc<BN>(acc, acc_s, acc_pitch(BN), 64 * (tid >> 7), tid & 127);
+        bn_table(bn, bn_tab, n0, BN, p.Ng, tid, kMmaWarps * 32);
+        named_bar_sync(1, kMmaWarps * 32);
+        epilogue_tile_a<0, true>(acc_s, warp, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
+                                 p.ring ? ring_all + (size_t)warp * kRingDepth * kRingSlotBytes : nullptr, EpiAff{},
+                                 0.f, nullptr, bn, bn_tab);
+      } else {
+        wg_tile_to_smem<BN>(acc, acc_s, tid);
+        epilogue_tile(acc_s, warp, off, rowoff, out, extra, bias, p.relu, n0, BN, p.Ng, lane,
+                      p.ring ? ring_all + (size_t)warp * kRingDepth * kRingSlotBytes : nullptr);
+      }
     }
   }
 }
@@ -617,12 +630,14 @@ tc_prep_weights_multi_kernel(const pf_tc_prep_seg* __restrict__ segs, const pf_w
 template <int MODE>
 int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, const void* a_lo, const void* b_hi,
                    const void* b_lo, float* out, const float* bias, const float* residual, cudaStream_t st,
-                   const char* who) {
+                   const char* who, const pf_tc_bn_out* bn) {
   const int Ng = p.Ng;
   // ---- tile width: the widest the warpgroup accumulators allow
   int BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
   const int forced = env_int("PF_TC_BN", 0);           // development knob
   if (forced >= 16 && forced <= kMaxBN && forced <= ((Ng + 15) / 16) * 16 && (forced & (forced - 1)) == 0) BN = forced;
+  // the folded batch norm's epilogue at BN = 128 does not fit the 128 registers per thread of this 512-thread kernel
+  if (bn && BN > 64) BN = 64;
   p.BN = BN;
   p.n_tiles = (Ng + BN - 1) / BN;
   p.total_tiles = p.m_tiles * p.n_tiles;
@@ -667,19 +682,27 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
                          p.b_stationary, p.n_stages, p.total_tiles, grid, 0, 0});
   if (p.total_tiles == 0) return PF_OK;
   cudaError_t err = cudaSuccess;
-  with_bn(BN, [&](auto bn) {
+  pf_tc_bn_out bn_p{};             // the folded batch norm (BNO kernels only)
+  if (bn) bn_p = *bn;
+  with_bn(BN, [&](auto bn_c) {
+    constexpr int B = decltype(bn_c)::value;
     if (a_hi) {
-      auto kern = conv_tc_persist_kernel<MODE, true, decltype(bn)::value>;
+      auto kern = conv_tc_persist_kernel<MODE, true, B>;
+      if constexpr (MODE == 0 && B <= 64)
+        if (bn) kern = conv_tc_persist_kernel<0, true, B, true>;
       err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (err == cudaSuccess)
         kern<<<grid, kThreadsP, smem, st>>>(nullptr, (const __nv_bfloat16*)a_hi, (const __nv_bfloat16*)a_lo,
-                                            (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo, out, bias, residual, p);
+                                            (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo, out, bias, residual, p,
+                                            bn_p);
     } else {
-      auto kern = conv_tc_persist_kernel<MODE, false, decltype(bn)::value>;
+      auto kern = conv_tc_persist_kernel<MODE, false, B>;
+      if constexpr (MODE == 0 && B <= 64)
+        if (bn) kern = conv_tc_persist_kernel<0, false, B, true>;
       err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (err == cudaSuccess)
         kern<<<grid, kThreadsP, smem, st>>>(src, nullptr, nullptr, (const __nv_bfloat16*)b_hi, (const __nv_bfloat16*)b_lo,
-                                            out, bias, residual, p);
+                                            out, bias, residual, p, bn_p);
     }
   });
   PF_CUDA(err);
@@ -690,7 +713,7 @@ int launch_persist(const TcGeom& g, TcP& p, const float* src, const void* a_hi, 
 template <int MODE>
 int launch_tc(const TcGeom& g, const float* src, const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
               float* out, int accumulate, const float* bias, int relu, const float* residual, cudaStream_t st,
-              const char* who) {
+              const char* who, const pf_tc_bn_out* bn = nullptr) {
   const int64_t M64 = (MODE == 0) ? (int64_t)g.N * g.P * g.Q : (int64_t)g.N * g.H * g.W;
   PF_REQUIRE(M64 < (1ll << 31), "%s: too many rows", who);
   TcP p;
@@ -746,9 +769,9 @@ int launch_tc(const TcGeom& g, const float* src, const void* a_hi, const void* a
         ++p.ncls;
       }
     p.m_tiles = tiles;
-    return launch_persist<2>(g, p, src, a_hi, a_lo, b_hi, b_lo, out, bias, residual, st, who);
+    return launch_persist<2>(g, p, src, a_hi, a_lo, b_hi, b_lo, out, bias, residual, st, who, nullptr);
   }
-  return launch_persist<MODE>(g, p, src, a_hi, a_lo, b_hi, b_lo, out, bias, residual, st, who);
+  return launch_persist<MODE>(g, p, src, a_hi, a_lo, b_hi, b_lo, out, bias, residual, st, who, bn);
 }
 
 // multi-tensor split-K reduction: the partials of every wgrad of a step in ONE launch (kind-0 work items)
@@ -848,7 +871,7 @@ int pf_conv2d_tc_prep_weights_multi(const pf_tc_prep_seg* segs_dev, const pf_wor
 
 static int tc_fwd_impl(const pf_conv_desc* d, const float* x_dev, const void* x_hi, const void* x_lo, const void* w_hi_dev,
                        const void* w_lo_dev, const float* bias_dev, int relu, const float* residual_dev, float* y_dev,
-                       void* stream, const char* who) {
+                       void* stream, const char* who, const pf_tc_bn_out* bn = nullptr) {
   TcGeom g;
   int rc = tc_geom(d, &g, who);
   if (rc) return rc;
@@ -857,13 +880,21 @@ static int tc_fwd_impl(const pf_conv_desc* d, const float* x_dev, const void* x_
   PF_REQUIRE((((uintptr_t)x_dev | (uintptr_t)x_hi | (uintptr_t)x_lo | (uintptr_t)y_dev | (uintptr_t)w_hi_dev |
                (uintptr_t)w_lo_dev | (uintptr_t)residual_dev | (uintptr_t)bias_dev) & 15) == 0,
              "%s: 16-byte alignment required", who);
+  if (bn) {
+    PF_REQUIRE(bn->mean && bn->var && bn->gamma && bn->beta && (bn->y || bn->hi), "%s: batch norm: null pointer", who);
+    PF_REQUIRE((bn->hi == nullptr) == (bn->lo == nullptr), "%s: batch norm: planes come in pairs", who);
+    PF_REQUIRE(bn->eps >= 0.f && bn->act >= 0 && bn->act <= 2, "%s: batch norm: eps < 0 or act not in 0..2", who);
+    PF_REQUIRE((((uintptr_t)bn->mean | (uintptr_t)bn->var | (uintptr_t)bn->gamma | (uintptr_t)bn->beta |
+                 (uintptr_t)bn->y) & 15) == 0 && (((uintptr_t)bn->hi | (uintptr_t)bn->lo) & 7) == 0,
+               "%s: batch norm: alignment", who);
+  }
   if (x_hi && conv_tma_eligible(0, g)) {
     const pf_tc_act a{x_hi, x_lo, nullptr, nullptr, 0, 0};
     const pf_tc_wt w{w_hi_dev, w_lo_dev, nullptr, nullptr, 0, 0};
-    return conv_tma_launch(0, g, a, w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who);
+    return conv_tma_launch(0, g, a, w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who, bn);
   }
   return launch_tc<0>(g, x_dev, x_hi, x_lo, w_hi_dev, w_lo_dev, y_dev, 0, bias_dev, relu, residual_dev,
-                      (cudaStream_t)stream, who);
+                      (cudaStream_t)stream, who, bn);
 }
 
 static int tc_dgrad_impl(const pf_conv_desc* d, const float* dy_dev, const void* dy_hi, const void* dy_lo,
@@ -898,6 +929,22 @@ int pf_conv2d_tc_fwd_planes(const pf_conv_desc* d, const void* x_hi_dev, const v
   PF_REQUIRE(x_hi_dev && x_lo_dev, "pf_conv2d_tc_fwd_planes: null pointer");
   return tc_fwd_impl(d, nullptr, x_hi_dev, x_lo_dev, w_hi_dev, w_lo_dev, bias_dev, relu, residual_dev, y_dev, stream,
                      "pf_conv2d_tc_fwd_planes");
+}
+
+int pf_conv2d_tc_fwd_bn(const pf_conv_desc* d, const float* x_dev, const void* w_hi_dev, const void* w_lo_dev,
+                        const float* bias_dev, int relu, const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn,
+                        void* stream) {
+  PF_REQUIRE(x_dev != nullptr && bn != nullptr, "pf_conv2d_tc_fwd_bn: null pointer");
+  return tc_fwd_impl(d, x_dev, nullptr, nullptr, w_hi_dev, w_lo_dev, bias_dev, relu, residual_dev, y_dev, stream,
+                     "pf_conv2d_tc_fwd_bn", bn);
+}
+
+int pf_conv2d_tc_fwd_planes_bn(const pf_conv_desc* d, const void* x_hi_dev, const void* x_lo_dev, const void* w_hi_dev,
+                               const void* w_lo_dev, const float* bias_dev, int relu, const float* residual_dev,
+                               float* y_dev, const pf_tc_bn_out* bn, void* stream) {
+  PF_REQUIRE(x_hi_dev && x_lo_dev && bn, "pf_conv2d_tc_fwd_planes_bn: null pointer");
+  return tc_fwd_impl(d, nullptr, x_hi_dev, x_lo_dev, w_hi_dev, w_lo_dev, bias_dev, relu, residual_dev, y_dev, stream,
+                     "pf_conv2d_tc_fwd_planes_bn", bn);
 }
 
 int pf_conv2d_tc_dgrad(const pf_conv_desc* d, const float* dy_dev, const void* wd_hi_dev, const void* wd_lo_dev,

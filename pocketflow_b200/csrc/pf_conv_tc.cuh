@@ -104,6 +104,14 @@ __device__ __forceinline__ void wg_tile_to_smem(float (&acc)[BN / 2], float* acc
 // the convolution of the fake-quantized tensors is   s_a s_c * sum_k j (n - centre)  +  s_a o_c * J[m],
 // J[m] = sum of the activation levels under the filter window of output row m (computed by the row's thread from
 // per-pixel channel sums and handed in as `my_j`).  AFF 1: only the scalar s_a (weight gradient: j (x) dy).
+// BNO (forward, AFF 0 only): after the fp32 store to `out`, the same register value also goes through the inference
+// batch norm `bn` (pf_b200.h: pf_tc_bn_out) with pf_bn_apply_eval's op chain, and is stored as split-bf16 planes and /
+// or fp32: the BN pass that would re-read `out` is folded into this one.  The tile's column constants come in `aff_tab`
+// (bn_table: rstd, mean, gamma, beta of column c at c, BN + c, 2 BN + c, 3 BN + c), formed by the kernel before the
+// epilogue: __frsqrt_rn has a called slow path, which inside the chunk loop would make ptxas save the loop's live
+// registers to local memory.  BNO loads the residual at each chunk instead of one chunk ahead (the second buffer would
+// not fit the registers beside the constants), and stores `out` with evict-first stores: nothing reads it soon, while
+// the post-BN planes are read by the next convolution.
 constexpr int kRingDepth = 4;
 constexpr int kRingSlotBytes = 32 * 32 * 4;
 
@@ -115,13 +123,14 @@ struct EpiAff {
   float w_rk, w_centre;    // 1 / (2^bits - 1), level subtracted from the stored weight levels
 };
 
-template <int EXTRA, int AFF, int RD = kRingDepth>
+template <int EXTRA, int AFF, int RD = kRingDepth, bool BNO = false>
 __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, int pitch, long long my_row_off,
                                                 long long* __restrict__ rowoff, float* __restrict__ out,
                                                 const float* __restrict__ extra, const float* __restrict__ bias,
                                                 int relu, int n0, int BN, int Ng, int lane, uint8_t* ring,
                                                 const EpiAff& aff, float my_j, float* __restrict__ jrow,
-                                                int c_begin, int c_step, const float* __restrict__ aff_tab) {
+                                                int c_begin, int c_step, const float* __restrict__ aff_tab,
+                                                const pf_tc_bn_out& bn) {
   // aff_tab (AFF == 2, TMA-fed kernels): the tile's per-column epilogue constants e1[c] (at c) and e2[c] (at 256 + c)
   // in shared memory, computed once per tile column range instead of being re-derived from global memory per chunk
   // c_begin / c_step: this warp handles the 32-column chunks c_begin, c_begin + c_step, ...
@@ -166,7 +175,7 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
   float4 xa[8], xb[8];                           // dead (eliminated) unless EXTRA == 1
-  if (EXTRA == 1) load_extra(c_begin, xa);
+  if (EXTRA == 1 && !BNO) load_extra(c_begin, xa);
   if (EXTRA == 2) {
 #pragma unroll
     for (int c = 0; c < RD; ++c) ring_issue(c_begin + c_step * c, c);
@@ -199,7 +208,15 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
       e2 = make_float4(fmaf(aff.w_centre, sx, be.x) * a_s, fmaf(aff.w_centre, sy, be.y) * a_s,
                        fmaf(aff.w_centre, sz, be.z) * a_s, fmaf(aff.w_centre, sw_, be.w) * a_s);
     }
-    if (EXTRA == 1 && c0 + c_step < BN) load_extra(c0 + c_step, xb);
+    float4 brs, bmu, bga, bbe;                   // BNO: the columns' batch-norm constants
+    if (BNO && cok) {
+      brs = *reinterpret_cast<const float4*>(aff_tab + cv);
+      bmu = *reinterpret_cast<const float4*>(aff_tab + BN + cv);
+      bga = *reinterpret_cast<const float4*>(aff_tab + 2 * BN + cv);
+      bbe = *reinterpret_cast<const float4*>(aff_tab + 3 * BN + cv);
+    }
+    if (EXTRA == 1 && !BNO && c0 + c_step < BN) load_extra(c0 + c_step, xb);
+    if (EXTRA == 1 && BNO) load_extra(c0, xa);
     if (EXTRA == 2) asm volatile("cp.async.wait_group %0;" ::"n"(RD - 1) : "memory");   // chunk c0 has landed
     const float* slot = reinterpret_cast<const float*>(ring + (size_t)(it & (RD - 1)) * kRingSlotBytes);
 #pragma unroll
@@ -228,10 +245,21 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
           const float4 x = (EXTRA == 2) ? xr[u] : xa[uu];
           w.x = __fadd_rn(w.x, x.x); w.y = __fadd_rn(w.y, x.y); w.z = __fadd_rn(w.z, x.z); w.w = __fadd_rn(w.w, x.w);
         }
-        *reinterpret_cast<float4*>(out + ((size_t)ro[uu] << 2) + n0 + cv) = w;
+        if (BNO)
+          __stcs(reinterpret_cast<float4*>(out + ((size_t)ro[uu] << 2) + n0 + cv), w);
+        else
+          *reinterpret_cast<float4*>(out + ((size_t)ro[uu] << 2) + n0 + cv) = w;
+        if (BNO) {
+          const int act = bn.act;
+          w.x = pf_bn_act(w.x, bmu.x, brs.x, bga.x, bbe.x, act); w.y = pf_bn_act(w.y, bmu.y, brs.y, bga.y, bbe.y, act);
+          w.z = pf_bn_act(w.z, bmu.z, brs.z, bga.z, bbe.z, act); w.w = pf_bn_act(w.w, bmu.w, brs.w, bga.w, bbe.w, act);
+          const int64_t e = ((int64_t)ro[uu] << 2) + n0 + cv;
+          if (bn.y) *reinterpret_cast<float4*>(bn.y + e) = w;
+          if (bn.hi) pf_st_planes4(bn.hi, bn.lo, e, w);
+        }
       }
     }
-    if (EXTRA == 1) {
+    if (EXTRA == 1 && !BNO) {
 #pragma unroll
       for (int u = 0; u < 8; ++u) xa[u] = xb[u];
     }
@@ -243,37 +271,54 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
   if (EXTRA == 2) asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// the folded batch norm's constants of columns [n0, n0 + BN) into `tab` (4 BN floats): rstd (formed as
+// pf_bn_apply_eval forms it), mean, gamma and beta of column c at c, BN + c, 2 BN + c and 3 BN + c; thread t of `nthr`
+// fills columns t, t + nthr, ...
+__device__ __forceinline__ void bn_table(const pf_tc_bn_out& bn, float* tab, int n0, int BN, int Ng, int t, int nthr) {
+  for (int c = t; c < BN; c += nthr) {
+    const bool ok = n0 + c < Ng;
+    tab[c] = ok ? __frsqrt_rn(__fadd_rn(__ldg(bn.var + n0 + c), bn.eps)) : 0.f;
+    tab[BN + c] = ok ? __ldg(bn.mean + n0 + c) : 0.f;
+    tab[2 * BN + c] = ok ? __ldg(bn.gamma + n0 + c) : 0.f;
+    tab[3 * BN + c] = ok ? __ldg(bn.beta + n0 + c) : 0.f;
+  }
+}
+
 // the epilogue of one warp over 32 rows of the accumulator tile starting at `acc`, 32-column chunks c_begin,
 // c_begin + c_step, ...: picks the residual / accumulate path (none, registers, cp.async ring of depth 2 or 4)
-template <int AFF>
+template <int AFF, bool BNO = false>
 __device__ __forceinline__ void epilogue_rows(const float* acc, int c_begin, int c_step, long long my_row_off,
                                               long long* rowoff, float* __restrict__ out, const float* __restrict__ extra,
                                               const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
                                               int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
-                                              const float* aff_tab, int ring_depth) {
+                                              const float* aff_tab, int ring_depth, const pf_tc_bn_out& bn) {
+  static_assert(!BNO || AFF == 0, "the folded batch norm is an inference-mode (split-bf16 operand) epilogue");
   const int pitch = acc_pitch(BN);
-  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra && ring) epilogue_tile_t<2, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else if (extra) epilogue_tile_t<1, AFF>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
-  else epilogue_tile_t<0, AFF>(acc, pitch, my_row_off, rowoff, out, nullptr, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab);
+  if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2, BNO>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
+  else if (extra && ring) epilogue_tile_t<2, AFF, kRingDepth, BNO>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
+  else if (extra) epilogue_tile_t<1, AFF, kRingDepth, BNO>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
+  else epilogue_tile_t<0, AFF, kRingDepth, BNO>(acc, pitch, my_row_off, rowoff, out, nullptr, bias, relu, n0, BN, Ng, lane, nullptr, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
 }
 
 // the epilogue of warp `ew` (0..7) of the MMA warps: rows 32 (ew % 4) .., chunks ew / 4, ew / 4 + 2, ...
-template <int AFF>
+template <int AFF, bool BNO = false>
 __device__ __forceinline__ void epilogue_tile_a(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
                                                 float* __restrict__ out, const float* __restrict__ extra,
                                                 const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
                                                 int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
-                                                const float* aff_tab = nullptr, int ring_depth = kRingDepth) {
-  epilogue_rows<AFF>(acc_s + (size_t)(32 * (ew & 3)) * acc_pitch(BN), 32 * (ew >> 2), 64, my_row_off, rowoff, out,
-                     extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, aff_tab, ring_depth);
+                                                const pf_tc_bn_out& bn, const float* aff_tab = nullptr,
+                                                int ring_depth = kRingDepth) {
+  epilogue_rows<AFF, BNO>(acc_s + (size_t)(32 * (ew & 3)) * acc_pitch(BN), 32 * (ew >> 2), 64, my_row_off, rowoff,
+                          out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, aff_tab, ring_depth, bn);
 }
 __device__ __forceinline__ void epilogue_tile(const float* acc_s, int ew, long long my_row_off, long long* rowoff,
                                               float* __restrict__ out, const float* __restrict__ extra,
                                               const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
                                               int lane, uint8_t* ring = nullptr) {
   const EpiAff none{};
-  epilogue_tile_a<0>(acc_s, ew, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, none, 0.f, nullptr);
+  const pf_tc_bn_out no_bn{};
+  epilogue_tile_a<0>(acc_s, ew, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, none, 0.f, nullptr,
+                     no_bn);
 }
 
 // dispatch on the tile width (the wgmma N is an immediate): f is called with std::integral_constant<int, BN>
@@ -294,7 +339,8 @@ void record_plan(const pf_tc_plan& p);
 void conv_tma_set_feed(int mode);
 bool conv_tma_eligible(int pass, const TcGeom& g);      // pass: 0 fwd, 1 dgrad, 2 wgrad
 int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_wt& w, float* out, int accumulate,
-                    const float* bias, int relu, const float* residual, cudaStream_t st, const char* who);
+                    const float* bias, int relu, const float* residual, cudaStream_t st, const char* who,
+                    const pf_tc_bn_out* bn = nullptr);
 int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& dy, int BN, int pps, int splits,
                           float* partial, cudaStream_t st, const char* who);
 

@@ -37,6 +37,7 @@ struct TmaP {
   const pf_tc_act_hdr* a_hdr;
   const float* csum;
   int nseg;
+  pf_tc_bn_out bn;                         // BNO kernels: the batch norm folded into the epilogue
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -61,7 +62,7 @@ constexpr int kPingPongWarps = 4;        // arrivals per turn release and per st
 constexpr int kPingPongThreads = (kMmaWarps + 4) * 32;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
-template <int AFF, int BN, int NA, int NB>
+template <int AFF, int BN, int NA, int NB, bool BNO>
 __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, uint32_t stage_bytes,
                                                   uint32_t n_stages, uint64_t* full_bar, uint64_t* empty_bar,
                                                   uint64_t* ml_bar, uint64_t* epi_bar, int* tab_n0, float* out,
@@ -72,8 +73,9 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
   float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
   long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
   float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
-  float* aff_tab = jrow_all + kMmaWarps * 32;               // AFF == 2: e1[256], e2[256] of the staged tile's columns
-  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : 0));
+  // AFF == 2: e1[256], e2[256] of the staged tile's columns; BNO: the folded batch norm's constants of them (bn_table)
+  float* aff_tab = jrow_all + kMmaWarps * 32;
+  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : (BNO ? 4 * kMaxBN : 0)));
   long long* rowoff = rowoff_all + warp * 32;
   float* jrow = jrow_all + warp * 32;
   uint8_t* ring = p.ring ? ring_all + (size_t)warp * p.ring * kRingSlotBytes : nullptr;
@@ -156,7 +158,8 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
     if (wait_turn) mbar_wait_bounded(&epi_bar[wg], turn_ph);            // the staging tile is this warpgroup's
     wgmma_store_acc<BN>(acc[0], acc_s, acc_pitch(BN), 0, wtid);
     wgmma_store_acc<BN>(acc[1], acc_s, acc_pitch(BN), 64, wtid);
-    const int tab_was = AFF == 2 ? *reinterpret_cast<volatile int*>(tab_n0) : 0;
+    constexpr bool TAB = AFF == 2 || BNO;
+    const int tab_was = TAB ? *reinterpret_cast<volatile int*>(tab_n0) : 0;
     if (AFF == 2 && tab_was != n0) {
       // per-column constants of this tile's columns, when they differ from the staged table's (with one n-tile per
       // row of tiles this runs once per CTA):  e1[c] = s_a * alpha_c / k_w ,  e2[c] = s_a * (centre * alpha_c / k_w + beta_c)
@@ -170,16 +173,17 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
         aff_tab[256 + c] = fmaf(p.aff.w_centre, sx, be) * a_s;
       }
     }
+    if (BNO && tab_was != n0) bn_table(p.bn, aff_tab, n0, BN, p.Ng, wtid, 128);
     named_bar_sync(2 + wg, 128);                       // the staged tile (and table) are visible to the warpgroup
-    if (AFF == 2 && tab_was != n0 && wtid == 0) *reinterpret_cast<volatile int*>(tab_n0) = n0;
-    epilogue_rows<AFF>(acc_s + (size_t)(32 * q) * acc_pitch(BN), 0, 32, off, rowoff, out, extra, bias, p.relu, n0, BN,
-                       p.Ng, lane, ring, p.aff, my_j, jrow, AFF == 2 ? aff_tab : nullptr, p.ring);
+    if (TAB && tab_was != n0 && wtid == 0) *reinterpret_cast<volatile int*>(tab_n0) = n0;
+    epilogue_rows<AFF, BNO>(acc_s + (size_t)(32 * q) * acc_pitch(BN), 0, 32, off, rowoff, out, extra, bias, p.relu, n0,
+                            BN, p.Ng, lane, ring, p.aff, my_j, jrow, TAB ? aff_tab : nullptr, p.ring, p.bn);
     __syncwarp();
     if (lane == 0) mbar_arrive(&epi_bar[wg ^ 1]);                         // this warp's reads of the tile are done
   }
 }
 
-template <int AFF, int BN>
+template <int AFF, int BN, bool BNO = false>
 __global__ void __launch_bounds__(kPingPongThreads, 1)
 conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
@@ -188,7 +192,7 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   __shared__ uint64_t full_bar[kTmaMaxStages], empty_bar[kTmaMaxStages], ml_bar[2], epi_bar[2];
-  __shared__ int tab_n0;                              // first column of the AFF == 2 table in shared memory (-1: none)
+  __shared__ int tab_n0;                              // first column of the column table in shared memory (-1: none)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int na = p.na;
   if (p.a_hdr) na = (__ldg(&p.a_hdr->nplanes) == 2) ? 2 : 1;
@@ -250,8 +254,8 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     // the plane counts are fixed for the whole launch: one straight-line mainloop per combination
     setmaxnreg_inc<kConsumerRegs>();
 #define PF_TMA_CONSUMER(NA_, NB_)                                                                                    \
-  conv_tma_consumer<AFF, BN, NA_, NB_>(p, smem, stage_bytes, n_stages, full_bar, empty_bar, ml_bar, epi_bar, &tab_n0, \
-                                       out, bias, residual)
+  conv_tma_consumer<AFF, BN, NA_, NB_, BNO>(p, smem, stage_bytes, n_stages, full_bar, empty_bar, ml_bar, epi_bar,     \
+                                            &tab_n0, out, bias, residual)
     if (na == 2) {
       if (nb == 2) PF_TMA_CONSUMER(2, 2);
       else PF_TMA_CONSUMER(2, 1);
@@ -409,7 +413,7 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_con
       const long long off = em < p.Mtot ? ((long long)un.split * p.Mtot + em) * g.K : -1;
       wg_tile_to_smem<BN>(acc, acc_s, tid);
       epilogue_tile_a<AFF>(acc_s, warp, off, rowoff, partial, nullptr, nullptr, 0, un.n0, BN, g.K, lane, nullptr, p.aff,
-                           0.f, jrow);
+                           0.f, jrow, pf_tc_bn_out{});
     }
     };
     using one = std::integral_constant<int, 1>;
@@ -463,7 +467,8 @@ static int pick_bn(int Ng) {
 
 // pass 0: fwd (a = x planes, b = [Cout][Kpad] weights); pass 1: unit-stride dgrad (a = dy planes, b = [Cin][Kpad_d])
 int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_wt& w, float* out, int accumulate,
-                    const float* bias, int relu, const float* residual, cudaStream_t st, const char* who) {
+                    const float* bias, int relu, const float* residual, cudaStream_t st, const char* who,
+                    const pf_tc_bn_out* bn) {
   TmaP p;
   memset(&p, 0, sizeof(p));
   const int CC = pass == 0 ? g.C : g.K;
@@ -520,10 +525,12 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     aff = 1;
     p.aff.a_scale = &a.hdr->scale;
   }
+  PF_REQUIRE(bn == nullptr || (pass == 0 && aff == 0), "%s: the folded batch norm needs a split-bf16 forward", who);
+  if (bn) p.bn = *bn;
   // ---- shared memory: [stages][accumulator tile, row offsets, J, column constants][residual ring]
   const int stage_max = p.na * (int)kATileBytes + p.nb * BN * 128;
   const bool has_extra = residual != nullptr || accumulate;
-  const int aff_tab_bytes = aff == 2 ? 2 * 256 * 4 : 0;       // the tile's per-column epilogue constants
+  const int aff_tab_bytes = aff == 2 ? 2 * 256 * 4 : (bn ? 4 * kMaxBN * 4 : 0);   // the tile's per-column constants
   const int epi_bytes = epi_fixed_bytes(BN) + aff_tab_bytes;
   // the residual / accumulate operand streams through a per-warp cp.async ring of 4 (else 2) 4 KB chunks when the
   // pipeline keeps enough stages beside it: 3, or nk + 1 for the short reductions of the 1x1 layers (a 64 -> 256 layer
@@ -562,9 +569,10 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   else
     tB1 = tB0;
   cudaError_t err = cudaSuccess;
-  with_bn(BN, [&](auto bn) {
-    constexpr int B = decltype(bn)::value;
-    auto kern = aff == 2 ? conv_tma_kernel<2, B> : (aff == 1 ? conv_tma_kernel<1, B> : conv_tma_kernel<0, B>);
+  with_bn(BN, [&](auto bn_c) {
+    constexpr int B = decltype(bn_c)::value;
+    auto kern = bn ? conv_tma_kernel<0, B, true>
+                   : (aff == 2 ? conv_tma_kernel<2, B> : (aff == 1 ? conv_tma_kernel<1, B> : conv_tma_kernel<0, B>));
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (err == cudaSuccess) kern<<<grid, kPingPongThreads, smem, st>>>(tA0, tA1, tB0, tB1, out, bias, residual, p);
   });

@@ -108,7 +108,6 @@ bn_stats_partial_kernel(const float* __restrict__ x, int M, int C, int rows_per_
 // moments pairwise: four fp64 divisions per split on a GPU with 1/64-rate fp64 — 36 us per launch).
 // kFinalWarps warps per channel stride over the splits; fixed-order shuffle + smem tree: deterministic.
 constexpr int kFinalWarps = 4;
-__device__ __forceinline__ float bn_act(float x, float mu, float rs, float ga, float be, int act);
 __global__ void __launch_bounds__(NT)
 bn_stats_final_kernel(const float* __restrict__ part, int M, int C, int splits, int rows_per_split,
                       float eps, float momentum, float* __restrict__ mean, float* __restrict__ var,
@@ -166,7 +165,7 @@ bn_stats_final_kernel(const float* __restrict__ part, int M, int C, int splits, 
   rstd[c] = rs_;
   if (nf == 5 && minmax_enc && xlo <= xhi) {
     // range of y = act(bn(x)) over this channel: attained at the extremes of x (monotone in x)
-    const float ya = bn_act(xlo, mu, rs_, gamma[c], beta[c], act), yb = bn_act(xhi, mu, rs_, gamma[c], beta[c], act);
+    const float ya = pf_bn_act(xlo, mu, rs_, gamma[c], beta[c], act), yb = pf_bn_act(xhi, mu, rs_, gamma[c], beta[c], act);
     atomicMin(minmax_enc, pf_enc(fminf(ya, yb)));
     atomicMax(minmax_enc + 1, pf_enc(fmaxf(ya, yb)));
   }
@@ -183,14 +182,6 @@ __global__ void __launch_bounds__(NT)
 bn_eval_prepare_kernel(const float* __restrict__ mov_var, int C, float eps, float* __restrict__ rstd) {
   const int c = blockIdx.x * NT + threadIdx.x;
   if (c < C) rstd[c] = __frsqrt_rn(__fadd_rn(mov_var[c], eps));
-}
-
-__device__ __forceinline__ float bn_act(float x, float mu, float rs, float ga, float be, int act) {
-  // ((x - mean) * rstd) * gamma + beta, each op rounded once
-  float y = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(x, mu), rs), ga), be);
-  if (act >= 1) y = fmaxf(y, 0.f);
-  if (act == 2) y = fminf(y, 6.f);
-  return y;
 }
 
 // y = act(bn(x)); optionally accumulates the per-tensor min/max of y (ordered-uint slots)
@@ -224,10 +215,10 @@ bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* 
   const uint32_t step = (uint32_t)((stride << 2) % (uint32_t)C);
   float mn = INFINITY, mx = -INFINITY;
   auto apply4 = [&](float4 v, const float4& mu, const float4& rs, const float4& ga, const float4& be, int64_t idx) {
-    v.x = bn_act(v.x, mu.x, rs.x, ga.x, be.x, act);
-    v.y = bn_act(v.y, mu.y, rs.y, ga.y, be.y, act);
-    v.z = bn_act(v.z, mu.z, rs.z, ga.z, be.z, act);
-    v.w = bn_act(v.w, mu.w, rs.w, ga.w, be.w, act);
+    v.x = pf_bn_act(v.x, mu.x, rs.x, ga.x, be.x, act);
+    v.y = pf_bn_act(v.y, mu.y, rs.y, ga.y, be.y, act);
+    v.z = pf_bn_act(v.z, mu.z, rs.z, ga.z, be.z, act);
+    v.w = pf_bn_act(v.w, mu.w, rs.w, ga.w, be.w, act);
     if (RES) {
       const float4 r = pf_ld_stream(res + (idx << 2));
       v.x = __fadd_rn(v.x, r.x); v.y = __fadd_rn(v.y, r.y); v.z = __fadd_rn(v.z, r.z); v.w = __fadd_rn(v.w, r.w);
@@ -339,15 +330,15 @@ bn_apply_levels_kernel(const float* __restrict__ x, int64_t total, int C, int cs
   auto emit = [&](float4 v, int64_t i, bool valid) {
     float4 lv;
     if (LEVELS_ONLY && lev) {
-      lv.x = pf_quant_level(bn_act(v.x, mu.x, rs.x, ga.x, be.x, act), q_alpha, q_beta, q_k, q_ra);
-      lv.y = pf_quant_level(bn_act(v.y, mu.y, rs.y, ga.y, be.y, act), q_alpha, q_beta, q_k, q_ra);
-      lv.z = pf_quant_level(bn_act(v.z, mu.z, rs.z, ga.z, be.z, act), q_alpha, q_beta, q_k, q_ra);
-      lv.w = pf_quant_level(bn_act(v.w, mu.w, rs.w, ga.w, be.w, act), q_alpha, q_beta, q_k, q_ra);
+      lv.x = pf_quant_level(pf_bn_act(v.x, mu.x, rs.x, ga.x, be.x, act), q_alpha, q_beta, q_k, q_ra);
+      lv.y = pf_quant_level(pf_bn_act(v.y, mu.y, rs.y, ga.y, be.y, act), q_alpha, q_beta, q_k, q_ra);
+      lv.z = pf_quant_level(pf_bn_act(v.z, mu.z, rs.z, ga.z, be.z, act), q_alpha, q_beta, q_k, q_ra);
+      lv.w = pf_quant_level(pf_bn_act(v.w, mu.w, rs.w, ga.w, be.w, act), q_alpha, q_beta, q_k, q_ra);
     } else {
-      v.x = pf_fake_quant_lv(bn_act(v.x, mu.x, rs.x, ga.x, be.x, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.x);
-      v.y = pf_fake_quant_lv(bn_act(v.y, mu.y, rs.y, ga.y, be.y, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.y);
-      v.z = pf_fake_quant_lv(bn_act(v.z, mu.z, rs.z, ga.z, be.z, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.z);
-      v.w = pf_fake_quant_lv(bn_act(v.w, mu.w, rs.w, ga.w, be.w, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.w);
+      v.x = pf_fake_quant_lv(pf_bn_act(v.x, mu.x, rs.x, ga.x, be.x, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.x);
+      v.y = pf_fake_quant_lv(pf_bn_act(v.y, mu.y, rs.y, ga.y, be.y, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.y);
+      v.z = pf_fake_quant_lv(pf_bn_act(v.z, mu.z, rs.z, ga.z, be.z, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.z);
+      v.w = pf_fake_quant_lv(pf_bn_act(v.w, mu.w, rs.w, ga.w, be.w, act), q_alpha, q_beta, q_k, q_ra, q_rk, lv.w);
     }
     const float4 s = lev ? lv : v;
     float part = 0.f;

@@ -66,6 +66,7 @@ class _TcConv(_ConvLowering):
         self.tw, self.xp, self.w_lv = ex.tc[op], ex.planes_of(self.x), ex.w_lv.get(op)
         self.x_lv = ex.act_lv.get(ex._root(self.x).op) if self.xp is not None else None
         self.res = ex.fused_add[op][1] if op in ex.fused_add else None
+        self.bn = ex.bn_fold.get(op)     # inference BN applied to the output in the epilogue (Executor._plan_bn_fold)
         self.tc_wgrad = op in ex.tc_wgrad
         if self.tc_wgrad:
             self.xw = ops.Planes(self.x.numel, ex.device, ex.x_scratch.buf) if self.xp is None else self.xp
@@ -91,12 +92,25 @@ class _TcConv(_ConvLowering):
     def prepare_weights(self):
         self.tw.prepare(self.ex.kernel_of(self.op))
 
+    def _bn_out(self):
+        """the folded BN's parameters and outputs: the planes of its consumers and the fp32 tensor where the BN apply
+        would write them"""
+        bn, ex = self.bn, self.ex
+        st, pl = ex.store, ex.xplanes.get(bn)
+        y = ex.buf[bn.output] if pl is None or ex.bn_need_f32[bn] else None
+        return ops.TcBnOut(st.view(bn.vars['moving_mean']), st.view(bn.vars['moving_variance']), bn.attrs['epsilon'],
+                           st.view(bn.vars['gamma']), st.view(bn.vars['beta']), ex.fused_act.get(bn, 0), y, pl)
+
     def forward(self):
         ex = self.ex
         res = ex.T(self.res) if self.res is not None else None
         with ex.timed('conv_fwd'):
             if self._levels():
                 ops.conv2d_tc_fwd_ex(self.d, self._x_act(), self._wt(), *self._epilogue(), res)
+            elif self.bn is not None:
+                fwd = ops.conv2d_tc_fwd_planes if self.xp is not None else ops.conv2d_tc_fwd
+                fwd(self.d, self.xp if self.xp is not None else ex.T(self.x), self.tw, *self._epilogue(), res,
+                    self._bn_out())
             elif self.xp is not None:
                 ops.conv2d_tc_fwd_planes(self.d, self.xp, self.tw, *self._epilogue(), res)
             else:
@@ -817,9 +831,37 @@ class Executor:
                 self._ste_grads = None
             self.beta1_power = F32(self.optimizer.get('beta1', 0.9))
             self.beta2_power = F32(self.optimizer.get('beta2', 0.999))
+        self.bn_fold = self._plan_bn_fold()
+        self._bn_folded = set(self.bn_fold.values())
         # ---- how each Conv2D / MatMul runs forward, backward and in layer_wgrad
         self.conv = {op: (_StemConv if op in self.im2col else _TcConv if op in self.tc else _ConvLowering)(self, op)
                      for op in self.ops if op.type in ('Conv2D', 'MatMul')}
+
+    def _plan_bn_fold(self):
+        """{tensor-core conv op: inference-mode BatchNorm op} of the BNs applied in the epilogue of the conv that
+        produces their input (the conv's own output, or the residual Add fused into it): the BN apply pass, which reads
+        the conv's fp32 output back, is not launched.  Only in inference executors on the GPU (the distillation teacher,
+        evaluation); training executors, and executors planned on the CPU (the golden plan snapshots), fold nothing.
+        Excluded: the stem (its output is not a tensor-core conv's) and BNs that already have a fused form (bn_add,
+        bn_gather) or feed an activation quantizer."""
+        fold = {}
+        if self.train or self.device.type != 'cuda':
+            return fold
+        add_conv = {a: c for c, (a, _) in self.fused_add.items()}
+        for op in self.ops:
+            if op.type != 'FusedBatchNorm' or op.attrs['training'] or op in self.bn_add or op in self.bn_gather:
+                continue
+            x, r = op.inputs[0], self._root(op.inputs[0])         # through Identity / Reshape / a fused ReLU
+            if r is None or r.shape[-1] != x.shape[-1]:
+                continue
+            conv = r.op if r.op.type == 'Conv2D' else add_conv.get(r.op)
+            if conv is None or conv not in self.tc or conv in self.im2col or conv in fold:
+                continue
+            act = self.fused_act.get(op, 0)
+            if act and self._consumers(op.output)[0] in self.aq_index:
+                continue
+            fold[conv] = op
+        return fold
 
     # ------------------------------------------------------------------ profiling (bench.py roofline)
     class _Timed:
@@ -962,6 +1004,8 @@ class Executor:
                 else:
                     with self.timed('bn_apply'):
                         ops.bn_apply_add_eval(x, m, c, mm, mv, op.attrs['epsilon'], gamma, beta, self.T(other), y_out, pl)
+            elif ty == 'FusedBatchNorm' and op in self._bn_folded:
+                continue                                   # applied by the producing conv's epilogue
             elif ty == 'FusedBatchNorm' and op in self.bn_gather:
                 gop = self.bn_gather[op]
                 x = self.T(op.inputs[0])

@@ -64,6 +64,8 @@ SIGNATURES = {
     'pf_conv2d_tc_wgrad_planes_workspace_bytes': (c_i64, [c_vp]),
     'pf_conv2d_tc_fwd_planes': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),
     'pf_conv2d_tc_dgrad_planes': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
+    'pf_conv2d_tc_fwd_bn': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    'pf_conv2d_tc_fwd_planes_bn': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_conv2d_tc_wgrad_planes': (c_i32, [c_vp] * 8),
     'pf_conv2d_tc_tma_supported': (c_i32, [c_vp, c_i32]),
     'pf_conv2d_tc_set_feed': (c_i32, [c_i32]),
@@ -144,6 +146,12 @@ class TcWt(ctypes.Structure):
     """pf_tc_wt: weight operand (split-bf16 planes, or integer levels + the quantizer's bucket scales)."""
     _fields_ = [('plane0', c_vp), ('plane1', c_vp), ('alpha', c_vp), ('beta', c_vp), ('per_channel', c_i32),
                 ('bits', c_i32)]
+
+
+class TcBnOut(ctypes.Structure):
+    """pf_tc_bn_out: the inference batch norm a forward tensor-core conv applies to its output in the epilogue."""
+    _fields_ = [('mean', c_vp), ('var', c_vp), ('gamma', c_vp), ('beta', c_vp), ('eps', c_f32), ('act', c_i32),
+                ('y', c_vp), ('hi', c_vp), ('lo', c_vp)]
 
 
 class TcPlan(ctypes.Structure):

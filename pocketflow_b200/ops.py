@@ -948,9 +948,26 @@ class TcWeightsBatch:
                                                                _stream()), 'pf_conv2d_tc_prep_weights_multi')
 
 
-def conv2d_tc_fwd(d, x, tw, bias, relu, y, residual=None):
-    _lib.check(_lib.load().pf_conv2d_tc_fwd(ctypes.byref(d), _p(x), _p(tw.f_hi), _p(tw.f_lo), _p(bias),
-                                            int(bool(relu)), _p(residual), _p(y), _stream()), 'pf_conv2d_tc_fwd')
+def conv2d_tc_fwd(d, x, tw, bias, relu, y, residual=None, bn_out=None):
+    """bn_out (TcBnOut): also apply that inference batch norm to the output in the epilogue (y is still written)"""
+    if bn_out is None:
+        _lib.check(_lib.load().pf_conv2d_tc_fwd(ctypes.byref(d), _p(x), _p(tw.f_hi), _p(tw.f_lo), _p(bias),
+                                                int(bool(relu)), _p(residual), _p(y), _stream()), 'pf_conv2d_tc_fwd')
+    else:
+        _lib.check(_lib.load().pf_conv2d_tc_fwd_bn(ctypes.byref(d), _p(x), _p(tw.f_hi), _p(tw.f_lo), _p(bias),
+                                                   int(bool(relu)), _p(residual), _p(y), ctypes.byref(bn_out),
+                                                   _stream()), 'pf_conv2d_tc_fwd_bn')
+
+
+class TcBnOut(_lib.TcBnOut):
+    """pf_tc_bn_out of tensors: act(bn(.)) with the moving statistics (pf_bn_apply_eval's arithmetic), written to the
+    fp32 tensor y and / or the operand planes `planes` by the forward conv whose output it normalizes"""
+
+    def __init__(self, mean, var, eps, gamma, beta, act, y=None, planes=None):
+        super().__init__(mean.data_ptr(), var.data_ptr(), gamma.data_ptr(), beta.data_ptr(), float(eps), int(act),
+                         y.data_ptr() if y is not None else None, planes.hi.data_ptr() if planes is not None else None,
+                         planes.lo.data_ptr() if planes is not None else None)
+        self._keep = (mean, var, gamma, beta, y, planes)
 
 
 def conv2d_tc_dgrad(d, dy, tw, accumulate, dx):
@@ -991,10 +1008,16 @@ def split_bf16(src, planes):
     _lib.check(_lib.load().pf_split_bf16(_p(src), _p(planes.hi), _p(planes.lo), src.numel(), _stream()), 'pf_split_bf16')
 
 
-def conv2d_tc_fwd_planes(d, xp, tw, bias, relu, y, residual=None):
-    _lib.check(_lib.load().pf_conv2d_tc_fwd_planes(ctypes.byref(d), _p(xp.hi), _p(xp.lo), _p(tw.f_hi), _p(tw.f_lo), _p(bias),
-                                                   int(bool(relu)), _p(residual), _p(y), _stream()),
-               'pf_conv2d_tc_fwd_planes')
+def conv2d_tc_fwd_planes(d, xp, tw, bias, relu, y, residual=None, bn_out=None):
+    """bn_out: as conv2d_tc_fwd"""
+    if bn_out is None:
+        _lib.check(_lib.load().pf_conv2d_tc_fwd_planes(ctypes.byref(d), _p(xp.hi), _p(xp.lo), _p(tw.f_hi), _p(tw.f_lo),
+                                                       _p(bias), int(bool(relu)), _p(residual), _p(y), _stream()),
+                   'pf_conv2d_tc_fwd_planes')
+    else:
+        _lib.check(_lib.load().pf_conv2d_tc_fwd_planes_bn(ctypes.byref(d), _p(xp.hi), _p(xp.lo), _p(tw.f_hi), _p(tw.f_lo),
+                                                          _p(bias), int(bool(relu)), _p(residual), _p(y),
+                                                          ctypes.byref(bn_out), _stream()), 'pf_conv2d_tc_fwd_planes_bn')
 
 
 def conv2d_tc_dgrad_planes(d, dyp, tw, accumulate, dx):
