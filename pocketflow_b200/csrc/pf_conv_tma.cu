@@ -32,6 +32,7 @@ struct TmaP {
   int base_w, base_h, str_w, str_h, flip;  // window origin of row (y, x): (base + x * str); flip: tap offsets mirrored
   int na, nb;                              // operand planes (na: upper bound when a_hdr decides)
   int accumulate, relu, ring, stage_budget;     // ring: 0 = none, else the residual ring's depth (2 or 4)
+  int chunked;                             // 1: the staging tile holds one 32-column chunk (fwd / dgrad, see the launcher)
   FastDiv d_hw, d_w, d_ntiles, d_cblocks, d_s;
   EpiAff aff;
   const pf_tc_act_hdr* a_hdr;
@@ -62,6 +63,37 @@ constexpr int kPingPongWarps = 4;        // arrivals per turn release and per st
 constexpr int kPingPongThreads = (kMmaWarps + 4) * 32;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
+// The epilogue of a 128 x 128 tile through a staging tile of one 32-column chunk (128 x 36 floats, 18 KB instead of
+// 66 KB): for each chunk, the warpgroup stores that chunk's accumulator fragments, and warp q runs the shared epilogue
+// (epilogue_rows) on rows 32 q .. + 32 of it, with the chunk's columns as the tile.  The values and the op chain are
+// those of the whole-tile epilogue, so the bits are too.  Only split-bf16 / bf16 tiles (AFF 0) without a residual /
+// accumulate operand and without a folded batch norm take this path (the launcher decides): the whole-tile epilogue
+// prefetches that operand one chunk ahead, which a chunk at a time cannot, and the batch-norm epilogue does not fit
+// the registers beside the accumulator chunks still held (6.5 KB of spills).  Warpgroup-local barriers order each
+// chunk's stores after the previous chunk's reads and before its own reads.
+__device__ __forceinline__ void conv_tma_epilogue_chunked(float (&acc)[2][64], const TmaP& p, float* acc_s,
+                                                          int n0, long long off, long long* rowoff, float* out,
+                                                          const float* bias, int wg, int q, int lane) {
+  constexpr int P = acc_pitch(32);
+  float* r0 = acc_s + (size_t)(16 * q + (lane >> 2)) * P + 2 * (lane & 3);
+#pragma unroll
+  for (int ch = 0; ch < 4; ++ch) {
+    if (ch > 0) named_bar_sync(2 + wg, 128);      // every warp has read the previous chunk
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * ch + jj;
+        *reinterpret_cast<float2*>(r0 + (size_t)(64 * h) * P + 8 * jj) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+        *reinterpret_cast<float2*>(r0 + (size_t)(64 * h + 8) * P + 8 * jj) =
+            make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+      }
+    named_bar_sync(2 + wg, 128);                  // the chunk is visible to the warpgroup
+    epilogue_rows<0>(acc_s + (size_t)(32 * q) * P, 0, 32, off, rowoff, out, nullptr, bias, p.relu, n0 + 32 * ch, 32,
+                     p.Ng, lane, nullptr, p.aff, 0.f, nullptr, nullptr, 0, p.bn);
+  }
+}
+
 template <int AFF, int BN, int NA, int NB, bool BNO>
 __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, uint32_t stage_bytes,
                                                   uint32_t n_stages, uint64_t* full_bar, uint64_t* empty_bar,
@@ -71,7 +103,7 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
   const int wg = warp >> 2, q = warp & 3, wtid = tid & 127;   // epilogue rows [32 q, 32 q + 32) of the tile
   const uint32_t b_bytes = (uint32_t)BN * 128u;
   float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
-  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(p.chunked ? 32 : BN));
   float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
   // AFF == 2: e1[256], e2[256] of the staged tile's columns; BNO: the folded batch norm's constants of them (bn_table)
   float* aff_tab = jrow_all + kMmaWarps * 32;
@@ -156,9 +188,17 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
       my_j = (a0 + a1) + (a2 + a3);
     }
     if (wait_turn) mbar_wait_bounded(&epi_bar[wg], turn_ph);            // the staging tile is this warpgroup's
+    constexpr bool TAB = AFF == 2 || BNO;
+    if constexpr (BN == 128 && AFF == 0 && !BNO) {
+      if (p.chunked) {
+        conv_tma_epilogue_chunked(acc, p, acc_s, n0, off, rowoff, out, bias, wg, q, lane);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&epi_bar[wg ^ 1]);                     // this warp's reads of the tile are done
+        continue;
+      }
+    }
     wgmma_store_acc<BN>(acc[0], acc_s, acc_pitch(BN), 0, wtid);
     wgmma_store_acc<BN>(acc[1], acc_s, acc_pitch(BN), 64, wtid);
-    constexpr bool TAB = AFF == 2 || BNO;
     const int tab_was = TAB ? *reinterpret_cast<volatile int*>(tab_n0) : 0;
     if (AFF == 2 && tab_was != n0) {
       // per-column constants of this tile's columns, when they differ from the staged table's (with one n-tile per
@@ -549,9 +589,23 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     }
     if (p.ring) budget = (kSmemLimit - epi_bytes - ring_bytes) / 1024 * 1024;
   }
+  // a split-bf16 / bf16 128 x 128 tile without a residual / accumulate operand or a folded batch norm goes through the
+  // staging tile one 32-column chunk at a time when the 48 KB saved buy the pipeline another stage the k-loop can use
+  // (split x split: 3 stages instead of 2)
+  int used_epi = epi_bytes;
+  p.chunked = 0;
+  if (BN == 128 && aff == 0 && !bn && !has_extra && p.nk >= 3) {
+    const int chunk_epi = epi_fixed_bytes(32);
+    const int chunk_budget = (kSmemLimit - chunk_epi) / 1024 * 1024;
+    if (budget / stage_max < 3 && chunk_budget / stage_max > budget / stage_max) {
+      p.chunked = 1;
+      budget = chunk_budget;
+      used_epi = chunk_epi;
+    }
+  }
   PF_REQUIRE(budget / stage_max >= 2 || p.nk <= 1, "%s: shared-memory plan failed (BN %d)", who, BN);
   p.stage_budget = budget;
-  const size_t smem = (size_t)budget + epi_bytes + (p.ring ? ring_bytes : 0);
+  const size_t smem = (size_t)budget + used_epi + (p.ring ? ring_bytes : 0);
   const int grid = std::min(p.total_tiles, PF_NUM_SMS);
   record_plan(pf_tc_plan{0, 1, pass, 0, BN, aff, p.na, p.nb, 0, p.ring, 0, budget, p.total_tiles, grid, 0, 0});
   if (p.total_tiles == 0) return PF_OK;
