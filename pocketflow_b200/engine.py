@@ -66,7 +66,7 @@ class _TcConv(_ConvLowering):
         self.tw, self.xp, self.w_lv = ex.tc[op], ex.planes_of(self.x), ex.w_lv.get(op)
         self.x_lv = ex.act_lv.get(ex._root(self.x).op) if self.xp is not None else None
         self.res = ex.fused_add[op][1] if op in ex.fused_add else None
-        self.bn = ex.bn_fold.get(op)     # inference BN applied to the output in the epilogue (Executor._plan_bn_fold)
+        self.bn_out = ex.batch_norm[ex.bn_fold[op]].bn_out if op in ex.bn_fold else None    # folded BN (_BnFolded)
         self.tc_wgrad = op in ex.tc_wgrad
         if self.tc_wgrad:
             self.xw = ops.Planes(self.x.numel, ex.device, ex.x_scratch.buf) if self.xp is None else self.xp
@@ -92,29 +92,16 @@ class _TcConv(_ConvLowering):
     def prepare_weights(self):
         self.tw.prepare(self.ex.kernel_of(self.op))
 
-    def _bn_out(self):
-        """the folded BN's parameters and outputs: the planes of its consumers and the fp32 tensor where the BN apply
-        would write them"""
-        bn, ex = self.bn, self.ex
-        st, pl = ex.store, ex.xplanes.get(bn)
-        y = ex.buf[bn.output] if pl is None or ex.bn_need_f32[bn] else None
-        return ops.TcBnOut(st.view(bn.vars['moving_mean']), st.view(bn.vars['moving_variance']), bn.attrs['epsilon'],
-                           st.view(bn.vars['gamma']), st.view(bn.vars['beta']), ex.fused_act.get(bn, 0), y, pl)
-
     def forward(self):
         ex = self.ex
         res = ex.T(self.res) if self.res is not None else None
         with ex.timed('conv_fwd'):
             if self._levels():
                 ops.conv2d_tc_fwd_ex(self.d, self._x_act(), self._wt(), *self._epilogue(), res)
-            elif self.bn is not None:
-                fwd = ops.conv2d_tc_fwd_planes if self.xp is not None else ops.conv2d_tc_fwd
-                fwd(self.d, self.xp if self.xp is not None else ex.T(self.x), self.tw, *self._epilogue(), res,
-                    self._bn_out())
             elif self.xp is not None:
-                ops.conv2d_tc_fwd_planes(self.d, self.xp, self.tw, *self._epilogue(), res)
+                ops.conv2d_tc_fwd_planes(self.d, self.xp, self.tw, *self._epilogue(), res, self.bn_out)
             else:
-                ops.conv2d_tc_fwd(self.d, ex.T(self.x), self.tw, *self._epilogue(), res)
+                ops.conv2d_tc_fwd(self.d, ex.T(self.x), self.tw, *self._epilogue(), res, self.bn_out)
 
     def wgrad(self, gy, ws, dw=None, dy_buf=None):
         if not self.tc_wgrad:
@@ -193,6 +180,104 @@ class _StemConv(_ConvLowering):
             ops.gather_rows(im['dwpad'], im['bwd_map'], dw, dw.shape[-1])
         else:
             ops.add(im['dwpad'][:dw.numel()], None, dw.reshape(-1))
+
+
+class _BnLowering:
+    """How one FusedBatchNorm runs, fixed at plan time; this class: the apply, with the quantizer of its fused ReLU in
+    the same pass (integer levels where it writes them).  `writes`: the op whose fp32 output / planes it writes."""
+
+    def __init__(self, ex, op, writes=None):
+        st, s = ex.store, ex.bn[op]
+        self.ex, self.op, self.x = ex, op, op.inputs[0]
+        c = op.output.shape[-1]
+        m = op.output.numel // c
+        gamma, beta = st.view(op.vars['gamma']), st.view(op.vars['beta'])
+        mm, mv, eps = st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance']), op.attrs['epsilon']
+        momentum = op.attrs['momentum'] if ex.update_moving_stats else 1.0
+        self.act = ex.fused_act.get(op, 0)
+        self.y, (self.y_out, self.pl) = ex.buf[op.output], ex.outputs_of(writes or op)
+        # the activation quantizer (an index into act_quant['bits'], which set_quant_bits changes) and its levels
+        self.aq, self.lv = ex._aq_of_bn(op), ex.act_lv.get(op)
+        self.slot = ex.aq_slots[self.aq] if self.aq is not None else None
+        # launch arguments after x: statistics pass (which with a quantizer also yields the range of act(bn(x))),
+        # batch-statistics apply (training), moving-statistics apply and its outputs (with a quantizer: fp32 + range)
+        q = (gamma, beta, self.act, self.slot) if self.slot is not None else ()
+        self.stats = (m, c, eps, momentum, s['mean'], s['var'], s['rstd'], mm, mv) + q
+        self.batch = (m, c, s['mean'], s['rstd'], gamma, beta)
+        self.moving = (m, c, mm, mv, eps, gamma, beta)
+        self.eval_out = (self.y, self.slot, None) if self.slot is not None else (self.y_out, None, self.pl)
+        if ex.train:
+            self.dparams = st.view(op.vars['gamma'], ex.G), st.view(op.vars['beta'], ex.G)
+            self.gp = ex.bn_gplanes.get(op)                          # the dy planes of the conv that reads dL/dx
+            self.only = self.gp is not None and ex.bn_gplanes_only[op]
+
+    def forward(self, training):
+        """the one per-pass choice: batch statistics in training passes of a training-mode BN, else moving statistics"""
+        ex, x = self.ex, self.ex.T(self.x)
+        batch_stats = self.op.attrs['training'] and training
+        if batch_stats:
+            with ex.timed('bn_stats'):
+                (ops.bn_train_stats if self.slot is None else ops.bn_train_stats_range)(x, *self.stats, ex.bn_ws)
+        with ex.timed('bn_apply'):
+            self._apply(x, batch_stats)
+        if self.slot is not None and not batch_stats:     # the BN apply wrote fp32 (+ range), the quantizer the planes
+            with ex.timed('act_quant'):
+                ops.act_quant(self.y, self.y_out, self.slot, ex.act_quant['bits'][self.aq], self.pl)
+
+    def _apply(self, x, batch_stats):
+        bits = self.ex.act_quant['bits'][self.aq] if self.slot is not None else None
+        if not batch_stats:
+            ops.bn_apply_eval(x, *self.moving, self.act, *self.eval_out)
+        elif self.slot is None:
+            ops.bn_apply(x, *self.batch, self.act, self.y_out, None, self.pl)
+        elif self.ex._lv_on and self.lv is not None:
+            ops.bn_apply_quant_levels(x, *self.batch, self.act, self.slot, bits, self.y_out, self.pl, self.lv['hdr'],
+                                      self.lv['csum'])
+        else:
+            ops.bn_apply_quant(x, *self.batch, self.act, self.slot, bits, self.y_out, self.pl)
+
+    def backward(self, gy):
+        gx, acc = self.ex.grad_target(self.x)
+        assert not (self.only and acc)
+        with self.ex.timed('bn_bwd'):
+            ops.bn_bwd(gy, self.ex.T(self.x), *self.batch, self.act, *self.dparams, None if self.only else gx, acc,
+                       self.ex.bn_ws, self.gp)
+
+
+class _BnAdd(_BnLowering):
+    """Linear bottleneck (Executor.bn_add): bn(x) + shortcut, written as the residual Add's output."""
+
+    def __init__(self, ex, op):
+        add_op, self.other = ex.bn_add[op]
+        super().__init__(ex, op, add_op)
+
+    def _apply(self, x, batch_stats):
+        if batch_stats:
+            ops.bn_apply_add(x, *self.batch, self.ex.T(self.other), self.y_out, self.pl)
+        else:
+            ops.bn_apply_add_eval(x, *self.moving, self.ex.T(self.other), self.y_out, self.pl)
+
+
+class _BnGather(_BnLowering):
+    """Inference-mode BN (+ activation) that writes the channel gather reading it (Executor.bn_gather)."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op, ex.bn_gather[op])
+        self.idx = ex.gather_idx[ex.bn_gather[op]]
+
+    def _apply(self, x, batch_stats):
+        ops.bn_apply_eval_gather(x, *self.moving, self.act, self.idx, self.y_out, self.pl)
+
+
+class _BnFolded(_BnLowering):
+    """Inference-mode BN that the conv producing its input applies in its epilogue (Executor.bn_fold), from `bn_out`."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op)
+        self.bn_out = ops.TcBnOut(*self.moving[2:], self.act, self.y_out, self.pl)
+
+    def forward(self, training):
+        """applied by the producing conv's epilogue"""
 
 
 class ParamStore:
@@ -415,7 +500,7 @@ class Executor:
         self.aq_out = {}           # relu op -> out-of-place quantized buffer (producer is not BN)
         # quantized weights live in a flat buffer with the same offsets as the parameters
         self.QW = torch.zeros(st.n_train, dtype=torch.float32, device=dev) if self.wq_ops else None
-        self.wq = None
+        self.wq, self.train_clusters = None, False
         if self.wq_ops:
             kvars = [op.vars['kernel'] for op in self.wq_ops]
             srcs = [st.view(v) for v in kvars]
@@ -582,101 +667,10 @@ class Executor:
                     self.add_fused.add(op)
                     self.buf[x_t] = self.buf[op.output]       # the conv output IS the add output
                     break
-        # ---- linear bottleneck: a BatchNorm without activation whose only consumer is a residual Add (MobileNet-v2's
-        # projection, conv_blocks.py:289-313) writes bn(x) + shortcut straight into the Add's buffer (and / or the
-        # Add's operand planes, below) — one pass instead of BN apply + add + split
-        self.bn_add = {}           # BN op -> (add op, other input tensor)
-        fuse_bn_add = os.environ.get('PF_FUSE_BN_ADD', '1') != '0'
-        for op in self.ops:
-            if op.type != 'Add' or op in self.add_fused or not fuse_bn_add:
-                continue
-            for i, x_t in enumerate(op.inputs):
-                src, other = x_t.op, op.inputs[1 - i]
-                if src.type == 'FusedBatchNorm' and src not in self.fused_act and x_t not in self.alias \
-                        and self._consumers(x_t) == [op] and other is not x_t \
-                        and self.g.ops.index(other.op) < self.g.ops.index(src):
-                    self.bn_add[src] = (op, other)
-                    self.add_fused.add(op)
-                    self.buf[x_t] = self.buf[op.output]       # the BN output IS the add output
-                    break
-        # ---- split-bf16 operand planes (tensor-core path): the BN-apply / activation-quantizer that produces a conv
-        # input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
-        # the fp32 copy is only written when some other consumer needs it
-        self.xplanes, self.bn_need_f32 = {}, {}
-        for op in self.ops:
-            if op in self.tc and op not in self.im2col:
-                r = self._root(op.inputs[0])
-                if r is not None and (r.op.type in ('FusedBatchNorm', 'GatherChannels') or r.op in self._add_of_bn()) \
-                        and r.numel % 8 == 0:
-                    if r.op not in self.xplanes:
-                        self.xplanes[r.op] = ops.Planes(r.numel, dev)
-                        self.bn_need_f32[r.op] = False
-                elif self.train:
-                    max_x = max(max_x, op.inputs[0].numel)
-        for bn_op in self.xplanes:
-            ts = [bn_op.output] + [c.output for c in self._consumers(bn_op.output) if c in self.fused_into]
-            for t in ts:
-                for c in self._consumers(t):
-                    if c in self.fused_into and self.fused_into[c] is bn_op:
-                        continue
-                    if not (c in self.tc and c not in self.im2col and (not self.train or c in self.tc_wgrad)):
-                        self.bn_need_f32[bn_op] = True
-        # ---- channel gathers of a compact (channel-pruned) graph, compact.py: a GatherChannels op writes its
-        # consumer's operand planes (above); when it is the only reader of an inference-mode BN (+ activation), the BN
-        # apply writes the gathered tensor itself and the full-width BN output is never materialised
-        self.gather_idx, self.bn_gather = {}, {}
-        for op in self.ops:
-            if op.type != 'GatherChannels':
-                continue
-            self.gather_idx[op] = torch.from_numpy(np.ascontiguousarray(op.attrs['index'], np.int32)).to(dev)
-            t = op.inputs[0]
-            bn = t.op.inputs[0].op if t.op in self.fused_into else t.op
-            if bn.type == 'FusedBatchNorm' and not bn.attrs['training'] and bn not in self.bn_add \
-                    and bn not in self.xplanes and self._consumers(t) == [op] \
-                    and (t.op is bn or self._consumers(bn.output) == [t.op]) and t.op not in self.aq_index:
-                self.bn_gather[bn] = op
-        self.gather_fused = set(self.bn_gather.values())
-        # ---- integer-level operands (TMA-fed kernels, SURVEY §7 hard part 1b): a <= 8-bit fake-quantized tensor is
-        # exactly scale * level, and the levels are exact in bf16 — one operand plane instead of hi + lo, one MMA per
-        # k-slice instead of three (two against a split gradient).  Activation side: the fused BN + ReLU + fake-quant
-        # pass writes levels + a device header + per-pixel channel sums when EVERY consumer of its planes is a TMA-fed
-        # kernel.  Weight side: the preparation launch derives the levels from the unquantized kernel with the
-        # quantizer's own op chain; needs per-layer / per-output-channel buckets and the input's channel sums.
-        self.act_lv, self.w_lv = {}, {}
-        use_lv = os.environ.get('PF_TC_LEVELS', '1') != '0' and self.train and dev.type == 'cuda'
-        if use_lv and self.aq_ops:
-            cons = {}
-            for op in self.ops:
-                if op in self.tc and op not in self.im2col:
-                    r = self._root(op.inputs[0])
-                    if r is not None and r.op in self.xplanes:
-                        cons.setdefault(r.op, []).append(op)
-            for bn_op, users in cons.items():
-                act = self.fused_act.get(bn_op, 0)
-                relu_op = self._consumers(bn_op.output)[0] if act else None
-                c = bn_op.output.shape[-1]
-                if relu_op not in self.aq_index or not bn_op.attrs['training'] or c < 16 or (c & (c - 1)):
-                    continue
-                if all(ops.conv2d_tc_tma_supported(self.desc[u], 0) and u in self.tc_wgrad
-                       and ops.conv2d_tc_tma_supported(self.desc[u], 2) for u in users):
-                    m = bn_op.output.numel // c
-                    nseg = (c + 127) // 128
-                    self.act_lv[bn_op] = dict(hdr=torch.zeros(2, dtype=torch.int32, device=dev),
-                                              csum=E((m * nseg,)), nseg=nseg)
-            wq = self.weight_quant
-            if self.wq is not None and isinstance(self.wq, ops.UniformWeightQuantizer) and \
-                    (not wq.get('use_buckets', False) or wq.get('bucket_type', 'channel') == 'channel'):
-                nbk = self.wq.n_buckets
-                for i, op in enumerate(self.wq_ops):
-                    if op not in self.tc or op in self.im2col or op.type != 'Conv2D':
-                        continue
-                    r = self._root(op.inputs[0])
-                    if r is None or r.op not in self.act_lv or not 1 <= self.wq.bits[i] <= 8:
-                        continue
-                    b0, ncols = int(self.wq.segs[i]['bucket0']), int(self.wq.segs[i]['ncols'])
-                    sc = self.wq.scales
-                    self.w_lv[op] = dict(index=i, ncols=ncols, alpha=sc[b0:b0 + ncols], beta=sc[nbk + b0:nbk + b0 + ncols],
-                                         ralpha=sc[2 * nbk + b0:2 * nbk + b0 + ncols])
+        self._plan_bn_add()
+        readers = self._plan_operand_planes()
+        self._plan_bn_gather()
+        self._plan_levels(readers, E)
         # one launch refreshes the split-bf16 copies of all (trainable) conv kernels
         self.tc_batch = None
         if self.tc and not self.static_weights:
@@ -766,41 +760,7 @@ class Executor:
                     self.gbuf[t] = E(t.shape)
                 if op.type in ('Conv2D', 'MatMul') and op in self.fused_act:
                     self.relu_scratch[op] = E(t.shape)
-            # ---- dy operand planes.  For every tensor-core conv, the LAST op that writes the gradient of its output
-            # before the conv's own backward runs; when that is a BatchNorm backward, it also emits the gradient as
-            # split-bf16 planes (dgrad + wgrad operands) instead of a separate split pass.  If the BN is the only
-            # writer and the conv the only reader, the fp32 copy is dropped and the planes live in its memory.
-            grad_writers = {}
-            for op in self.ops:
-                if op.type == 'Placeholder' or self._passthrough(op) or op in self.fused_into:
-                    continue
-                ins = op.inputs if op.type == 'Add' else op.inputs[:1]
-                for x_t in ins:
-                    if x_t.op.type == 'Placeholder':
-                        continue
-                    k = self.gkey(x_t)
-                    if op.type == 'Add' and k is self.gkey(op.output):
-                        continue
-                    grad_writers.setdefault(k, []).append(op)
-            self.bn_gplanes, self.bn_gplanes_only, self.conv_dy_planes = {}, {}, {}
-            for op in self.ops:
-                if op not in self.tc_wgrad or op in self.fused_act or 'bias' in op.vars or op.output.numel % 8:
-                    if op in self.tc_wgrad:
-                        max_dy = max(max_dy, op.output.numel)
-                    continue
-                k = self.gkey(op.output)
-                later = [w for w in grad_writers.get(k, []) if pos[w] > pos[op]]
-                lw = min(later, key=lambda w: pos[w]) if later else None
-                if lw is None or lw.type != 'FusedBatchNorm' or lw.inputs[0].numel != op.output.numel:
-                    max_dy = max(max_dy, op.output.numel)
-                    continue
-                if lw not in self.bn_gplanes:
-                    readers = [o for o in self.ops if o.type != 'Placeholder' and self.gkey(o.output) is k]
-                    only = len(grad_writers[k]) == 1 and readers == [op]
-                    self.bn_gplanes_only[lw] = only
-                    self.bn_gplanes[lw] = ops.Planes(op.output.numel, dev,
-                                                     self.gbuf[k].view(-1).view(torch.bfloat16) if only else None)
-                self.conv_dy_planes[op] = self.bn_gplanes[lw]
+            self._plan_dy_planes(pos)
             # split-K partials of every tensor-core wgrad get their own buffer; ONE reduction launch at the end of the
             # backward pass sums them into the flat gradient buffer (fixed order: deterministic)
             self.wg_part, red_items = {}, []
@@ -813,8 +773,11 @@ class Executor:
                         red_items.append((self.wg_part[op], gk, splits))
             self._red_items = red_items
             self.wg_reduce = ops.TcWgradReduceBatch(red_items, dev) if red_items else None
-            self.x_scratch = ops.Planes(max_x, dev)
-            self.dy_scratch = ops.Planes(max_dy, dev)
+            # the x / dy operands of the tensor-core convs that no producer writes as planes are split into these
+            self.x_scratch = ops.Planes(max([max_x] + [op.inputs[0].numel for op in self.tc if op not in self.im2col
+                                                       and self.planes_of(op.inputs[0]) is None]), dev)
+            self.dy_scratch = ops.Planes(max([max_dy] + [op.output.numel for op in self.tc_wgrad
+                                                         if op not in self.conv_dy_planes]), dev)
             if self.maskable:
                 self.MASK = torch.ones(st.n_masked, dtype=torch.float32, device=dev)
                 self.BKUP = st.P[:st.n_masked].clone()
@@ -832,10 +795,134 @@ class Executor:
             self.beta1_power = F32(self.optimizer.get('beta1', 0.9))
             self.beta2_power = F32(self.optimizer.get('beta2', 0.999))
         self.bn_fold = self._plan_bn_fold()
-        self._bn_folded = set(self.bn_fold.values())
-        # ---- how each Conv2D / MatMul runs forward, backward and in layer_wgrad
+        # ---- how each FusedBatchNorm and each Conv2D / MatMul runs forward, backward and in layer_wgrad
+        self.batch_norm = {op: (_BnAdd if op in self.bn_add else _BnFolded if op in self.bn_fold.values() else
+                                _BnGather if op in self.bn_gather else _BnLowering)(self, op)
+                           for op in self.ops if op.type == 'FusedBatchNorm'}
         self.conv = {op: (_StemConv if op in self.im2col else _TcConv if op in self.tc else _ConvLowering)(self, op)
                      for op in self.ops if op.type in ('Conv2D', 'MatMul')}
+
+    def _plan_bn_add(self):
+        """Linear bottleneck: a BatchNorm without activation whose only consumer is a residual Add (MobileNet-v2's
+        projection, conv_blocks.py:289-313) writes bn(x) + shortcut straight into the Add's buffer (and / or the Add's
+        operand planes) — one pass instead of BN apply + add + split."""
+        self.bn_add = {}           # BN op -> (add op, other input tensor)
+        fuse_bn_add = os.environ.get('PF_FUSE_BN_ADD', '1') != '0'
+        for op in self.ops:
+            if op.type != 'Add' or op in self.add_fused or not fuse_bn_add:
+                continue
+            for i, x_t in enumerate(op.inputs):
+                src, other = x_t.op, op.inputs[1 - i]
+                if src.type == 'FusedBatchNorm' and src not in self.fused_act and x_t not in self.alias \
+                        and self._consumers(x_t) == [op] and other is not x_t \
+                        and self.g.ops.index(other.op) < self.g.ops.index(src):
+                    self.bn_add[src] = (op, other)
+                    self.add_fused.add(op)
+                    self.buf[x_t] = self.buf[op.output]       # the BN output IS the add output
+                    break
+
+    def _plan_operand_planes(self):
+        """Split-bf16 operand planes (tensor-core path): the BN apply / activation quantizer / gather that produces a
+        conv input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
+        the fp32 copy is only written when some other consumer needs it.  Returns {producer: the convs reading them}."""
+        bn_adds = {a for a, _ in self.bn_add.values()}
+        self.xplanes, self.bn_need_f32, readers = {}, {}, {}
+        for op in self.ops:
+            if op in self.tc and op not in self.im2col:
+                r = self._root(op.inputs[0])
+                if r is not None and (r.op.type in ('FusedBatchNorm', 'GatherChannels') or r.op in bn_adds) \
+                        and r.numel % 8 == 0:
+                    if r.op not in self.xplanes:
+                        self.xplanes[r.op] = ops.Planes(r.numel, self.device)
+                        self.bn_need_f32[r.op] = False
+                    readers.setdefault(r.op, []).append(op)
+        for bn_op in self.xplanes:
+            ts = [bn_op.output] + [c.output for c in self._consumers(bn_op.output) if c in self.fused_into]
+            for t in ts:
+                for c in self._consumers(t):        # a reader that is not the fused activation nor a planes conv
+                    if self.fused_into.get(c) is not bn_op and \
+                            not (c in self.tc and c not in self.im2col and (not self.train or c in self.tc_wgrad)):
+                        self.bn_need_f32[bn_op] = True
+        return readers
+
+    def _plan_bn_gather(self):
+        """Channel gathers of a compact (channel-pruned) graph, compact.py: a GatherChannels op writes its consumer's
+        operand planes; when it is the only reader of an inference-mode BN (+ activation), the BN apply writes the
+        gathered tensor itself and the full-width BN output is never materialised."""
+        self.gather_idx, self.bn_gather = {}, {}
+        for op in self.ops:
+            if op.type != 'GatherChannels':
+                continue
+            self.gather_idx[op] = torch.from_numpy(np.ascontiguousarray(op.attrs['index'], np.int32)).to(self.device)
+            t = op.inputs[0]
+            bn = t.op.inputs[0].op if t.op in self.fused_into else t.op
+            if bn.type == 'FusedBatchNorm' and not bn.attrs['training'] and bn not in self.bn_add \
+                    and bn not in self.xplanes and self._consumers(t) == [op] \
+                    and (t.op is bn or self._consumers(bn.output) == [t.op]) and t.op not in self.aq_index:
+                self.bn_gather[bn] = op
+        self.gather_fused = set(self.bn_gather.values())
+
+    def _plan_levels(self, readers, E):
+        """Integer-level operands (TMA-fed kernels, SURVEY §7 hard part 1b): a <= 8-bit fake-quantized tensor is
+        exactly scale * level, and the levels are exact in bf16 — one operand plane instead of hi + lo, one MMA per
+        k-slice instead of three (two against a split gradient).  Activation side: the fused BN + ReLU + fake-quant pass
+        writes levels + a device header + per-pixel channel sums when EVERY reader of its planes is a TMA-fed kernel.
+        Weight side: the preparation launch derives the levels from the unquantized kernel with the quantizer's own op
+        chain; needs per-layer / per-output-channel buckets and the input's channel sums."""
+        self.act_lv, self.w_lv = {}, {}
+        if os.environ.get('PF_TC_LEVELS', '1') == '0' or not (self.train and self.aq_ops) or self.device.type != 'cuda':
+            return
+        for bn_op, users in readers.items():
+            c = bn_op.output.shape[-1]
+            if self._aq_of_bn(bn_op) is not None and bn_op.attrs['training'] and c >= 16 and not c & (c - 1) \
+                    and all(ops.conv2d_tc_tma_supported(self.desc[u], 0) and u in self.tc_wgrad
+                            and ops.conv2d_tc_tma_supported(self.desc[u], 2) for u in users):
+                m = bn_op.output.numel // c
+                nseg = (c + 127) // 128
+                self.act_lv[bn_op] = dict(hdr=torch.zeros(2, dtype=torch.int32, device=self.device),
+                                          csum=E((m * nseg,)), nseg=nseg)
+        wq = self.weight_quant
+        if self.wq is not None and isinstance(self.wq, ops.UniformWeightQuantizer) and \
+                (not wq.get('use_buckets', False) or wq.get('bucket_type', 'channel') == 'channel'):
+            nbk = self.wq.n_buckets
+            lv_readers = {u for bn_op in self.act_lv for u in readers[bn_op]}
+            for i, op in enumerate(self.wq_ops):
+                if op in lv_readers and op.type == 'Conv2D' and 1 <= self.wq.bits[i] <= 8:
+                    b0, ncols = int(self.wq.segs[i]['bucket0']), int(self.wq.segs[i]['ncols'])
+                    sc = self.wq.scales
+                    self.w_lv[op] = dict(index=i, ncols=ncols, alpha=sc[b0:b0 + ncols], beta=sc[nbk + b0:nbk + b0 + ncols],
+                                         ralpha=sc[2 * nbk + b0:2 * nbk + b0 + ncols])
+
+    def _plan_dy_planes(self, pos):
+        """dy operand planes.  For every tensor-core conv, the LAST op that writes the gradient of its output before
+        the conv's own backward runs; when that is a BatchNorm backward, it also emits the gradient as split-bf16
+        planes (dgrad + wgrad operands) instead of a separate split pass.  If the BN is the only writer and the conv the
+        only reader, the fp32 copy is dropped and the planes live in its memory."""
+        grad_writers = {}
+        for op in self.ops:
+            if op.type == 'Placeholder' or self._passthrough(op) or op in self.fused_into:
+                continue
+            ins = op.inputs if op.type == 'Add' else op.inputs[:1]
+            for x_t in ins:
+                k = self.gkey(x_t)
+                if x_t.op.type != 'Placeholder' and not (op.type == 'Add' and k is self.gkey(op.output)):
+                    grad_writers.setdefault(k, []).append(op)
+        self.bn_gplanes, self.bn_gplanes_only, self.conv_dy_planes = {}, {}, {}
+        for op in self.ops:
+            if op not in self.tc_wgrad or op in self.fused_act or 'bias' in op.vars or op.output.numel % 8:
+                continue
+            k = self.gkey(op.output)
+            later = [w for w in grad_writers.get(k, []) if pos[w] > pos[op]]
+            lw = min(later, key=lambda w: pos[w]) if later else None
+            if lw is None or lw.type != 'FusedBatchNorm' or lw.inputs[0].numel != op.output.numel:
+                continue
+            if lw not in self.bn_gplanes:
+                readers = [o for o in self.ops if o.type != 'Placeholder' and self.gkey(o.output) is k]
+                only = len(grad_writers[k]) == 1 and readers == [op]
+                self.bn_gplanes_only[lw] = only
+                self.bn_gplanes[lw] = ops.Planes(op.output.numel, self.device,
+                                                 self.gbuf[k].view(-1).view(torch.bfloat16) if only else None)
+            self.conv_dy_planes[op] = self.bn_gplanes[lw]
 
     def _plan_bn_fold(self):
         """{tensor-core conv op: inference-mode BatchNorm op} of the BNs applied in the epilogue of the conv that
@@ -855,10 +942,8 @@ class Executor:
             if r is None or r.shape[-1] != x.shape[-1]:
                 continue
             conv = r.op if r.op.type == 'Conv2D' else add_conv.get(r.op)
-            if conv is None or conv not in self.tc or conv in self.im2col or conv in fold:
-                continue
-            act = self.fused_act.get(op, 0)
-            if act and self._consumers(op.output)[0] in self.aq_index:
+            if conv is None or conv not in self.tc or conv in self.im2col or conv in fold \
+                    or self._aq_of_bn(op) is not None:
                 continue
             fold[conv] = op
         return fold
@@ -916,8 +1001,10 @@ class Executor:
         """ops that launch nothing and whose output (and gradient) buffer is their input's"""
         return op.type in ('Reshape', 'Identity') or (op.type == 'Dropout' and op not in self.dropout)
 
-    def _add_of_bn(self):
-        return {a for a, _ in self.bn_add.values()}
+    def _aq_of_bn(self, bn_op):
+        """the activation quantizer (index into aq_ops) that reads the Relu / Relu6 fused into bn_op, else None"""
+        relu_op = self._consumers(bn_op.output)[0] if bn_op in self.fused_act else None
+        return self.aq_index.get(relu_op)
 
     def _root(self, t):
         """The tensor whose buffer holds t (following Reshape / fused-activation aliases); None when t is
@@ -927,6 +1014,11 @@ class Executor:
                 return None
             t = self.alias[t]
         return t
+
+    def outputs_of(self, op):
+        """(fp32 output or None, operand planes or None) of a BN / bn_add Add / gather: fp32 if no planes or a reader"""
+        pl = self.xplanes.get(op)
+        return (self.buf[op.output] if pl is None or self.bn_need_f32[op] else None), pl
 
     def planes_of(self, t):
         r = self._root(t)
@@ -957,7 +1049,6 @@ class Executor:
     # ------------------------------------------------------------------ forward
     def forward(self, training=None, upto=None):
         """upto: stop after this op has run (its output buffer is the result wanted)."""
-        st = self.store
         training = self.train if training is None else training
         if self.aq_ops:
             ops.minmax_reset(self.aq_slots)
@@ -984,97 +1075,19 @@ class Executor:
             elif ty == 'DepthwiseConv2dNative':
                 with self.timed('dwconv'):
                     ops.dwconv_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), self.buf[op.output])
-            elif ty == 'FusedBatchNorm' and op in self.bn_add:
-                x, y = self.T(op.inputs[0]), self.buf[op.output]
-                c = y.shape[-1]
-                m = y.numel() // c
-                b = self.bn[op]
-                gamma, beta = st.view(op.vars['gamma']), st.view(op.vars['beta'])
-                mm, mv = st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance'])
-                add_op, other = self.bn_add[op]
-                pl = self.xplanes.get(add_op)
-                y_out = y if (pl is None or self.bn_need_f32[add_op]) else None
-                if op.attrs['training'] and training:
-                    with self.timed('bn_stats'):
-                        ops.bn_train_stats(x, m, c, op.attrs['epsilon'],
-                                           op.attrs['momentum'] if self.update_moving_stats else 1.0, b['mean'],
-                                           b['var'], b['rstd'], mm, mv, self.bn_ws)
-                    with self.timed('bn_apply'):
-                        ops.bn_apply_add(x, m, c, b['mean'], b['rstd'], gamma, beta, self.T(other), y_out, pl)
-                else:
-                    with self.timed('bn_apply'):
-                        ops.bn_apply_add_eval(x, m, c, mm, mv, op.attrs['epsilon'], gamma, beta, self.T(other), y_out, pl)
-            elif ty == 'FusedBatchNorm' and op in self._bn_folded:
-                continue                                   # applied by the producing conv's epilogue
-            elif ty == 'FusedBatchNorm' and op in self.bn_gather:
-                gop = self.bn_gather[op]
-                x = self.T(op.inputs[0])
-                c = x.shape[-1]
-                pl = self.xplanes.get(gop)
-                with self.timed('bn_apply'):
-                    ops.bn_apply_eval_gather(x, x.numel() // c, c, st.view(op.vars['moving_mean']),
-                                             st.view(op.vars['moving_variance']), op.attrs['epsilon'],
-                                             st.view(op.vars['gamma']), st.view(op.vars['beta']),
-                                             self.fused_act.get(op, 0), self.gather_idx[gop],
-                                             self.buf[gop.output] if pl is None or self.bn_need_f32[gop] else None, pl)
+            elif ty == 'FusedBatchNorm':
+                self.batch_norm[op].forward(training)
             elif ty == 'GatherChannels':
                 if op in self.gather_fused:
                     continue                               # written by the producing BN apply
-                pl = self.xplanes.get(op)
                 with self.timed('gather'):
-                    ops.gather_channels(self.T(op.inputs[0]), self.gather_idx[op],
-                                        self.buf[op.output] if pl is None or self.bn_need_f32[op] else None, pl)
-            elif ty == 'FusedBatchNorm':
-                x, y = self.T(op.inputs[0]), self.buf[op.output]
-                c = y.shape[-1]
-                m = y.numel() // c
-                b = self.bn[op]
-                gamma, beta = st.view(op.vars['gamma']), st.view(op.vars['beta'])
-                mm, mv = st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance'])
-                act = self.fused_act.get(op, 0)
-                relu_op = self._consumers(op.output)[0] if act else None
-                slot = self.aq_slots[self.aq_index[relu_op]] if relu_op in self.aq_index else None
-                pl = self.xplanes.get(op)
-                need_f32 = pl is None or self.bn_need_f32[op]
-                # with an activation quantizer the BN pass writes fp32 (+ range) and the quantizer writes the planes
-                pl_bn = pl if slot is None else None
-                y_bn = y if (need_f32 or slot is not None) else None
-                bn_mom = op.attrs['momentum'] if self.update_moving_stats else 1.0
-                if op.attrs['training'] and training and slot is not None:
-                    # the statistics pass also yields the range of act(bn(x)); one fused BN + fake-quant pass
-                    with self.timed('bn_stats'):
-                        ops.bn_train_stats_range(x, m, c, op.attrs['epsilon'], bn_mom, b['mean'], b['var'],
-                                                 b['rstd'], mm, mv, gamma, beta, act, slot, self.bn_ws)
-                    with self.timed('bn_apply'):
-                        bits = self.act_quant['bits'][self.aq_index[relu_op]]
-                        if self._lv_on and op in self.act_lv:
-                            lv = self.act_lv[op]
-                            ops.bn_apply_quant_levels(x, m, c, b['mean'], b['rstd'], gamma, beta, act, slot, bits,
-                                                      y if need_f32 else None, pl, lv['hdr'], lv['csum'])
-                        else:
-                            ops.bn_apply_quant(x, m, c, b['mean'], b['rstd'], gamma, beta, act, slot, bits,
-                                               y if need_f32 else None, pl)
-                    slot = None                                    # quantized already
-                elif op.attrs['training'] and training:
-                    with self.timed('bn_stats'):
-                        ops.bn_train_stats(x, m, c, op.attrs['epsilon'], bn_mom, b['mean'], b['var'],
-                                           b['rstd'], mm, mv, self.bn_ws)
-                    with self.timed('bn_apply'):
-                        ops.bn_apply(x, m, c, b['mean'], b['rstd'], gamma, beta, act, y_bn, slot, pl_bn)
-                else:
-                    with self.timed('bn_apply'):
-                        ops.bn_apply_eval(x, m, c, mm, mv, op.attrs['epsilon'], gamma, beta, act, y_bn, slot, pl_bn)
-                if slot is not None:
-                    with self.timed('act_quant'):
-                        ops.act_quant(y, y if need_f32 else None, slot, self.act_quant['bits'][self.aq_index[relu_op]], pl)
+                    ops.gather_channels(self.T(op.inputs[0]), self.gather_idx[op], *self.outputs_of(op))
             elif ty in ACT_TYPES:
-                src = self.fused_into[op]
-                if op in self.aq_index and src.type != 'FusedBatchNorm':
-                    y = self.buf[src.output]
-                    slot = self.aq_slots[self.aq_index[op]]
+                if op in self.aq_out:                      # a quantized ReLU whose producer is not a BN
+                    y, i = self.buf[self.fused_into[op].output], self.aq_index[op]
                     with self.timed('act_quant'):
-                        ops.act_minmax(y, slot)
-                        ops.act_quant(y, self.aq_out[op], slot, self.act_quant['bits'][self.aq_index[op]])
+                        ops.act_minmax(y, self.aq_slots[i])
+                        ops.act_quant(y, self.aq_out[op], self.aq_slots[i], self.act_quant['bits'][i])
             elif ty == 'MaxPool':
                 with self.timed('pool'):
                     ops.maxpool_fwd(self.desc[op], self.T(op.inputs[0]), self.buf[op.output], self.pool_argmax.get(op))
@@ -1111,7 +1124,7 @@ class Executor:
             return self._bk
         self._bk = None
         st = self.store
-        if os.environ.get('PF_AR_BUCKETS', '2') == '1' or not self.overlap or getattr(self, 'train_clusters', False) \
+        if os.environ.get('PF_AR_BUCKETS', '2') == '1' or not self.overlap or self.train_clusters \
                 or not st.ranges:
             return None
         s0, e0 = st.ranges[0][0], st.ranges[0][1]
@@ -1219,20 +1232,7 @@ class Executor:
                         gx, acc = self.grad_target(x_t)
                         ops.dwconv_dgrad(d, gy, self.kernel_of(op), acc, gx)
             elif ty == 'FusedBatchNorm':
-                x_t = op.inputs[0]
-                y = self.buf[op.output]
-                c = y.shape[-1]
-                m = y.numel() // c
-                b = self.bn[op]
-                gx, acc = self.grad_target(x_t)
-                gp = self.bn_gplanes.get(op)
-                only = gp is not None and self.bn_gplanes_only[op]
-                assert not (only and acc)
-                with self.timed('bn_bwd'):
-                    ops.bn_bwd(gy, self.T(x_t), m, c, b['mean'], b['rstd'], st.view(op.vars['gamma']),
-                               st.view(op.vars['beta']), self.fused_act.get(op, 0),
-                               st.view(op.vars['gamma'], self.G), st.view(op.vars['beta'], self.G),
-                               None if only else gx, acc, self.bn_ws, gp)
+                self.batch_norm[op].backward(gy)
             elif ty == 'MaxPool':
                 x_t = op.inputs[0]
                 gx, acc = self.grad_target(x_t)
@@ -1280,7 +1280,7 @@ class Executor:
                 self.wg_reduce.reduce()
         if self._ste_grads is not None:
             self.wq.ste_backward_(self._ste_grads)
-        if getattr(self, 'train_clusters', False):
+        if self.train_clusters:
             # codebook gradients from the gradients w.r.t. the quantized kernels (which stay, unchanged, as the kernels'
             # own gradients: the straight-through estimator of utils.py:303-306)
             with self.timed('weight_quant'):

@@ -10,6 +10,7 @@ Arguments are normalised: a pointer becomes the ordinal of its address's first a
 is 0), a ConvDesc / TcAct / TcWt passed by reference becomes its name and fields, numbers stay as they are.
 
     python tests/golden/make_launch_trace.py        # rewrites tests/golden/launches_v1.json
+    python tests/golden/make_launch_trace.py --gpu  # rewrites tests/golden/launches_gpu_v1.json (on an H100)
 """
 import ctypes
 import json
@@ -25,6 +26,7 @@ for p in (ROOT, HERE):
 import make_plan_snapshot as SNAP  # noqa: E402
 
 OUT = os.path.join(HERE, 'launches_v1.json')
+OUT_GPU = os.path.join(HERE, 'launches_gpu_v1.json')
 
 # entry points that launch nothing: answered by the library itself
 QUERIES = {'pf_abi_version', 'pf_last_error', 'pf_conv2d_tc_supported', 'pf_conv2d_tc_weight_elems',
@@ -71,15 +73,21 @@ class Recorder:
         return launch
 
 
-def install(mp):
-    """Route every library call through a Recorder (mp: a pytest MonkeyPatch).  Returns the recorder."""
+def install(mp, streams=False):
+    """Route every library call through a Recorder (mp: a pytest MonkeyPatch).  Returns the recorder.
+    streams: launches keep the current stream's handle (the default stream is NULL, other streams get pointer
+    ordinals), so stream placement is part of the trace."""
     from pocketflow_b200 import lib, ops
     rec = Recorder(lib.load())
     mp.setattr(lib, '_lib', rec)
     mp.setattr(lib, 'load', lambda: rec)
-    mp.setattr(ops, '_stream', lambda: None)
+    if not streams:
+        mp.setattr(ops, '_stream', lambda: None)
     mp.setattr(ops, '_check_f32', lambda *ts: None)
     return rec
+
+
+MOBILENET_V2 = ('mobilenet_at_ilsvrc12', dict(batch_size=64, mobilenet_version=2))
 
 
 def uq8(g):
@@ -91,7 +99,7 @@ def uq8(g):
     return dict(weight_quant=uq.weight_quant_spec(), act_quant=uq.act_quant_spec())
 
 
-def compact_executor(net):
+def compact_executor(net, device='cpu'):
     """the compact inference executor of a fake-pruned network (as tests/test_chn_compact_cpu.py builds it)"""
     import numpy as np
     import torch
@@ -104,7 +112,7 @@ def compact_executor(net):
     st = {v.name: v.initializer(rng, v.shape) for op in C.reachable_ops(g, lg) for v in op.vars.values()}
     st = C.fake_prune(g, lg, st, 0.5, 1)
     cg, ci, cl = C.build_graph(g, im, lg, C.plan(g, lg, st))
-    return Executor(cg, ci, cl, torch.device('cpu'), train=False)
+    return Executor(cg, ci, cl, torch.device(device), train=False)
 
 
 def trace_step(rec, ex):
@@ -115,11 +123,18 @@ def trace_step(rec, ex):
     return rec.launches
 
 
+def trace_eval(rec, ex):
+    """the evaluation pass of a training executor: BN in inference mode, quantizers active"""
+    rec.reset()
+    ex.forward(training=False)
+    return rec.launches
+
+
 def trace_layer_wgrad(rec, ex):
     import torch
     convs = [op for op in ex.ops if op.type in ('Conv2D', 'MatMul')]
-    gys = [torch.empty(op.output.shape) for op in convs]
-    dws = [torch.empty(op.vars['kernel'].shape) for op in convs]
+    gys = [torch.empty(op.output.shape, device=ex.device) for op in convs]
+    dws = [torch.empty(op.vars['kernel'].shape, device=ex.device) for op in convs]
     rec.reset()
     ex.forward()
     for op, gy, dw in zip(convs, gys, dws):
@@ -136,11 +151,16 @@ def snapshot():
             out[key] = trace_step(rec, SNAP.build(net, flags))
             if teacher:
                 out[key + '_teacher'] = trace_step(rec, SNAP.build(net, flags, train=False))
-        out['resnet20_uq8_b256'] = trace_step(rec, SNAP.build(*SNAP.CASES['resnet20_b256'][:2], edit=uq8))
+        ex = SNAP.build(*SNAP.CASES['resnet20_b256'][:2], edit=uq8)
+        out['resnet20_uq8_b256'] = trace_step(rec, ex)
+        out['resnet20_uq8_b256_eval'] = trace_eval(rec, ex)
         out['resnet50_uq8_b128'] = trace_step(rec, SNAP.build(*SNAP.CASES['resnet50_b128'][:2], edit=uq8))
         out['resnet20_b256_unfused_add'] = trace_step(rec, SNAP.build(*SNAP.CASES['resnet20_b256'][:2], fuse_add=False))
-        out['mobilenet_v2_b64'] = trace_step(rec, SNAP.build('mobilenet_at_ilsvrc12',
-                                                             dict(batch_size=64, mobilenet_version=2)))
+        ex = SNAP.build(*MOBILENET_V2)
+        out['mobilenet_v2_b64'] = trace_step(rec, ex)
+        out['mobilenet_v2_b64_eval'] = trace_eval(rec, ex)
+        out['mobilenet_v2_b64_inference'] = trace_step(rec, SNAP.build(*MOBILENET_V2, train=False))
+        out['lenet_uq8_b128'] = trace_step(rec, SNAP.build(*SNAP.CASES['lenet_b128'][:2], edit=uq8))
         with mp.context() as env:
             env.setenv('PF_STEM_S2D', '0')
             out['mobilenet_v1_b256_no_s2d'] = trace_step(rec, SNAP.build(*SNAP.CASES['mobilenet_v1_b256'][:2]))
@@ -151,6 +171,46 @@ def snapshot():
     return out
 
 
+def snapshot_gpu():
+    """The forms only an executor planned on a CUDA device takes (integer-level operands, the side-stream weight
+    gradient, batch norms folded into the conv epilogue), traced on cuda:0 with stream placement.  Nothing is
+    launched; executors are freed one by one to bound device memory.  Returns {'sm_count': .., 'cases': {..}}: the
+    split-K partition of a weight gradient follows the device's SM count."""
+    import gc
+
+    import pytest
+    import torch
+    out = {}
+
+    def done():
+        gc.collect()
+        torch.cuda.empty_cache()
+    with pytest.MonkeyPatch.context() as mp:
+        rec = install(mp, streams=True)
+        for key in ('resnet50_b128', 'resnet20_b256'):
+            net, flags, _ = SNAP.CASES[key]
+            uq = key.replace('_b', '_uq8_b')
+            ex = SNAP.build(net, flags, edit=uq8, device='cuda:0')
+            out[uq] = trace_step(rec, ex)
+            out[uq + '_eval'] = trace_eval(rec, ex)
+            if key == 'resnet20_b256':
+                out[uq + '_layer_wgrad'] = trace_layer_wgrad(rec, ex)
+            del ex
+            done()
+            out[key + '_teacher'] = trace_step(rec, SNAP.build(net, flags, train=False, device='cuda:0'))
+            done()
+        for net in ('resnet50', 'mobilenet_v1'):
+            out[net + '_compact_b2'] = trace_step(rec, compact_executor(net, 'cuda:0'))
+            done()
+        out['mobilenet_v2_b64_inference'] = trace_step(rec, SNAP.build(*MOBILENET_V2, train=False, device='cuda:0'))
+        done()
+    return dict(sm_count=torch.cuda.get_device_properties(0).multi_processor_count, cases=out)
+
+
+def dumps_gpu(snap):
+    return '{"sm_count": %d,\n"cases": %s}\n' % (snap['sm_count'], dumps(snap['cases']).rstrip('\n'))
+
+
 def dumps(trace):
     """one launch per line"""
     cases = ['%s: [\n%s\n]' % (json.dumps(k), ',\n'.join(json.dumps(l, separators=(',', ':')) for l in v))
@@ -159,6 +219,11 @@ def dumps(trace):
 
 
 if __name__ == '__main__':
-    with open(OUT, 'w') as f:
-        f.write(dumps(snapshot()))
-    print('wrote', OUT)
+    if '--gpu' in sys.argv:       # needs cuda:0; the fixture is only valid for devices with its SM count
+        with open(OUT_GPU, 'w') as f:
+            f.write(dumps_gpu(snapshot_gpu()))
+        print('wrote', OUT_GPU)
+    else:
+        with open(OUT, 'w') as f:
+            f.write(dumps(snapshot()))
+        print('wrote', OUT)

@@ -25,7 +25,7 @@ CASES = {
 }
 
 
-def build(net, flags, train=True, edit=None, **kw):
+def build(net, flags, train=True, edit=None, device='cpu', **kw):
     """edit(graph) -> extra Executor arguments (quantization specs); kw: further Executor arguments"""
     import importlib
 
@@ -50,8 +50,8 @@ def build(net, flags, train=True, edit=None, **kw):
     if edit is not None:
         kw.update(edit(g))
     if not train:
-        return Executor(g, im, out, torch.device('cpu'), train=False, **kw)
-    return Executor(g, im, out, torch.device('cpu'), train=True, loss=loss, labels=lab,
+        return Executor(g, im, out, torch.device(device), train=False, **kw)
+    return Executor(g, im, out, torch.device(device), train=True, loss=loss, labels=lab,
                     optimizer=dict(kind='momentum', momentum=0.9), **kw)
 
 

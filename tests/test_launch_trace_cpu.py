@@ -10,11 +10,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 WANT = json.load(open(os.path.join(GOLDEN, 'launches_v1.json')))
 
-# the conv lowerings the trace has to reach (the level operands and the side-stream weight gradient need a CUDA
-# device: the GPU tests cover them)
+# the conv and batch-norm lowerings the trace has to reach (the level operands, the side-stream weight gradient and
+# the folded batch norm need a CUDA device: tests/test_launch_trace_gpu.py covers them)
 COVERED = ('pf_conv2d_tc_fwd', 'pf_conv2d_tc_fwd_planes', 'pf_conv2d_fwd', 'pf_conv2d_tc_dgrad',
            'pf_conv2d_tc_dgrad_planes', 'pf_conv2d_dgrad', 'pf_conv2d_tc_wgrad_planes', 'pf_conv2d_wgrad', 'pf_im2col',
-           'pf_im2col_planes', 'pf_s2d_planes', 'pf_gather_rows', 'pf_fold_diag_blocks', 'pf_split_bf16')
+           'pf_im2col_planes', 'pf_s2d_planes', 'pf_gather_rows', 'pf_fold_diag_blocks', 'pf_split_bf16',
+           'pf_bn_apply_add_eval', 'pf_uq_act_quant_planes', 'pf_uq_act_quant', 'pf_uq_act_minmax')
 
 
 def test_trace_reaches_every_conv_lowering():

@@ -150,8 +150,7 @@ def run_eval(workload, fold, monkeypatch):
     outs = {}
     for op in ex.ops:
         if op.type == 'FusedBatchNorm':
-            pl = ex.xplanes.get(op)
-            f32 = ex.buf[op.output] if pl is None or ex.bn_need_f32[op] else None
+            f32, pl = ex.outputs_of(op)
             outs[op.name] = (f32.clone() if f32 is not None else None,
                              (pl.hi.clone(), pl.lo.clone()) if pl is not None else None)
     nfold = len(ex.bn_fold)

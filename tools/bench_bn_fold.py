@@ -57,17 +57,10 @@ def main():
     torch.cuda.synchronize()
     flush = torch.zeros(64 << 20, device=dev)
     rows, tot_u, tot_f, tot_b = [], 0.0, 0.0, 0
-    st = ex.store
     for conv, bn in ex.bn_fold.items():
-        lo = ex.conv[conv]
+        lo, bl = ex.conv[conv], ex.batch_norm[bn]
         bias, relu, y = lo._epilogue()
         res = ex.T(lo.res) if lo.res is not None else None
-        pl = ex.xplanes.get(bn)
-        y_bn = ex.buf[bn.output] if pl is None or ex.bn_need_f32[bn] else None
-        c = y.shape[-1]
-        m = y.numel() // c
-        bn_args = (st.view(bn.vars['moving_mean']), st.view(bn.vars['moving_variance']), bn.attrs['epsilon'],
-                   st.view(bn.vars['gamma']), st.view(bn.vars['beta']), ex.fused_act.get(bn, 0))
 
         def conv_call(bn_out=None):
             if lo.xp is not None:
@@ -77,18 +70,16 @@ def main():
 
         def unfused():
             conv_call()
-            mu, var, eps, ga, be, act = bn_args
-            ops.bn_apply_eval(y, m, c, mu, var, eps, ga, be, act, y_bn, None, pl)
+            ops.bn_apply_eval(y, *bl.moving, bl.act, bl.y_out, None, bl.pl)
 
-        bn_out = ops.TcBnOut(*bn_args, y_bn, pl)
         t_u = median_ms(unfused, flush, n)
-        t_f = median_ms(lambda: conv_call(bn_out), flush, n)
+        t_f = median_ms(lambda: conv_call(bl.bn_out), flush, n)
         t_c = median_ms(conv_call, flush, n)
         saved = 4 * y.numel()                     # the BN pass's read of the conv output
         d = lo.d
         row = dict(conv=conv.name.split('/')[-2] if '/' in conv.name else conv.name,
                    shape='%dx%dx%d->%d %dx%d/%d' % (d.h, d.w, d.c, d.k, d.r, d.s, d.stride_h),
-                   residual=res is not None, f32_out=y_bn is not None, conv_ms=t_c, conv_bn_ms=t_u, fused_ms=t_f,
+                   residual=res is not None, f32_out=bl.y_out is not None, conv_ms=t_c, conv_bn_ms=t_u, fused_ms=t_f,
                    saved_mb=saved / 1e6)
         rows.append(row)
         tot_u += t_u

@@ -100,8 +100,7 @@ def gather_kernels(cm, n, torch):
         if op.type != 'GatherChannels':
             continue
         idx = ex.gather_idx[op]
-        pl = ex.xplanes.get(op)
-        y = ex.buf[op.output] if pl is None or ex.bn_need_f32[op] else None
+        y, pl = ex.outputs_of(op)
         m = op.output.numel // op.output.shape[-1]
         kept = int((idx >= 0).sum().item())
         nbytes = 4 * m * kept + (4 if y is not None else 0) * op.output.numel + (4 if pl is not None else 0) * op.output.numel
