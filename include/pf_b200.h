@@ -574,6 +574,23 @@ int pf_bn_apply_eval_gather(const float* x_dev, int64_t m, int cin, const float*
                             const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev, int act,
                             int cout, const int32_t* idx_dev, float* y_dev, void* y_hi_dev, void* y_lo_dev,
                             void* stream);
+/* training of the compact graph (fine-tuning a channel-pruned model at its pruned width):
+ *   pf_bn_apply_gather   y = gather(act(bn(x))) with the batch statistics mean / rstd of pf_bn_train_stats (cin entries,
+ *                        taken at the BN's own width), bit-identical to pf_bn_apply at full width followed by
+ *                        pf_gather_channels; reads 4 B per kept element, writes 4 B (fp32) and / or 4 B (planes).
+ *   pf_scatter_channels  the backward of pf_gather_channels: dx[:, idx[j]] (+)= dy[:, j] for idx[j] >= 0.  dy is
+ *                        [m, cout], dx [m, cin] (cin % 4 == 0); inv_dev[cin] is the inverse of the gather's table
+ *                        (inv[c] = j with idx[j] == c, else -1; 16-byte aligned) — positions are unique, so every
+ *                        element of dx has one writer and there are no atomics.  accumulate == 0 writes ALL of dx (zeros
+ *                        where inv < 0); accumulate != 0 adds into the fp32 dx and leaves ungathered channels alone.
+ *                        dx may also (or only, without accumulate) be written as split-bf16 planes of the final value,
+ *                        the convention of pf_bn_bwd_planes.  4 B read per compact element + 4 B written per element
+ *                        of dx (+ 4 B read per touched element when accumulating). */
+int pf_bn_apply_gather(const float* x_dev, int64_t m, int cin, const float* mean_dev, const float* rstd_dev,
+                       const float* gamma_dev, const float* beta_dev, int act, int cout, const int32_t* idx_dev,
+                       float* y_dev, void* y_hi_dev, void* y_lo_dev, void* stream);
+int pf_scatter_channels(const float* dy_dev, int64_t m, int cin, int cout, const int32_t* inv_dev, int accumulate,
+                        float* dx_dev, void* dx_hi_dev, void* dx_lo_dev, void* stream);
 /* dropout (slim.dropout, mobilenet.py:369; TF 1.x nn_ops.dropout): y = (x / keep) * floor(keep + u), u in [0, 1) from
  * Philox4x32-10 keyed by (seed, rank) with counter (element index / 4 [64 bits], step [low 32 bits], stream_id);
  * mask_dev[i] <- floor(keep + u) (0 / 1).  stream_id tells the Dropout ops of one graph apart (each passes its own

@@ -23,9 +23,21 @@ tools/conversion/export_chn_pruned_tflite_model.py (`insert_alt_routines`: `gath
 
 Padding channels carry zero kernel rows and columns, zero bias, and BN gamma = beta = moving mean = 0, moving
 variance = 1, so they stay exactly zero through every op.
+
+The same plan applies to the TRAINING graph of a ModelHelper (forward_train): training-mode BN, Dropout and the
+linear-bottleneck BN + Add are per-channel ops too.  `CompactTrainer` builds the training step of a channel-pruning
+learner at the pruned width from the learner's masked full-width step executor: parameters, optimizer slots and masks
+are sliced into it (`slice_state`) and expanded back (`expand_state`), so the learner keeps writing its masked
+full-width checkpoints.  A padding channel also stays exactly zero through a training step: its activations are 0, so
+its batch mean and variance are 0 and BN gives ((0 - 0) * rstd) * 0 + 0 = 0; the BN backward multiplies dx by gamma = 0
+and forms dgamma from xhat = 0; dbeta and a bias gradient are column sums of a gradient that is 0 because every
+consumer reads the channel through zero kernel rows (dgrad) or never gathers it (scatter); the weight gradient of a
+padding row is a sum of 0 * dy and of a padding column a sum of x * 0; with zero weight, slot and gradient the Momentum
+update acc = m * acc + (g + wd * 0), w -= lr * acc leaves 0, and the sliced mask is 0 there besides.
 """
 import json
 import os
+from collections import OrderedDict
 
 import numpy as np
 
@@ -237,8 +249,9 @@ def _take(a, axis, lay, fill=0.0):
     return np.ascontiguousarray(np.moveaxis(r, 0, axis))
 
 
-def slice_state(graph, logits, rec, state):
-    """Compact state dict (same variable names) of the masked full-width `state`."""
+def slice_state(graph, logits, rec, state, partial=False):
+    """Compact state dict (same variable names) of the masked full-width `state`.  partial: `state` may hold only some
+    of the variables (per-variable views of an optimizer slot, the masks of the maskable kernels)."""
     out = {}
     for op in reachable_ops(graph, logits):
         if not op.vars:
@@ -246,6 +259,8 @@ def slice_state(graph, logits, rec, state):
         lout = rec['tensors'][op.output.name]
         lin = _input_layouts(op, rec)[0] if op.inputs else None
         for role, v in op.vars.items():
+            if partial and v.name not in state:
+                continue
             a = state[v.name]
             if op.type == 'Conv2D' and role == 'kernel':
                 a = _take(_take(a, 2, lin), 3, lout)
@@ -259,6 +274,128 @@ def slice_state(graph, logits, rec, state):
     return out
 
 
+def expand_state(graph, logits, rec, compact_state, full_state):
+    """The inverse of slice_state: a copy of `full_state` whose kept entries (non-negative positions of the layouts)
+    come from `compact_state`; dead producer channels and the zero kernel rows keep what `full_state` holds.  Variables
+    missing from `compact_state` are copied unchanged.  expand_state(slice_state(s), s) == s bit for bit."""
+    out = {k: np.array(v, np.float32, copy=True) for k, v in full_state.items()}
+    for op in reachable_ops(graph, logits):
+        if not op.vars:
+            continue
+        lout = np.asarray(rec['tensors'][op.output.name], np.int64)
+        lin = np.asarray(_input_layouts(op, rec)[0], np.int64) if op.inputs else None
+        jo = np.nonzero(lout >= 0)[0]
+        for role, v in op.vars.items():
+            if v.name not in compact_state:
+                continue
+            a, f = np.asarray(compact_state[v.name], np.float32), out[v.name]
+            if op.type in ('Conv2D', 'MatMul') and role == 'kernel':
+                ji = np.nonzero(lin >= 0)[0]
+                f[..., lin[ji][:, None], lout[jo][None, :]] = a[..., ji[:, None], jo[None, :]]
+            elif op.type == 'DepthwiseConv2dNative':
+                f[:, :, lout[jo], :] = a[:, :, jo, :]
+            else:
+                f[lout[jo]] = a[jo]
+    return out
+
+
+def check_widths(graph, logits):
+    """Every narrowed shape must be one the kernels run: the BN / depthwise / pooling kernels move 4 channels at a time
+    (the executor checks the gathers' own widths when it plans them; a convolution runs at any width, on the CUDA cores
+    where the tensor-core kernels do not take it — CompactTrainer.report names those).  Raises a ValueError naming the
+    first layer that is not."""
+    for op in reachable_ops(graph, logits):
+        if op.type in ('FusedBatchNorm', 'DepthwiseConv2dNative', 'MaxPool', 'Mean', 'Add') \
+                and (op.output.shape[-1] % 4 or op.inputs[0].shape[-1] % 4):
+            raise ValueError('%s: %d -> %d channels at the pruned width; the per-channel kernels need multiples of 4'
+                             % (op.name, op.inputs[0].shape[-1], op.output.shape[-1]))
+
+
+class CompactTrainer:
+    """The fine-tune step of a channel-pruning learner at the pruned width.
+
+        ct = CompactTrainer(ex)      # ex: the learner's masked full-width step Executor, channels already chosen
+        ct.ex.run_step(lr, allreduce)
+        ct.push()                    # parameters, moving statistics and optimizer slots back into `ex`
+    The compact executor shares `ex`'s image and label buffers, its distillation teacher (which stays at full width),
+    optimizer and grad_scale; its flat gradient buffer (what a data-parallel step all-reduces) has the compact size.
+    Deviations from the masked step: a producer channel that no consumer reads is frozen at the value it has when the
+    trainer is built instead of decaying under weight decay, and the reported L2 loss omits it (it cannot reach the
+    logits either way); a narrowed K dimension is summed in another fp32 order, so logits agree to rounding."""
+
+    def __init__(self, ex):
+        from .engine import Executor
+        self.full = ex
+        g, logits = ex.g, ex.logits_t
+        self.rec = plan(g, logits, ex.store.state_dict())
+        self.graph, self.images, self.logits = build_graph(g, ex.images, logits, self.rec)
+        check_widths(self.graph, self.logits)
+        cvar, L = self.graph.variables, ex.loss
+        loss = G.LossSpec()
+        loss.ce = (L.ce[0], self.logits, L.ce[2])
+        loss.l2 = OrderedDict((cvar[v.name], c) for v, c in L.l2.items())
+        if L.dst is not None:
+            loss.dst = (self.logits,) + tuple(L.dst[1:])
+        self.ex = Executor(self.graph, self.images, self.logits, ex.device, train=True, loss=loss, labels=ex.labels_t,
+                           optimizer=ex.optimizer, maskable=[cvar[v.name] for v in ex.maskable], teacher=ex.teacher,
+                           seed=ex.seed, grad_scale=ex.grad_scale, conv_path=ex.conv_path, fuse_add=ex.fuse_add)
+        self.ex.buf[self.images] = ex.buf[ex.images]              # one mini-batch feeds both executors
+        self.ex.buf[ex.labels_t] = ex.buf[ex.labels_t]
+        self.pull()
+
+    def _flat_pairs(self):
+        """(full flat buffer, compact flat buffer, variables of the full executor held in it)"""
+        f, c = self.full, self.ex
+        pairs = [(f.S1, c.S1, f.store.train_vars), (f.MASK, c.MASK, f.maskable)]
+        if f.S2 is not None:
+            pairs.append((f.S2, c.S2, f.store.train_vars))
+        return [p for p in pairs if p[0] is not None]
+
+    def pull(self):
+        """full-width learner state -> compact executor: parameters, moving statistics, slots, masks, step count"""
+        f, c = self.full, self.ex
+        g, lg, cvar = f.g, f.logits_t, self.graph.variables
+        c.store.load_state_dict(slice_state(g, lg, self.rec, f.store.state_dict()), strict=True)
+        for fb, cb, vs in self._flat_pairs():
+            part = slice_state(g, lg, self.rec, {v.name: f.store.view(v, fb).cpu().numpy() for v in vs}, partial=True)
+            for name, a in part.items():
+                c.store.view(cvar[name], cb).copy_(_to_device(a, cb))
+        c.step_count, c.beta1_power, c.beta2_power = f.step_count, f.beta1_power, f.beta2_power
+
+    def push(self):
+        """compact executor -> full-width learner state (the masks do not change while fine-tuning)"""
+        f, c = self.full, self.ex
+        g, lg = f.g, f.logits_t
+        f.store.load_state_dict(expand_state(g, lg, self.rec, c.store.state_dict(), f.store.state_dict()), strict=True)
+        for fb, cb, vs in self._flat_pairs():
+            if fb is f.MASK:
+                continue
+            comp = {v.name: c.store.view(self.graph.variables[v.name], cb).cpu().numpy() for v in vs}
+            full = expand_state(g, lg, self.rec, comp, {v.name: f.store.view(v, fb).cpu().numpy() for v in vs})
+            for v in vs:
+                f.store.view(v, fb).copy_(_to_device(full[v.name], fb))
+        f.step_count, f.beta1_power, f.beta2_power = c.step_count, c.beta1_power, c.beta2_power
+
+    def report(self):
+        """what tools/export_chn_pruned.py prints: every conv's kept input channels, and the parameter counts"""
+        lines = ['%s: reducing %d channels to %d' % (op.name, op.inputs[0].shape[-1], len(self.rec['convs'][op.name]))
+                 for op in reachable_ops(self.full.g, self.full.logits_t) if op.type == 'Conv2D']
+        n_full = sum(v.numel for v in self.full.variables)
+        n_comp = sum(v.numel for v in self.ex.variables)
+        lines.append('parameters: %d -> %d (%.1f %%)' % (n_full, n_comp, 100.0 * n_comp / n_full))
+        cops = {op.name: op for op in self.ex.ops}
+        lost = [op.name for op in self.full.ops if op in self.full.tc_wgrad and cops[op.name] not in self.ex.tc_wgrad]
+        if lost:
+            lines.append('%d convolutions leave the tensor-core weight-gradient kernel at the pruned width: %s'
+                         % (len(lost), ', '.join(lost)))
+        return lines
+
+
+def _to_device(a, like):
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a, np.float32)).to(like.device)
+
+
 def build_eval_graph(model_helper, batch_size, scope='model'):
     """A ModelHelper's inference graph at `batch_size`: (graph, images, logits)."""
     g = G.Graph()
@@ -267,6 +404,17 @@ def build_eval_graph(model_helper, batch_size, scope='model'):
             images = G.placeholder((batch_size,) + tuple(model_helper.dataset_eval.image_shape), 'images')
         with G.variable_scope(scope):
             logits = model_helper.forward_eval(images)
+    return g, images, logits
+
+
+def build_train_graph(model_helper, batch_size, scope='model'):
+    """A ModelHelper's training graph (forward_train) at `batch_size`: (graph, images, logits)."""
+    g = G.Graph()
+    with g.as_default():
+        with G.variable_scope('data'):
+            images = G.placeholder((batch_size,) + tuple(model_helper.dataset_train.image_shape), 'images')
+        with G.variable_scope(scope):
+            logits = model_helper.forward_train(images)
     return g, images, logits
 
 

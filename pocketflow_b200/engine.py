@@ -259,14 +259,18 @@ class _BnAdd(_BnLowering):
 
 
 class _BnGather(_BnLowering):
-    """Inference-mode BN (+ activation) that writes the channel gather reading it (Executor.bn_gather)."""
+    """BN (+ activation) that writes the channel gather reading it (Executor.bn_gather).  Its backward is the base
+    class's: the gather's own backward has scattered dL/dy into this BN's full-width gradient buffer by then."""
 
     def __init__(self, ex, op):
         super().__init__(ex, op, ex.bn_gather[op])
         self.idx = ex.gather_idx[ex.bn_gather[op]]
 
     def _apply(self, x, batch_stats):
-        ops.bn_apply_eval_gather(x, *self.moving, self.act, self.idx, self.y_out, self.pl)
+        if batch_stats:
+            ops.bn_apply_gather(x, *self.batch, self.act, self.idx, self.y_out, self.pl)
+        else:
+            ops.bn_apply_eval_gather(x, *self.moving, self.act, self.idx, self.y_out, self.pl)
 
 
 class _BnFolded(_BnLowering):
@@ -847,16 +851,22 @@ class Executor:
 
     def _plan_bn_gather(self):
         """Channel gathers of a compact (channel-pruned) graph, compact.py: a GatherChannels op writes its consumer's
-        operand planes; when it is the only reader of an inference-mode BN (+ activation), the BN apply writes the
-        gathered tensor itself and the full-width BN output is never materialised."""
-        self.gather_idx, self.bn_gather = {}, {}
+        operand planes; when it is the only reader of a BN (+ activation), the BN apply writes the gathered tensor
+        itself and the full-width BN output is never materialised (a training-mode BN only in a training executor:
+        pf_bn_apply_gather).  A training executor also holds each gather's inverse table, for its backward."""
+        self.gather_idx, self.bn_gather, self.scatter_inv = {}, {}, {}
         for op in self.ops:
             if op.type != 'GatherChannels':
                 continue
-            self.gather_idx[op] = torch.from_numpy(np.ascontiguousarray(op.attrs['index'], np.int32)).to(self.device)
             t = op.inputs[0]
+            if len(op.attrs['index']) % 4 or (self.train and t.shape[-1] % 4):
+                raise ValueError('%s: the channel gather / scatter kernels need widths that are multiples of 4 (%d -> %d)'
+                                 % (op.name, t.shape[-1], len(op.attrs['index'])))
+            self.gather_idx[op] = torch.from_numpy(np.ascontiguousarray(op.attrs['index'], np.int32)).to(self.device)
+            if self.train:
+                self.scatter_inv[op] = torch.from_numpy(ops.scatter_table(op.attrs['index'], t.shape[-1])).to(self.device)
             bn = t.op.inputs[0].op if t.op in self.fused_into else t.op
-            if bn.type == 'FusedBatchNorm' and not bn.attrs['training'] and bn not in self.bn_add \
+            if bn.type == 'FusedBatchNorm' and (self.train or not bn.attrs['training']) and bn not in self.bn_add \
                     and bn not in self.xplanes and self._consumers(t) == [op] \
                     and (t.op is bn or self._consumers(bn.output) == [t.op]) and t.op not in self.aq_index:
                 self.bn_gather[bn] = op
@@ -895,7 +905,8 @@ class Executor:
 
     def _plan_dy_planes(self, pos):
         """dy operand planes.  For every tensor-core conv, the LAST op that writes the gradient of its output before
-        the conv's own backward runs; when that is a BatchNorm backward, it also emits the gradient as split-bf16
+        the conv's own backward runs; when that is a BatchNorm backward or a channel scatter (the backward of a
+        GatherChannels), it also emits the gradient as split-bf16
         planes (dgrad + wgrad operands) instead of a separate split pass.  If the BN is the only writer and the conv the
         only reader, the fp32 copy is dropped and the planes live in its memory."""
         grad_writers = {}
@@ -914,7 +925,7 @@ class Executor:
             k = self.gkey(op.output)
             later = [w for w in grad_writers.get(k, []) if pos[w] > pos[op]]
             lw = min(later, key=lambda w: pos[w]) if later else None
-            if lw is None or lw.type != 'FusedBatchNorm' or lw.inputs[0].numel != op.output.numel:
+            if lw is None or lw.type not in ('FusedBatchNorm', 'GatherChannels') or lw.inputs[0].numel != op.output.numel:
                 continue
             if lw not in self.bn_gplanes:
                 readers = [o for o in self.ops if o.type != 'Placeholder' and self.gkey(o.output) is k]
@@ -1233,6 +1244,14 @@ class Executor:
                         ops.dwconv_dgrad(d, gy, self.kernel_of(op), acc, gx)
             elif ty == 'FusedBatchNorm':
                 self.batch_norm[op].backward(gy)
+            elif ty == 'GatherChannels':
+                # also the backward of a gather fused into its BN: the scatter fills that BN's dy buffer
+                gp = self.bn_gplanes.get(op)
+                only = gp is not None and self.bn_gplanes_only[op]
+                gx, acc = self.grad_target(op.inputs[0])
+                assert not (only and acc)
+                with self.timed('scatter'):
+                    ops.scatter_channels(gy, self.scatter_inv[op], None if only else gx, acc, gp)
             elif ty == 'MaxPool':
                 x_t = op.inputs[0]
                 gx, acc = self.grad_target(x_t)

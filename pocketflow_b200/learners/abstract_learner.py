@@ -25,6 +25,7 @@ DEFINE_string('save_path_eval', './models_eval/model.ckpt', 'model\'s save path 
 DEFINE_string('ckpt_format', 'npz', 'checkpoint format to write: npz | tf (TensorFlow V2 bundle)')
 DEFINE_boolean('enbl_dst', False, 'enable the distillation loss for training')
 DEFINE_boolean('enbl_warm_start', False, 'enable warm start for training')
+DEFINE_boolean('enbl_compact_ft', False, 'fine-tune the channel-pruned model at its pruned width (chn-pruned-gpu / chn-pruned-rmt)')
 
 
 def latest_checkpoint(ckpt_dir):
@@ -99,6 +100,7 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         self.ckpt_file = 'models_%s_at_%s.tar.gz' % (self.model_name, self.dataset_name)
         self.graph_train = None
         self._iterator_eval = None
+        self.compact = None             # compact.CompactTrainer of a channel-pruning learner (--enbl_compact_ft)
 
     @abstractmethod
     def train(self):
@@ -246,6 +248,27 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         iterator.copy_enqueued()
         ops.preprocess_images(dev[0], dev[1], dev_images)
         return nbytes + desc.numel() + labels.numel() * 4
+
+    # ------------------------------------------------------------------ fine-tuning at the pruned width
+    def start_compact_ft(self):
+        """--enbl_compact_ft, once the channels of `sess_train`'s masked model are chosen: the fine-tune steps run on a
+        compact executor planned from that state (compact.CompactTrainer); `sess_train` keeps evaluating and saving."""
+        if not FLAGS.enbl_compact_ft:
+            return
+        from ..compact import CompactTrainer
+        self.compact = CompactTrainer(self.sess_train)
+        if self.is_primary_worker('global'):
+            print('\n'.join(self.compact.report()))
+
+    @property
+    def sess_step(self):
+        """the executor whose run_step is one fine-tune step"""
+        return self.sess_train if self.compact is None else self.compact.ex
+
+    def sync_from_compact(self):
+        """before `sess_train` is saved or evaluated: expand the compact state into it"""
+        if self.compact is not None:
+            self.compact.push()
 
     def grad_allreduce(self):
         """The one collective of the data-parallel step (replaces DistributedOptimizer,

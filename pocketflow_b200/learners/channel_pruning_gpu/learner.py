@@ -15,7 +15,12 @@ fine-tuning with masked gradients (:404-443):
 Flagged deviations: with several workers the reference adapts lr_pgd from each worker's LOCAL loss (the workers'
 python loops can then disagree); here the loss is averaged over the workers first.  A channel whose norm is exactly 0
 while the threshold is 0 gives 0/0 = NaN in the reference's shrink factor; here it stays 0.  Without a pre-trained
-checkpoint (synthetic runs) the full model keeps its seed initialisation."""
+checkpoint (synthetic runs) the full model keeps its seed initialisation.
+--enbl_compact_ft (off by default) runs the fine-tune steps at the pruned width (compact.CompactTrainer) and expands the
+state back before every save, so the masked full-width checkpoint, evaluate() and the export tool are unchanged.  Its
+deviations: (a) producer channels that no consumer reads are frozen at their post-selection values instead of decaying
+under weight decay, and the reported loss omits their L2 term; they cannot influence the logits either way; (b) the
+fp32 accumulation order of a narrowed K dimension differs from the masked one, so logits agree to rounding."""
 from timeit import default_timer as timer
 
 import numpy as np
@@ -68,6 +73,8 @@ class ChannelPrunedGpuLearner(AbstractLearner):  # pylint: disable=too-many-inst
         self.init_from_full()
         # choose channels and evaluate the model before re-training (:152-157)
         self.choose_channels()
+        self.start_compact_ft()
+        ex = self.sess_step
         if self.is_primary_worker('global'):
             self.__save_model()
             self.evaluate()
@@ -116,12 +123,13 @@ class ChannelPrunedGpuLearner(AbstractLearner):  # pylint: disable=too-many-inst
             mgw.broadcast_global_variables([ex.store.P, ex.store.O, self.store_full.P, self.store_full.O])
 
     def __save_model(self):
+        self.sync_from_compact()
         ex = self.sess_train
         print('model saved to ' + save_checkpoint(FLAGS.cpg_save_path, ex.store.state_dict(), ex.step_count))
 
     def train_step(self):
-        ex = self.sess_train
-        self.h2d_bytes = self.feed(ex, self.iterator_train)
+        ex = self.sess_step
+        self.h2d_bytes = self.feed(self.sess_train, self.iterator_train)
         ex.run_step(self.lrn_rate(ex.step_count), self.grad_allreduce())
 
     def evaluate(self, nb_iters=None):

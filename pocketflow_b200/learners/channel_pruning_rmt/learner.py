@@ -36,7 +36,13 @@ reference's beta1 m + (1 - beta1) g (:499-500), and its GEMMs run on the conv ke
 the shape allows) — the refit is held to a tolerance.  A conv whose bias is fused into its epilogue (MobileNet's
 logits) has the bias subtracted from the gathered outputs (fp32 rounding of y - b).  A conv with a fused activation
 (conv -> Relu with nothing between, LeNet) has no materialised pre-activation output and is refused.  Without a
-pre-trained checkpoint (synthetic runs) the full model keeps its seed initialisation."""
+pre-trained checkpoint (synthetic runs) the full model keeps its seed initialisation.
+--enbl_compact_ft (off by default) runs the fine-tune steps at the pruned width (compact.CompactTrainer), after the
+selection or after --cpr_warm_start, and expands the
+state back before every save, so the masked full-width checkpoint, evaluate() and the export tool are unchanged.  Its
+deviations: (a) producer channels that no consumer reads are frozen at their post-selection values instead of decaying
+under weight decay, and the reported loss omits their L2 term; they cannot influence the logits either way; (b) the
+fp32 accumulation order of a narrowed K dimension differs from the masked one, so logits agree to rounding."""
 import math
 import os
 from timeit import default_timer as timer
@@ -179,6 +185,8 @@ class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-inst
         self.init_masks()
         if FLAGS.enbl_multi_gpu:
             mgw.broadcast_global_variables([ex.store.P, ex.store.O])
+        self.start_compact_ft()
+        ex = self.sess_step
         if self.is_primary_worker('global'):
             self.__save_model()
             self.evaluate()
@@ -201,7 +209,7 @@ class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-inst
                 self.auto_barrier()
         if self.is_primary_worker('global'):
             self.__save_model()
-            print('model saved to ' + save_checkpoint(FLAGS.cpr_save_path_eval, ex.store.state_dict()))
+            print('model saved to ' + save_checkpoint(FLAGS.cpr_save_path_eval, self.sess_train.store.state_dict()))
             self.evaluate()
 
     def init_masks(self):
@@ -213,12 +221,13 @@ class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-inst
         ex.step_count = 0
 
     def __save_model(self):
+        self.sync_from_compact()
         ex = self.sess_train
         print('model saved to ' + save_checkpoint(FLAGS.cpr_save_path, ex.store.state_dict(), ex.step_count))
 
     def train_step(self):
-        ex = self.sess_train
-        self.h2d_bytes = self.feed(ex, self.iterator_train)
+        ex = self.sess_step
+        self.h2d_bytes = self.feed(self.sess_train, self.iterator_train)
         ex.run_step(self.lrn_rate(ex.step_count), self.grad_allreduce())
 
     def evaluate(self, nb_iters=None):

@@ -5,6 +5,9 @@ from ..flags import FLAGS
 def create_learner(sm_writer, model_helper):
     """Create the learner as specified by FLAGS.learner."""
     learner = None
+    if FLAGS.enbl_compact_ft and FLAGS.learner not in ('chn-pruned-gpu', 'chn-pruned-rmt'):
+        raise ValueError('--enbl_compact_ft applies to the channel-pruning learners (chn-pruned-gpu, chn-pruned-rmt), '
+                         'not to ' + FLAGS.learner)
     if FLAGS.learner == 'full-prec':
         from .full_precision.learner import FullPrecLearner
         learner = FullPrecLearner(sm_writer, model_helper)

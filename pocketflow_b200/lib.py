@@ -98,6 +98,8 @@ SIGNATURES = {
     'pf_gather_channels': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_apply_eval_gather': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp,
                                         c_vp, c_vp]),
+    'pf_bn_apply_gather': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'pf_scatter_channels': (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_dropout_fwd':(c_i32, [c_vp, c_i64, c_f32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, c_vp, c_vp, c_vp,
                                c_vp]),
     'pf_dropout_bwd': (c_i32, [c_vp, c_vp, c_i64, c_f32, c_i32, c_vp, c_vp]),

@@ -797,6 +797,38 @@ def bn_apply_eval_gather(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, idx,
                'pf_bn_apply_eval_gather')
 
 
+def bn_apply_gather(x, m, c, mean, rstd, gamma, beta, act, idx, y=None, planes=None):
+    """gather(act(bn(x))) with the batch statistics (training mode) in one launch: x is [m, c], the result
+    [m, idx.numel()] goes to fp32 `y` and / or operand `planes`"""
+    _lib.check(_lib.load().pf_bn_apply_gather(_p(x), m, c, _p(mean), _p(rstd), _p(gamma), _p(beta), int(act),
+                                              idx.numel(), _p(idx), _p(y),
+                                              _p(planes.hi if planes is not None else None),
+                                              _p(planes.lo if planes is not None else None), _stream()),
+               'pf_bn_apply_gather')
+
+
+def scatter_table(index, cin):
+    """inverse of a gather's index table (numpy int32 [cin]): the compact position of every full-width channel, -1 for
+    a channel the gather dropped — what scatter_channels takes"""
+    index = np.asarray(index, np.int64)
+    kept = index[index >= 0]
+    if len(np.unique(kept)) != len(kept) or (len(kept) and kept.max() >= cin):
+        raise ValueError('a gather index table holds every channel of its input at most once')
+    inv = np.full(cin, -1, np.int32)
+    inv[kept] = np.nonzero(index >= 0)[0]
+    return inv
+
+
+def scatter_channels(dy, inv, dx=None, accumulate=False, planes=None):
+    """backward of gather_channels: dx[..., c] (+)= dy[..., inv[c]] (0 where inv[c] < 0; with `accumulate` those
+    channels are left as they are), to fp32 `dx` and / or the `planes` of the final value"""
+    cout, cin = dy.shape[-1], inv.numel()
+    _lib.check(_lib.load().pf_scatter_channels(_p(dy), dy.numel() // cout, cin, cout, _p(inv), int(bool(accumulate)),
+                                               _p(dx), _p(planes.hi if planes is not None else None),
+                                               _p(planes.lo if planes is not None else None), _stream()),
+               'pf_scatter_channels')
+
+
 def dropout_fwd(x, keep_prob, seed, rank, state, y, mask, stream_id=0):
     """slim.dropout in a training pass: y = (x / keep) * mask, mask = floor(keep + u) (uint8), u from Philox4x32-10 keyed
     by (seed, rank) at the step held in `state` (int64 [2] on the device, advanced by the launch) of stream `stream_id`
