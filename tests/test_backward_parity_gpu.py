@@ -66,7 +66,7 @@ THROUGH = ('Reshape', 'Identity', 'Dropout', 'Relu', 'Relu6')
 EXEMPT = {
     'clusters': "codebooks in the non-uniform learner's 'weights' mode: frozen, so the step computes no gradient for "
                 "them (cluster_grad runs only when they train); asserted: their gradient stays zero and the optimizer "
-                "leaves them and their slots alone",
+                "leaves them and their slots alone.  Trained codebooks are compared (Parity.codebook_terms)",
 }
 
 
@@ -411,12 +411,43 @@ class Parity:
         self.note('dropout dx', max_rel(c, ref, e), BAR_DX)
 
     # ------------------------------------------------------------------------------------------ after the step
+    def codebook_terms(self):
+        """Trained codebooks ('cluster' / 'both' mode): per quantized op (kernel's float64 gradient g, its sum of |terms|,
+        the device's centroid index of every weight, alpha, codebook size 2^bits).  The quantizer's STE sends the
+        gradient of the quantized kernel unchanged to the gathered centroid (utils.py:303-306), through the inverse
+        scale: dL/dc_j = alpha * sum over {i: idx_i = j} of g_i."""
+        ex, wq = self.ex, self.ex.wq
+        assert not wq.use_buckets, 'bucketed codebook training has no float64 reference here'
+        idx, rng, out = wq.idx.cpu().numpy(), wq.uq.ranges(), {}
+        for i, op in enumerate(ex.wq_ops):
+            kv = op.vars['kernel']
+            g, mag = self.var_ref[kv]
+            a = wq.idx_offsets[i]
+            mn, mx = rng[i]
+            alpha = float(F32(F32(mx[0]) - F32(mn[0])) + F32(1e-10))
+            out[op] = (g, mag, torch.from_numpy(idx[a:a + kv.numel].astype(np.int64)).to(g.device), alpha,
+                       1 << wq.uq.bits[i])
+        return out
+
+    @staticmethod
+    def codebook_ref(shape, g, mag, idx, alpha, k):
+        """(dL/dc, sum of |terms|) of one codebook variable of `shape` (entries >= k get no gradient)"""
+        n = int(np.prod(shape))
+        assert int(idx.max()) < k <= n
+        ref = torch.zeros(n, dtype=torch.float64, device=g.device).index_add_(0, idx, g.reshape(-1)) * alpha
+        m = torch.zeros(n, dtype=torch.float64, device=g.device).index_add_(0, idx, mag.reshape(-1)) * alpha
+        return ref.view(shape), m.view(shape)
+
     def variables(self):
         """every trainable variable's gradient in G against its float64 reference; returns (compared, exempt)"""
         ex, st = self.ex, self.ex.store
         key_of = {v: k for op in ex.ops for k, v in op.vars.items()}
         done, exempt = 0, 0
         self.rec = dict(op=None)
+        if ex.train_clusters:
+            self.codebooks = self.codebook_terms()
+            for op, t in self.codebooks.items():
+                self._wref(op.vars['clusters'], *self.codebook_ref(op.vars['clusters'].shape, *t))
         for v in st.train_vars:
             g = st.view(v, ex.G).double()
             if v not in self.var_ref:

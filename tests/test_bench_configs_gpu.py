@@ -84,9 +84,11 @@ def level_flips(ex, orc, state, img):
     return flips, total
 
 
-def local_parity(ex, orc, state, img):
+def local_parity(ex, orc, state, img, training=True):
     """Teacher-forced comparison: (worst conv error relative to the output scale, # fused BN+act+quant elements on a
-    different level, # such elements, worst non-flip difference in units of one level)."""
+    different level, # such elements, worst non-flip difference in units of one level).  training=False: the device
+    ran an inference-mode pass (moving statistics, no dropout), and so does the oracle.  A non-finite output (a buffer
+    no kernel wrote, under PF_POISON) counts as an infinite error."""
     params = {k: torch.from_numpy(np.array(v, dtype=F32, copy=True)) for k, v in state.items()}
     force = {}
     for op in ex.ops:
@@ -95,10 +97,15 @@ def local_parity(ex, orc, state, img):
         elif op.type in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative') and op not in ex.fused_add and op not in ex.fused_act:
             force[op.output.name] = ex.T(op.output).float().cpu()
         elif op.type in ('MaxPool', 'Add', 'Mean'):
-            force[op.output.name] = ex.T(op.output).float().cpu()
+            pl = ex.xplanes.get(op)                  # a linear bottleneck's Add that only its planes hold
+            if pl is not None and not ex.bn_need_f32[op]:
+                n = op.output.numel
+                force[op.output.name] = (pl.hi[:n].float() + pl.lo[:n].float()).cpu().view(op.output.shape)
+            else:
+                force[op.output.name] = ex.T(op.output).float().cpu()
     local = {}
     with torch.no_grad():
-        orc.forward(params, torch.from_numpy(img), True, force=force, local_out=local)
+        orc.forward(params, torch.from_numpy(img), training, force=force, local_out=local)
     worst_conv, worst_name, flips, total, worst_frac = 0.0, '', 0, 0, 0.0
     bits_of = dict(zip([o.name for o in ex.aq_ops], ex.act_quant['bits'])) if ex.aq_ops else {}
     for op in ex.ops:
@@ -106,6 +113,9 @@ def local_parity(ex, orc, state, img):
         if name not in force or name not in local:
             continue
         got, ref = force[name].numpy(), local[name].numpy()
+        if not np.isfinite(got).all():
+            worst_conv, worst_name = float('inf'), op.name + ' (non-finite)'
+            continue
         if op.type in ('Relu', 'Relu6') and op.name in bits_of and int(bits_of[op.name]) <= 16:
             step = (float(ref.max()) - float(ref.min())) / float(2 ** int(bits_of[op.name]) - 1)
             if step > 0:
