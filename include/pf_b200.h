@@ -598,6 +598,14 @@ int pf_scatter_channels(const float* dy_dev, int64_t m, int cin, int cout, const
  * by one, so a replayed CUDA graph draws a fresh mask each time.  Backward: dx (+)= (dy * mask) / keep. */
 int pf_dropout_fwd(const float* x_dev, int64_t n, float keep_prob, uint32_t seed, uint32_t rank, uint32_t stream_id,
                    uint64_t* state_dev, float* y_dev, uint8_t* mask_dev, void* stream);
+/* the same draw for a channel-pruned tensor [n / c, c] whose channel j is channel layout_dev[j] of the full-width
+ * tensor [n / c, cfull] (layout_dev: c int32 on the device, -1 for a zero padding channel): element (row, j) takes the
+ * uniform full-width element row * cfull + layout_dev[j] takes under pf_dropout_fwd with the same seed, rank, stream_id
+ * and step, so the mask is the full-width one gathered by the layout; a padding channel gets mask 0.  layout_dev NULL:
+ * exactly pf_dropout_fwd. */
+int pf_dropout_fwd_mapped(const float* x_dev, int64_t n, float keep_prob, uint32_t seed, uint32_t rank,
+                          uint32_t stream_id, const int32_t* layout_dev, int c, int cfull, uint64_t* state_dev,
+                          float* y_dev, uint8_t* mask_dev, void* stream);
 int pf_dropout_bwd(const float* dy_dev, const uint8_t* mask_dev, int64_t n, float keep_prob, int accumulate, float* dx_dev,
                    void* stream);
 /* out (+)= a (+ b): residual add (resnet_model.py:199,314) / gradient fan-out; b_dev may be NULL */

@@ -227,7 +227,12 @@ def build_graph(graph, images, logits, rec):
                 else:
                     shape = (wout,)
                 vs[role] = g.get_variable(v.name[:-2], shape, v.initializer, v.trainable)
-            nop = g.add_op(op.type, op.type, ins, vs, dict(op.attrs), op.output.shape[:-1] + (wout,), name=op.name)
+            attrs = dict(op.attrs)
+            if op.type == 'Dropout':
+                # the compact mask is the full-width one gathered by the layout (pf_dropout_fwd_mapped)
+                attrs.update(layout=np.asarray(rec['tensors'][op.output.name], np.int32),
+                             full_width=op.output.shape[-1])
+            nop = g.add_op(op.type, op.type, ins, vs, attrs, op.output.shape[:-1] + (wout,), name=op.name)
             if op.type == 'Placeholder':
                 g.placeholders[nop.name] = nop.output
             tmap[op.output] = nop.output
@@ -319,6 +324,8 @@ class CompactTrainer:
         ct.push()                    # parameters, moving statistics and optimizer slots back into `ex`
     The compact executor shares `ex`'s image and label buffers, its distillation teacher (which stays at full width),
     optimizer and grad_scale; its flat gradient buffer (what a data-parallel step all-reduces) has the compact size.
+    A compact Dropout draws the masked step's mask gathered by its layout (pf_dropout_fwd_mapped; its step counter moves
+    with the state in pull / push), so the two steps drop the same activations.
     Deviations from the masked step: a producer channel that no consumer reads is frozen at the value it has when the
     trainer is built instead of decaying under weight decay, and the reported L2 loss omits it (it cannot reach the
     logits either way); a narrowed K dimension is summed in another fp32 order, so logits agree to rounding."""
@@ -352,7 +359,8 @@ class CompactTrainer:
         return [p for p in pairs if p[0] is not None]
 
     def pull(self):
-        """full-width learner state -> compact executor: parameters, moving statistics, slots, masks, step count"""
+        """full-width learner state -> compact executor: parameters, moving statistics, slots, masks, step count,
+        dropout step counters"""
         f, c = self.full, self.ex
         g, lg, cvar = f.g, f.logits_t, self.graph.variables
         c.store.load_state_dict(slice_state(g, lg, self.rec, f.store.state_dict()), strict=True)
@@ -361,6 +369,16 @@ class CompactTrainer:
             for name, a in part.items():
                 c.store.view(cvar[name], cb).copy_(_to_device(a, cb))
         c.step_count, c.beta1_power, c.beta2_power = f.step_count, f.beta1_power, f.beta2_power
+        self._copy_drop_state(f, c)
+
+    def _copy_drop_state(self, src, dst):
+        """the dropout step counters (a Dropout op keeps its name and its stream index in the compact graph)"""
+        if src.drop_state is None:
+            return
+        for op, i in src.drop_stream.items():
+            j = [k for o, k in dst.drop_stream.items() if o.name == op.name]
+            assert j == [i], (op.name, i, j)
+        dst.drop_state.copy_(src.drop_state)
 
     def push(self):
         """compact executor -> full-width learner state (the masks do not change while fine-tuning)"""
@@ -375,6 +393,7 @@ class CompactTrainer:
             for v in vs:
                 f.store.view(v, fb).copy_(_to_device(full[v.name], fb))
         f.step_count, f.beta1_power, f.beta2_power = c.step_count, c.beta1_power, c.beta2_power
+        self._copy_drop_state(c, f)
 
     def report(self):
         """what tools/export_chn_pruned.py prints: every conv's kept input channels, and the parameter counts"""

@@ -74,6 +74,41 @@ dropout_fwd_kernel(const float* __restrict__ x, int64_t n, float keep, uint2 key
   }
 }
 
+// The channel-mapped draw of a compact tensor [rows, c] whose channel j is channel layout[j] of a full-width tensor
+// [rows, cfull]: element (row, j) takes the uniform of full-width element f = row * cfull + layout[j], i.e. component
+// f & 3 of Philox block f >> 2 at the same step and stream, so the mask is the full-width mask gathered by the layout.
+// A padding channel (layout[j] < 0) gets mask 0.  One Philox block per element: a compact Dropout is a head layer.
+__global__ void __launch_bounds__(NT)
+dropout_fwd_mapped_kernel(const float* __restrict__ x, int64_t n, int c, int cfull, const int32_t* __restrict__ layout,
+                          float keep, uint2 key, uint32_t stream, unsigned long long* state, float* __restrict__ y,
+                          uint8_t* __restrict__ mask) {
+  __shared__ unsigned long long s_step;
+  if (threadIdx.x == 0) s_step = __ldcg(state);
+  __syncthreads();
+  const unsigned long long step = s_step;
+  for (int64_t i = (int64_t)blockIdx.x * NT + threadIdx.x; i < n; i += (int64_t)gridDim.x * NT) {
+    const int64_t row = i / c;
+    const int l = layout[i - row * c];
+    float m = 0.f;
+    if (l >= 0) {
+      const int64_t f = row * cfull + l, g = f >> 2;
+      const uint4 r = philox4x32_10(make_uint4((uint32_t)g, (uint32_t)(g >> 32), (uint32_t)step, stream), key);
+      const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+      m = floorf(__fadd_rn(keep, u01(w[f & 3])));
+    }
+    y[i] = __fmul_rn(__fdiv_rn(x[i], keep), m);
+    mask[i] = (uint8_t)m;
+  }
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(state + 1, 1ull) == gridDim.x - 1) {
+      state[1] = 0ull;
+      state[0] = step + 1ull;
+      __threadfence();
+    }
+  }
+}
+
 __global__ void __launch_bounds__(NT)
 dropout_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ mask, int64_t n, float keep, int accumulate,
                    float* __restrict__ dx) {
@@ -107,6 +142,23 @@ int pf_dropout_fwd(const float* x_dev, int64_t n, float keep_prob, uint32_t seed
                                                                                       make_uint2(seed, rank), stream_id, st,
                                                                                       y_dev, mask_dev);
   PF_CHECK_LAUNCH("pf_dropout_fwd");
+  return PF_OK;
+}
+
+int pf_dropout_fwd_mapped(const float* x_dev, int64_t n, float keep_prob, uint32_t seed, uint32_t rank,
+                          uint32_t stream_id, const int32_t* layout_dev, int c, int cfull, uint64_t* state_dev,
+                          float* y_dev, uint8_t* mask_dev, void* stream) {
+  if (!layout_dev)
+    return pf_dropout_fwd(x_dev, n, keep_prob, seed, rank, stream_id, state_dev, y_dev, mask_dev, stream);
+  PF_REQUIRE(n > 0 && x_dev && y_dev && mask_dev && state_dev, "pf_dropout_fwd_mapped: bad arguments");
+  PF_REQUIRE(keep_prob > 0.f && keep_prob <= 1.f, "pf_dropout_fwd_mapped: keep_prob must be in (0, 1]");
+  PF_REQUIRE(((uintptr_t)state_dev & 7) == 0, "pf_dropout_fwd_mapped: state must be 8-byte aligned");
+  PF_REQUIRE(c > 0 && c <= cfull && n % c == 0, "pf_dropout_fwd_mapped: need 0 < c <= cfull and n % c == 0");
+  dropout_fwd_mapped_kernel<<<grid_of(n), NT, 0, (cudaStream_t)stream>>>(x_dev, n, c, cfull, layout_dev, keep_prob,
+                                                                        make_uint2(seed, rank), stream_id,
+                                                                        reinterpret_cast<unsigned long long*>(state_dev),
+                                                                        y_dev, mask_dev);
+  PF_CHECK_LAUNCH("pf_dropout_fwd_mapped");
   return PF_OK;
 }
 

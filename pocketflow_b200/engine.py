@@ -532,8 +532,10 @@ class Executor:
         self.qvars = {op: op.vars['kernel'] for op in self.wq_ops}
         # ---- dropout (slim.dropout): per training-mode Dropout op a mask, a Philox stream index (its position among the
         # graph's Dropout ops) and a device-side step counter (row of drop_state) that the forward kernel advances, so a
-        # replayed CUDA graph draws a fresh mask each step; an inference-mode Dropout is the identity (an alias)
-        self.dropout, self.drop_stream = {}, {}
+        # replayed CUDA graph draws a fresh mask each step; an inference-mode Dropout is the identity (an alias).  A
+        # Dropout of a compact graph (attrs 'layout', 'full_width': compact.build_graph) draws the masked full-width
+        # model's mask gathered by its layout (drop_layout)
+        self.dropout, self.drop_stream, self.drop_layout = {}, {}, {}
         for op in self.ops:
             if op.type == 'Dropout' and op.attrs['training']:
                 mask = torch.empty(op.output.numel, dtype=torch.uint8, device=dev)
@@ -541,6 +543,8 @@ class Executor:
                     mask.fill_(0xff)
                 self.drop_stream[op] = len(self.dropout)
                 self.dropout[op] = mask
+                if 'layout' in op.attrs:
+                    self.drop_layout[op] = torch.as_tensor(np.asarray(op.attrs['layout'], np.int32), device=dev)
         self.drop_state = torch.zeros(len(self.dropout), 2, dtype=torch.int64, device=dev) if self.dropout else None
         self.drop_key = (self.seed, mgw.rank())
         self._drop_on = False          # set per forward(): masks only in training-mode passes
@@ -1112,7 +1116,8 @@ class Executor:
                     with self.timed('dropout'):
                         i = self.drop_stream[op]
                         ops.dropout_fwd(self.T(op.inputs[0]), op.attrs['keep_prob'], self.drop_key[0], self.drop_key[1],
-                                        self.drop_state[i], self.buf[op.output], self.dropout[op], stream_id=i)
+                                        self.drop_state[i], self.buf[op.output], self.dropout[op], stream_id=i,
+                                        layout=self.drop_layout.get(op), full_width=op.attrs.get('full_width'))
             elif ty == 'Add':
                 if op in self.add_fused:
                     continue                               # computed by the producing conv's / BN's epilogue

@@ -102,6 +102,8 @@ SIGNATURES = {
     'pf_scatter_channels': (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_dropout_fwd':(c_i32, [c_vp, c_i64, c_f32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, c_vp, c_vp, c_vp,
                                c_vp]),
+    'pf_dropout_fwd_mapped': (c_i32, [c_vp, c_i64, c_f32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, c_vp, c_i32,
+                                      c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_dropout_bwd': (c_i32, [c_vp, c_vp, c_i64, c_f32, c_i32, c_vp, c_vp]),
     'pf_add': (c_i32, [c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]),
     'pf_fold_diag_blocks': (c_i32, [c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]),

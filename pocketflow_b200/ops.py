@@ -829,14 +829,21 @@ def scatter_channels(dy, inv, dx=None, accumulate=False, planes=None):
                'pf_scatter_channels')
 
 
-def dropout_fwd(x, keep_prob, seed, rank, state, y, mask, stream_id=0):
+def dropout_fwd(x, keep_prob, seed, rank, state, y, mask, stream_id=0, layout=None, full_width=None):
     """slim.dropout in a training pass: y = (x / keep) * mask, mask = floor(keep + u) (uint8), u from Philox4x32-10 keyed
     by (seed, rank) at the step held in `state` (int64 [2] on the device, advanced by the launch) of stream `stream_id`
-    (one per Dropout op of a graph)"""
+    (one per Dropout op of a graph).  layout (int32 [C] on the device, C = x.shape[-1], -1 for padding) and full_width:
+    x is the channel-pruned view of a [..., full_width] tensor, and draws the full-width mask gathered by the layout
+    (pf_dropout_fwd_mapped)"""
     assert state.dtype == torch.int64 and state.numel() >= 2 and mask.dtype == torch.uint8 and mask.numel() >= x.numel()
-    _lib.check(_lib.load().pf_dropout_fwd(_p(x), x.numel(), float(keep_prob), int(seed) & 0xffffffff,
-                                          int(rank) & 0xffffffff, int(stream_id) & 0xffffffff, _p(state), _p(y), _p(mask),
-                                          _stream()), 'pf_dropout_fwd')
+    args = (_p(x), x.numel(), float(keep_prob), int(seed) & 0xffffffff, int(rank) & 0xffffffff,
+            int(stream_id) & 0xffffffff)
+    if layout is None:
+        _lib.check(_lib.load().pf_dropout_fwd(*args, _p(state), _p(y), _p(mask), _stream()), 'pf_dropout_fwd')
+        return
+    assert layout.dtype == torch.int32 and layout.numel() == x.shape[-1]
+    _lib.check(_lib.load().pf_dropout_fwd_mapped(*args, _p(layout), layout.numel(), int(full_width), _p(state), _p(y),
+                                                 _p(mask), _stream()), 'pf_dropout_fwd_mapped')
 
 
 def dropout_bwd(dy, mask, keep_prob, dx, accumulate=False):

@@ -92,7 +92,19 @@ def local_parity(ex, orc, state, img, training=True):
     params = {k: torch.from_numpy(np.array(v, dtype=F32, copy=True)) for k, v in state.items()}
     force = {}
     for op in ex.ops:
-        if op.type in ('Relu', 'Relu6'):
+        if op.type == 'GatherChannels':
+            # a compact graph's channel gather, as the next conv reads it (fp32 or operand planes)
+            y, pl = ex.outputs_of(op)
+            if y is None:
+                n = op.output.numel
+                force[op.output.name] = (pl.hi[:n].float() + pl.lo[:n].float()).cpu().view(op.output.shape)
+            else:
+                force[op.output.name] = y.float().cpu().view(op.output.shape)
+        elif any(c in ex.gather_fused for c in ex._consumers(op.output)):
+            # a BN (+ activation) whose gather is fused into its apply (pf_bn_apply_gather) never writes its
+            # full-width output: the oracle computes it, and the gather's output is compared instead
+            continue
+        elif op.type in ('Relu', 'Relu6'):
             force[op.output.name] = torch.from_numpy(np.ascontiguousarray(gpu_activation(ex, op)))
         elif op.type in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative') and op not in ex.fused_add and op not in ex.fused_act:
             force[op.output.name] = ex.T(op.output).float().cpu()

@@ -96,7 +96,10 @@ def test_bn_apply_eval_gather_equals_bn_apply_then_gather(c, kept, cout, act):
 def _net(name, batch):
     import importlib
     FLAGS.reset()
-    mod = {'mobilenet_v1': 'mobilenet_at_ilsvrc12', 'resnet50': 'resnet_at_ilsvrc12', 'resnet20': 'resnet_at_cifar10'}
+    mod = {'mobilenet_v1': 'mobilenet_at_ilsvrc12', 'mobilenet_v2': 'mobilenet_at_ilsvrc12', 'resnet50': 'resnet_at_ilsvrc12',
+           'resnet20': 'resnet_at_cifar10', 'lenet': 'lenet_at_cifar10'}
+    if name == 'mobilenet_v2':
+        FLAGS.mobilenet_version = 2
     if name == 'resnet50':
         FLAGS.resnet_size = 50
     if name == 'resnet20':
@@ -131,7 +134,8 @@ def _torch_conv64(x, k, op):
 
 @pytest.mark.parametrize('path', ['tc', 'fp32'])
 @pytest.mark.parametrize('name,res_batch', [('mobilenet_v1', 2), ('mobilenet_v1', 100), ('resnet50', 2),
-                                            ('resnet50', 100)])
+                                            ('resnet50', 100), ('mobilenet_v2', 2), ('mobilenet_v2', 64), ('lenet', 2),
+                                            ('lenet', 100)])
 def test_compact_convs_teacher_forced_against_the_masked_full_width_conv(name, res_batch, path):
     g, im, lg = _net(name, res_batch)
     st = _masked_state(g, lg, 0.5, 3)
@@ -185,7 +189,7 @@ def test_compact_convs_teacher_forced_against_the_masked_full_width_conv(name, r
     assert checked == sum(1 for op in fops.values() if op.type == 'Conv2D')
 
 
-@pytest.mark.parametrize('name', ['mobilenet_v1', 'resnet50'])
+@pytest.mark.parametrize('name', ['mobilenet_v1', 'resnet50', 'mobilenet_v2', 'lenet'])
 def test_compact_logits_match_the_masked_full_width_model_and_round_trip(name, tmp_path):
     g, im, lg = _net(name, 16)
     st = _masked_state(g, lg, 0.5, 5)
