@@ -9,15 +9,15 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'tests'))
-from test_bench_configs_gpu import build, oracles, gpu_activation  # noqa: E402
+import bench  # noqa: E402
+from support import gpu_activation, oracles  # noqa: E402
 
 F32 = np.float32
 
 
 def main():
     workload, batch = sys.argv[1], int(sys.argv[2])
-    lrn = build(workload, batch)
+    lrn = bench.build_learner(workload, 1, batch)
     if len(sys.argv) > 3:
         from pocketflow_b200.flags import FLAGS
         import importlib

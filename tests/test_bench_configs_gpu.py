@@ -16,55 +16,17 @@ sensitivity to a 1e-6 perturbation of ITS OWN input).  The tests therefore check
   * END TO END: 1e-5 on every loss term where no discontinuity is active (A32) or no level differs; otherwise the bar is the
     oracle's own sensitivity (10 x the loss change under a 1e-6 relative perturbation of the input images), floor 2e-4.
 Counts go to parity_flips.json in $PF_PARITY_DIR (default: the system temp directory); DESIGN.md §4 quotes them."""
-import json
-import os
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if ROOT not in sys.path:
-    sys.path.insert(0, ROOT)
-
-from oracle import pf_oracle as O  # noqa: E402
-from oracle.step_oracle import StepOracle  # noqa: E402
-from pocketflow_b200 import ops  # noqa: E402
+from oracle import pf_oracle as O
+from oracle.step_oracle import StepOracle
+from support import gpu_activation, local_parity, make, oracles, record, rel
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-
-
-def rel(a, b):
-    return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
-
-
-def build(workload, batch):
-    import bench
-    return bench.build_learner(workload, 1, batch)
-
-
-def oracles(lrn):
-    ex = lrn.sess_train
-    teacher = StepOracle(ex.teacher.ops, ex.teacher.logits_t, lrn.images) if ex.teacher is not None else None
-    return StepOracle(ex.ops, ex.logits_t, lrn.images, lrn.labels, ex.loss, ex.weight_quant, ex.act_quant, teacher)
-
-
-def gpu_activation(ex, relu_op):
-    """Value of a quantized activation as the consuming convolutions see it (fp32 copy, split planes or levels)."""
-    bn = ex.fused_into.get(relu_op)
-    pl = ex.xplanes.get(bn) if bn is not None else None
-    if pl is None:
-        return ex.T(relu_op.output).float().cpu().numpy()
-    shape = relu_op.output.shape
-    lv = ex.act_lv.get(bn)
-    if lv is not None and ex._lv_on:
-        hdr = lv['hdr'].cpu().numpy().view(ops.ACT_HDR)[0]
-        if int(hdr['nplanes']) == 1:
-            return (pl.hi.float() * float(hdr['scale'])).cpu().numpy().reshape(shape)
-    return (pl.hi.float() + pl.lo.float()).cpu().numpy().reshape(shape)
 
 
 def level_flips(ex, orc, state, img):
@@ -84,66 +46,6 @@ def level_flips(ex, orc, state, img):
     return flips, total
 
 
-def local_parity(ex, orc, state, img, training=True):
-    """Teacher-forced comparison: (worst conv error relative to the output scale, # fused BN+act+quant elements on a
-    different level, # such elements, worst non-flip difference in units of one level).  training=False: the device
-    ran an inference-mode pass (moving statistics, no dropout), and so does the oracle.  A non-finite output (a buffer
-    no kernel wrote, under PF_POISON) counts as an infinite error."""
-    params = {k: torch.from_numpy(np.array(v, dtype=F32, copy=True)) for k, v in state.items()}
-    force = {}
-    for op in ex.ops:
-        if op.type == 'GatherChannels':
-            # a compact graph's channel gather, as the next conv reads it (fp32 or operand planes)
-            y, pl = ex.outputs_of(op)
-            if y is None:
-                n = op.output.numel
-                force[op.output.name] = (pl.hi[:n].float() + pl.lo[:n].float()).cpu().view(op.output.shape)
-            else:
-                force[op.output.name] = y.float().cpu().view(op.output.shape)
-        elif any(c in ex.gather_fused for c in ex._consumers(op.output)):
-            # a BN (+ activation) whose gather is fused into its apply (pf_bn_apply_gather) never writes its
-            # full-width output: the oracle computes it, and the gather's output is compared instead
-            continue
-        elif op.type in ('Relu', 'Relu6'):
-            force[op.output.name] = torch.from_numpy(np.ascontiguousarray(gpu_activation(ex, op)))
-        elif op.type in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative') and op not in ex.fused_add and op not in ex.fused_act:
-            force[op.output.name] = ex.T(op.output).float().cpu()
-        elif op.type in ('MaxPool', 'Add', 'Mean'):
-            pl = ex.xplanes.get(op)                  # a linear bottleneck's Add that only its planes hold
-            if pl is not None and not ex.bn_need_f32[op]:
-                n = op.output.numel
-                force[op.output.name] = (pl.hi[:n].float() + pl.lo[:n].float()).cpu().view(op.output.shape)
-            else:
-                force[op.output.name] = ex.T(op.output).float().cpu()
-    local = {}
-    with torch.no_grad():
-        orc.forward(params, torch.from_numpy(img), training, force=force, local_out=local)
-    worst_conv, worst_name, flips, total, worst_frac = 0.0, '', 0, 0, 0.0
-    bits_of = dict(zip([o.name for o in ex.aq_ops], ex.act_quant['bits'])) if ex.aq_ops else {}
-    for op in ex.ops:
-        name = op.output.name
-        if name not in force or name not in local:
-            continue
-        got, ref = force[name].numpy(), local[name].numpy()
-        if not np.isfinite(got).all():
-            worst_conv, worst_name = float('inf'), op.name + ' (non-finite)'
-            continue
-        if op.type in ('Relu', 'Relu6') and op.name in bits_of and int(bits_of[op.name]) <= 16:
-            step = (float(ref.max()) - float(ref.min())) / float(2 ** int(bits_of[op.name]) - 1)
-            if step > 0:
-                dlev = np.abs(got - ref) / step
-                f = dlev > 0.5
-                flips += int(f.sum())
-                total += ref.size
-                if (~f).any():
-                    worst_frac = max(worst_frac, float(dlev[~f].max()))
-        else:
-            e = float(np.abs(got - ref).max() / (np.abs(ref).max() + 1e-30))
-            if e > worst_conv:
-                worst_conv, worst_name = e, op.name
-    return worst_conv, worst_name, flips, total, worst_frac
-
-
 def relu_flips(ex, orc, state, img):
     params = {k: torch.from_numpy(np.array(v, dtype=F32, copy=True)) for k, v in state.items()}
     with torch.no_grad():
@@ -153,16 +55,6 @@ def relu_flips(ex, orc, state, img):
         if op.type in ('Relu', 'Relu6'):
             bad += int(((gpu_activation(ex, op) > 0) != (val[op.output.name].numpy() > 0)).sum())
     return bad
-
-
-def record(name, **kw):
-    # outside the source tree, which may be read-only: $PF_PARITY_DIR, else the system temp directory
-    out = os.environ.get('PF_PARITY_DIR') or tempfile.gettempdir()
-    os.makedirs(out, exist_ok=True)
-    p = os.path.join(out, 'parity_flips.json')
-    d = json.load(open(p)) if os.path.exists(p) else {}
-    d[name] = kw
-    json.dump(d, open(p, 'w'), indent=1, sort_keys=True)
 
 
 def check_quantized_weights(ex, state, use_buckets=True):
@@ -223,7 +115,8 @@ def test_resnet50_uq_step_matches_oracle(a_bits):
     """BENCH workload resnet50_uq8_dst_b128 at batch 2: W8 per-channel, A8 / A32, distillation, tensor-core path with
     TMA-fed kernels and integer-level operands (the default)."""
     from pocketflow_b200.flags import FLAGS
-    lrn = build('resnet50_uq8_dst_b128', 2)
+    import bench
+    lrn = bench.build_learner('resnet50_uq8_dst_b128', 1, 2)
     if a_bits != 8:
         FLAGS.uql_activation_bits = a_bits
         from pocketflow_b200.learners.learner_utils import create_learner
@@ -251,14 +144,16 @@ def test_resnet50_uq_step_matches_oracle(a_bits):
 
 def test_resnet20_cifar_config2_step_matches_oracle():
     """configs[1]: ResNet-20 / CIFAR-10, W8A8 + distillation at the full batch 256."""
-    lrn = build('resnet20_uq8_dst_b256', 256)
+    import bench
+    lrn = bench.build_learner('resnet20_uq8_dst_b256', 1, 256)
     check_step('resnet20_w8a8_b256', lrn, dict(kind='adam', slots={}), True)
 
 
 def test_resnet50_weight_sparse_step_and_mask_rebuild():
     """configs[2] at batch 2: one masked-momentum step with distillation vs the oracle, then a mask rebuild whose masks /
     thresholds / backups are bit-exact against the oracle's restatement of __build_masks."""
-    lrn = build('resnet50_ws50_dst_b128', 2)
+    import bench
+    lrn = bench.build_learner('resnet50_ws50_dst_b128', 1, 2)
     ex = lrn.sess_train
     orc = oracles(lrn)
     masks = {v.name: ex.store.view(v, ex.MASK).cpu().numpy().copy() for v in lrn.maskable_vars}
@@ -289,8 +184,7 @@ def test_resnet50_weight_sparse_step_and_mask_rebuild():
 
 def test_nonuniform_learner_step_on_tensor_core_path():
     """The codebook learner (config 5's learner) on the default tc path (test_learners_gpu.py runs it on fp32)."""
-    from test_learners_gpu import make
-    lrn = make('non-uniform', nuql_weight_bits=4, enbl_dst=True)
+    lrn = make('resnet_at_cifar10', 'non-uniform', 16, reload=None, resnet_size=8, nuql_weight_bits=4, enbl_dst=True)
     ex = lrn.sess_train
     assert len(ex.tc) >= 8
     state, tstate = ex.store.state_dict(), ex.teacher.store.state_dict()
@@ -317,8 +211,7 @@ def test_nonuniform_learner_step_on_tensor_core_path():
 
 def test_mobilenet_channel_pruned_step_on_tensor_core_path():
     """configs[3] steady state on the default tc path (pointwise convs on the tensor cores, depthwise on CUDA cores)."""
-    from test_learners_gpu import make_mobilenet
-    lrn = make_mobilenet('chn-pruned-gpu', cpg_prune_ratio=0.5)
+    lrn = make('mobilenet_at_ilsvrc12', 'chn-pruned-gpu', 2, nb_classes=1001, cpg_prune_ratio=0.5)
     ex = lrn.sess_train
     assert len(ex.tc) >= 13
     lrn.init_from_full()

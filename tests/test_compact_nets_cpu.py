@@ -14,33 +14,15 @@ import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-for p in (HERE, os.path.join(HERE, 'golden')):
-    if p not in sys.path:
-        sys.path.insert(0, p)
+sys.path.insert(0, os.path.join(HERE, 'golden'))
 
-from test_compact_train_cpu import seed_state, train_graph  # noqa: E402
-from test_mbv2_gpu import MASK32, philox4x32_10, ref_mask  # noqa: E402
 from pocketflow_b200 import compact as C  # noqa: E402
 from pocketflow_b200.engine import Executor  # noqa: E402
 from pocketflow_b200.flags import FLAGS  # noqa: E402
+from support import mapped_mask, ref_mask, seed_state, train_graph  # noqa: E402
 
 V2_MULTS = [0.35, 0.75, 1.0, 1.4]
 RATIOS = [0.3, 0.5, 0.7]
-
-
-def mapped_mask(rows, layout, cfull, keep, seed, rank, step, stream=0):
-    """pf_dropout_fwd_mapped in numpy: element (row, j) of the compact [rows, len(layout)] tensor takes the uniform of
-    full-width element f = row * cfull + layout[j], word f & 3 of Philox block f >> 2; padding (layout[j] < 0) is 0"""
-    lay = np.asarray(layout, np.int64)
-    f = (np.arange(rows, dtype=np.uint64)[:, None] * np.uint64(cfull) + np.maximum(lay, 0).astype(np.uint64)[None, :])
-    g = f >> np.uint64(2)
-    ctr = np.stack([g & np.uint64(MASK32), g >> np.uint64(32), np.full_like(g, step & MASK32),
-                    np.full_like(g, stream)], -1).astype(np.uint32)
-    w = np.take_along_axis(philox4x32_10(ctr, (seed, rank)), (f & np.uint64(3)).astype(np.int64)[..., None], -1)[..., 0]
-    u = ((w & np.uint32(0x7fffff)) | np.uint32(0x3f800000)).view(np.float32) - np.float32(1.0)
-    m = np.floor(np.float32(keep) + u).astype(np.float32)
-    m[:, lay < 0] = 0.0
-    return m
 
 
 def v2_train_graph(mult):

@@ -12,27 +12,16 @@
 * chn-pruned-gpu on MobileNet-v2 and both learners on ResNet-8 with --enbl_dst, with and without the flag.
 * A final test fails if a path the configurations are there for was never taken."""
 import gc
-import os
-import sys
 import types
 
 import numpy as np
 import pytest
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-if HERE not in sys.path:
-    sys.path.insert(0, HERE)
-
-from test_backward_parity_gpu import snapshot  # noqa: E402
-from test_bench_configs_gpu import local_parity  # noqa: E402
-from test_compact_nets_cpu import mapped_mask  # noqa: E402
-from test_compact_train_gpu import tapped_step  # noqa: E402
-from test_config_sweep_gpu import BAR_FWD, make  # noqa: E402
-from test_mbv2_gpu import ref_mask  # noqa: E402
-from oracle.mbv2_oracle import DropoutStepOracle  # noqa: E402
-from pocketflow_b200 import compact as C  # noqa: E402
-from pocketflow_b200 import lib, ops  # noqa: E402
+from oracle.mbv2_oracle import DropoutStepOracle
+from pocketflow_b200 import compact as C
+from pocketflow_b200 import lib, ops
+from support import BAR_FWD, QUIET, free, local_parity, make, mapped_mask, ref_mask, snapshot, tapped_step
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
@@ -47,8 +36,7 @@ def _release():
     yield
     from pocketflow_b200.flags import FLAGS
     FLAGS.reset()
-    gc.collect()
-    torch.cuda.empty_cache()
+    free()
 
 
 def seen(path, where):
@@ -169,6 +157,7 @@ CONFIGS = [
     ('resnet20_dst_fp32', 'resnet_at_cifar10', dict(CIFAR, resnet_size=20), 16, 'fp32', True),
     ('resnet50_dst_b32_tc', 'resnet_at_ilsvrc12', dict(resnet_size=50), 32, 'tc', True),
 ]
+BUILD = dict(QUIET, nb_classes=1001)   # what every learner below is built with besides its own flags
 K_MASKED = 2                  # masked steps before the compact trainer is built
 
 
@@ -257,7 +246,7 @@ def test_compact_step_matches_float64_and_the_masked_step(cfg, monkeypatch):
     name, mod, nflags, batch, path, dst = cfg
     monkeypatch.setenv('PF_CONV_PATH', path)
     torch.cuda.reset_peak_memory_stats()
-    lrn = make(mod, 'chn-pruned-gpu', batch, **dict(nflags, enbl_dst=dst))
+    lrn = make(mod, 'chn-pruned-gpu', batch, **dict(BUILD, **nflags, enbl_dst=dst))
     ex = lrn.sess_train
     assert (ex.teacher is not None) == dst
     prune_all(lrn, 0.5, 3)
@@ -342,7 +331,7 @@ def test_compact_step_matches_float64_and_the_masked_step(cfg, monkeypatch):
 def test_v2_compact_step_under_poison_is_finite_and_replays_bit_identically(monkeypatch):
     """every buffer filled with NaN at allocation (PF_POISON=1): a buffer some kernel forgets to write reaches the loss"""
     monkeypatch.setenv('PF_POISON', '1')
-    lrn = make(V2, 'chn-pruned-gpu', 64, mobilenet_version=2)
+    lrn = make(V2, 'chn-pruned-gpu', 64, **BUILD, mobilenet_version=2)
     ex = lrn.sess_train
     prune_all(lrn, 0.5, 5)
     images, labels = lrn.iterator_train.next_batch()
@@ -372,6 +361,11 @@ def test_v2_compact_step_under_poison_is_finite_and_replays_bit_identically(monk
 
 
 # ------------------------------------------------------------------------------------------ the learners end to end
+def resnet8(learner, **flags):
+    """ResNet-8 on CIFAR-10 at batch 16, as tests/test_compact_train_gpu.py builds it"""
+    return make('resnet_at_cifar10', learner, 16, reload='cifar10_dataset', **dict(QUIET, resnet_size=8, **flags))
+
+
 def _losses(lrn, nb_iters):
     out = []
     step = lrn.train_step
@@ -405,7 +399,7 @@ def test_v2_compact_steps_track_the_masked_steps_as_closely_as_a_rounding_pertur
     runs apart), and the compact steps.  The compact cross-entropy must stay as close to the masked one as the control
     does (within 10x, or 1e-5), and the first step must agree at the one-step bars."""
     monkeypatch.setenv('PF_CONV_PATH', path)
-    lrn = make(V2, 'chn-pruned-gpu', 4, mobilenet_version=2)
+    lrn = make(V2, 'chn-pruned-gpu', 4, **BUILD, mobilenet_version=2)
     ex = lrn.sess_train
     prune_all(lrn, 0.5, 3)
     batches = [tuple(t.clone() if torch.is_tensor(t) else t for t in lrn.iterator_train.next_batch()) for _ in range(5)]
@@ -449,7 +443,7 @@ def test_chn_pruned_gpu_on_v2_tracks_the_masked_losses(tmp_path, monkeypatch, pa
     monkeypatch.setenv('PF_CONV_PATH', path)
     runs = {}
     for ft in (False, True):
-        lrn = make(V2, 'chn-pruned-gpu', 4, mobilenet_version=2, enbl_compact_ft=ft, cpg_nb_iters_layer=2,
+        lrn = make(V2, 'chn-pruned-gpu', 4, **BUILD, mobilenet_version=2, enbl_compact_ft=ft, cpg_nb_iters_layer=2,
                    cpg_save_path=str(tmp_path / ('c' if ft else 'm') / 'model.ckpt'))
         runs[ft] = _losses(lrn, 5)
         if ft:
@@ -470,18 +464,17 @@ def test_learners_fine_tune_resnet8_with_distillation_at_the_pruned_width(tmp_pa
     """ResNet-8 with --enbl_dst, 5 fine-tune steps with and without --enbl_compact_ft from the same selection on the
     same batches: the cross-entropy and the distillation term track per step at the 2e-3 of the ResNet-8 test of
     tests/test_compact_train_gpu.py; the compact executor shares the full-width teacher"""
-    from test_compact_train_gpu import make_learner
     base = dict(enbl_dst=True, cpr_save_path_ws=str(tmp_path / 'ws' / 'model.ckpt'), cpg_nb_iters_layer=2,
                 cpr_nb_smpls=40, cpr_nb_crops_per_smpl=3, cpr_ista_nb_iters=30, cpr_lstsq_nb_iters=10)
     if learner == 'chn-pruned-rmt':
         # one selection leaves the warm-start file both fine-tune runs start from
-        sel = make_learner('resnet8', learner, **base)
+        sel = resnet8(learner, **base)
         sel.choose_channels()
         del sel
     runs = {}
     for ft in (False, True):
         sub = tmp_path / ('c' if ft else 'm')
-        lrn = make_learner('resnet8', learner, **dict(
+        lrn = resnet8(learner, **dict(
             base, enbl_compact_ft=ft, cpr_warm_start=learner == 'chn-pruned-rmt',
             cpg_save_path=str(sub / 'cpg' / 'model.ckpt'), cpr_save_path=str(sub / 'cpr' / 'model.ckpt'),
             cpr_save_path_eval=str(sub / 'eval' / 'model.ckpt')))

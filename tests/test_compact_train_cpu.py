@@ -24,23 +24,9 @@ from pocketflow_b200 import graph as G  # noqa: E402
 from pocketflow_b200 import ops  # noqa: E402
 from pocketflow_b200.engine import Executor  # noqa: E402
 from pocketflow_b200.flags import FLAGS  # noqa: E402
+from support import seed_state, train_graph  # noqa: E402
 
 NETS = ['lenet', 'resnet20', 'resnet50', 'mobilenet_v1', 'mobilenet_v2']
-
-
-def train_graph(net):
-    import make_golden_chn_export as M
-    mod, flags = M.NETS[net]
-    FLAGS.reset()
-    for k, v in flags.items():
-        setattr(FLAGS, k, v)
-    mh = importlib.import_module('pocketflow_b200.nets.' + mod).ModelHelper()
-    return C.build_train_graph(mh, 2)
-
-
-def seed_state(g, lg, rng):
-    return {v.name: np.asarray(v.initializer(rng, v.shape), np.float32) + (0.5 if v.name.endswith('beta:0') else 0.0)
-            for op in C.reachable_ops(g, lg) for v in op.vars.values()}
 
 
 @pytest.mark.parametrize('ratio', [0.3, 0.5])

@@ -2,8 +2,6 @@
 torch / the unfused kernels, one training step of the compact model against the masked full-width step from the same
 state and batch, padding channels through three steps, eager step against CUDA-graph replay, and both channel-pruning
 learners end to end with and without --enbl_compact_ft."""
-import gc
-import importlib
 import os
 import subprocess
 import sys
@@ -12,15 +10,12 @@ import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if os.path.join(ROOT, 'tests') not in sys.path:
-    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+from pocketflow_b200 import compact as C
+from pocketflow_b200 import ops
+from pocketflow_b200.flags import FLAGS
+from support import QUIET, free, make, prune_interior, tapped_step
 
-from test_backward_parity_gpu import (BAR_DX, Parity, backward_ops, check_optimizer, max_rel, planes_value,  # noqa: E402
-                                      snapshot)
-from pocketflow_b200 import compact as C  # noqa: E402
-from pocketflow_b200 import ops  # noqa: E402
-from pocketflow_b200.flags import FLAGS  # noqa: E402
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
@@ -31,8 +26,7 @@ def release_device_memory():
     """the ResNet-50 case holds two benchmarked steps at batch 128: hand the cached blocks back for the tests (and their
     child processes) that follow"""
     yield
-    gc.collect()
-    torch.cuda.empty_cache()
+    free()
 
 
 def _idx(kept, cout):
@@ -121,98 +115,16 @@ def test_bn_apply_gather_equals_bn_apply_then_gather(c, kept, cout, act):
 
 
 # ------------------------------------------------------------------ one training step, compact against masked
+# net -> (net module, dataset module reloaded with it, batch, net flags)
+NETS = {'mobilenet': ('mobilenet_at_ilsvrc12', 'ilsvrc12_dataset', 4, dict(nb_classes=1001)),
+        'resnet50': ('resnet_at_ilsvrc12', 'ilsvrc12_dataset', 128, dict(resnet_size=50, nb_classes=1001)),
+        'resnet20': ('resnet_at_cifar10', 'cifar10_dataset', 16, dict(resnet_size=20)),
+        'resnet8': ('resnet_at_cifar10', 'cifar10_dataset', 16, dict(resnet_size=8))}
+
+
 def make_learner(net, learner, **flags):
-    FLAGS.reset()
-    if net == 'mobilenet':
-        import pocketflow_b200.datasets.ilsvrc12_dataset as D
-        importlib.reload(D)
-        mod = importlib.reload(importlib.import_module('pocketflow_b200.nets.mobilenet_at_ilsvrc12'))
-        FLAGS.batch_size, FLAGS.nb_classes = 4, 1001
-    elif net == 'resnet50':
-        import pocketflow_b200.datasets.ilsvrc12_dataset as D
-        importlib.reload(D)
-        mod = importlib.reload(importlib.import_module('pocketflow_b200.nets.resnet_at_ilsvrc12'))
-        FLAGS.resnet_size, FLAGS.batch_size, FLAGS.nb_classes = 50, 128, 1001
-    else:
-        import pocketflow_b200.datasets.cifar10_dataset as D
-        importlib.reload(D)
-        mod = importlib.reload(importlib.import_module('pocketflow_b200.nets.resnet_at_cifar10'))
-        FLAGS.resnet_size, FLAGS.batch_size = (8 if net == 'resnet8' else 20), 16
-    from pocketflow_b200.learners.learner_utils import create_learner
-    importlib.import_module('pocketflow_b200.learners.channel_pruning_gpu.learner')
-    importlib.import_module('pocketflow_b200.learners.channel_pruning_rmt.learner')
-    FLAGS.learner = learner
-    for k, v in dict(dict(summ_step=10 ** 9, save_step=10 ** 9), **flags).items():
-        setattr(FLAGS, k, v)
-    return create_learner(None, mod.ModelHelper())
-
-
-def prune_interior(lrn, ratio, seed):
-    """zero int(cin * ratio) random input channels of every maskable kernel but the first and the last, and set the
-    learner's masks from them (what the selection leaves behind)"""
-    ex = lrn.sess_train
-    lrn.init_from_full()
-    rng = np.random.RandomState(seed)
-    for v in lrn.maskable_vars[1:-1]:
-        w = ex.store.view(v)
-        cin = w.shape[2]
-        w[:, :, torch.from_numpy(rng.permutation(cin)[:int(cin * ratio)]).to(DEV), :] = 0.0
-    for v in lrn.maskable_vars:
-        ops.cpg_channel_mask(ex.store.view(v), ex.store.view(v, ex.MASK))
-    ex.reset_optimizer_state()
-
-
-class CompactParity(Parity):
-    """tests/test_backward_parity_gpu.py's tap (every op's backward rebuilt alone in float64 from the device's own
-    inputs and upstream gradient, the chain of contributions, coverage) with the backward of a channel gather:
-    dx[..., c] = dy[..., j] where index[j] == c, zero elsewhere.  A scatter that writes a whole buffer must give those
-    bits; one that accumulates, the fp32 sum; one that emits dy planes alone, their bf16 split."""
-
-    def __init__(self, ex):
-        super().__init__(ex)
-        self.scatters = []                                   # (op, accumulate, dy planes, planes only)
-
-    def _contribution(self, t, buf, acc, pre):
-        op = self.rec['op']
-        if op is not None and op.type == 'GatherChannels' and self.ex.bn_gplanes_only.get(op, False):
-            return planes_value(self.ex.bn_gplanes[op], t.shape), True, 0.0
-        return super()._contribution(t, buf, acc, pre)
-
-    def _op_GatherChannels(self, op, rec, writes):
-        idx = torch.from_numpy(np.asarray(op.attrs['index'], np.int64)).to(DEV)
-        gy = rec['read'][0]
-        ref = torch.zeros(op.inputs[0].shape, dtype=torch.float64, device=DEV)
-        ref[..., idx[idx >= 0]] = gy[..., idx >= 0]
-        (t, (c, planes, e)), = writes.items()
-        acc = [a for tt, _, a, _ in rec['writes'] if tt is t][0]
-        self.scatters.append((op, acc, op in self.ex.bn_gplanes, planes))
-        if acc or planes:
-            self.note('scatter dx (accumulate)' if acc else 'scatter dx (dy planes)', max_rel(c, ref, e), BAR_DX)
-        else:
-            self.note('scatter dx', float(not torch.equal(c, ref)), 0.0)
-
-
-def tapped_step(cex, lr):
-    """one eager step of `cex` under the tap: every backward op and the loss against float64, every variable's gradient,
-    the optimizer update bit for bit from the device's gradient, the moving statistics.  Returns the tap."""
-    before = snapshot(cex)
-    par = CompactParity(cex)
-    par.install()
-    cex.run_step(lr)
-    torch.cuda.synchronize()
-    assert all(t.op.type == 'Placeholder' for t in par.pending), [t.name for t in par.pending]
-    missing = [op.name for op in backward_ops(cex) if op not in par.checked_ops]
-    assert not missing and 'loss' in par.checked_ops, missing
-    nvar, nexempt = par.variables()
-    nopt, _ = check_optimizer(cex, before, lr, set())
-    print('compact step: %d backward ops, %d variable gradients, %d updates bit-exact; worst %s'
-          % (len(par.checked_ops) - 1, nvar, nopt, {k: float('%.3g' % v) for k, v in sorted(par.worst.items())}))
-    assert not par.fails, par.fails[:20]
-    assert nexempt == 0 and nvar == nopt == len(cex.store.train_vars)
-    del cex.grad_of, cex.grad_target, cex.loss_and_backward          # the tap lives on the instances: take it off
-    for lo in cex.conv.values():
-        del lo.wgrad, lo.dgrad
-    return par
+    mod, data, batch, nflags = NETS[net]
+    return make(mod, learner, batch, reload=data, **dict(dict(QUIET, **nflags), **flags))
 
 
 @pytest.mark.parametrize('net,learner,conv_path', [

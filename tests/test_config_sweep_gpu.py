@@ -22,25 +22,17 @@ channel counts are not multiples of 16 or 64 reach plan branches the benchmarked
     forward against a reference that uses the batch statistics, each miss their bar by more than 10x.
 Worst errors, runtime and peak device memory go to parity_flips.json in $PF_PARITY_DIR (default: the system temp
 directory); DESIGN.md §4 quotes them."""
-import importlib
-import os
-import sys
 import time
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if ROOT not in sys.path:
-    sys.path.insert(0, ROOT)
-
-from oracle import pf_oracle as O  # noqa: E402
-from oracle.mbv2_oracle import DropoutStepOracle  # noqa: E402
-from oracle.step_oracle import StepOracle  # noqa: E402
-from test_backward_parity_gpu import BAR_W, free, run_parity, snapshot  # noqa: E402
-from test_bench_configs_gpu import local_parity, record  # noqa: E402
-from pocketflow_b200 import engine  # noqa: E402
+from oracle import pf_oracle as O
+from oracle.mbv2_oracle import DropoutStepOracle
+from oracle.step_oracle import StepOracle
+from pocketflow_b200 import engine
+from support import BAR_FWD, BAR_W, QUIET, free, local_parity, make, record, run_parity, snapshot
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -49,13 +41,9 @@ F32 = np.float32
 # ResNet-18 / 34's last stage (3x3x512, a 4608-long reduction) with both operands split — the teacher, inference passes,
 # codebook weights, dgrad — measured up to 3.3e-5 (outputs) and 2.1e-5 (dx) on an H100, so this sweep's bars are 4e-5
 # and 3e-5 (DESIGN.md §4, "Open": the error of a split operand scales with the sum of |terms|, not with max|output|).
-BAR_FWD = 4e-5
 BAR_DX = 3e-5
 BAR_FLIPS = 1e-4        # of the quantized activation elements
 
-LEARNER_MODULE = {'uniform': 'uniform_quantization', 'non-uniform': 'nonuniform_quantization',
-                  'full-prec': 'full_precision', 'weight-sparse': 'weight_sparsification',
-                  'chn-pruned-gpu': 'channel_pruning_gpu'}
 UQ8 = dict(uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel')
 R18 = ('resnet_at_ilsvrc12', dict(resnet_size=18))
 
@@ -116,23 +104,6 @@ def _reset_flags():
     yield
     from pocketflow_b200.flags import FLAGS
     FLAGS.reset()
-
-
-def make(net_module, learner, batch, **flags):
-    """A learner as the command line would build it: FLAGS reset, the dataset and net modules reloaded (each re-declares
-    its defaults), then create_learner."""
-    from pocketflow_b200.flags import FLAGS
-    FLAGS.reset()
-    importlib.import_module('pocketflow_b200.learners.%s.learner' % LEARNER_MODULE[learner])
-    importlib.import_module('pocketflow_b200.learners.distillation_helper')
-    importlib.reload(importlib.import_module('pocketflow_b200.datasets.ilsvrc12_dataset'))
-    mod = importlib.reload(importlib.import_module('pocketflow_b200.nets.' + net_module))
-    from pocketflow_b200.learners.learner_utils import create_learner
-    FLAGS.learner, FLAGS.batch_size, FLAGS.nb_classes = learner, batch, 1001
-    FLAGS.summ_step = FLAGS.save_step = 10 ** 9
-    for k, v in flags.items():
-        setattr(FLAGS, k, v)
-    return create_learner(None, mod.ModelHelper())
 
 
 # ------------------------------------------------------------------------------------------ plan branches
@@ -295,14 +266,14 @@ def mixed_bits(ex):
 
 @pytest.mark.parametrize('cfg', CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_config_matches_float64_layer_by_layer(cfg, monkeypatch):
-    import test_backward_parity_gpu
+    import support
     name, (net, net_flags), learner, batch, flags, extra = cfg
     monkeypatch.setenv('PF_POISON', '1')
-    monkeypatch.setattr(test_backward_parity_gpu, 'BAR_DX', BAR_DX)
+    monkeypatch.setattr(support, 'BAR_DX', BAR_DX)
     free()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.time()
-    lrn = make(net, learner, batch, **dict(net_flags, **flags))
+    lrn = make(net, learner, batch, **dict(dict(QUIET, nb_classes=1001, **net_flags), **flags))
     try:
         ex = lrn.sess_train
         if extra.get('choose_channels'):

@@ -10,6 +10,7 @@ from oracle import cpr_oracle as C
 from pocketflow_b200 import ops
 from pocketflow_b200.flags import FLAGS
 from pocketflow_b200.learners.channel_pruning_rmt import learner as L
+from support import check_selection
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -232,34 +233,6 @@ def make_mobilenet(**flags):
     for k, v in base.items():
         setattr(FLAGS, k, v)
     return create_learner(None, M.ModelHelper())
-
-
-def kept_channels(w):
-    return int((np.square(w).sum(axis=(0, 1, 3)) > 0).sum())
-
-
-def check_selection(lrn, full_state):
-    ex = lrn.sess_train
-    assert len(lrn.selection_log) == lrn.nb_layers
-    for rec, v in zip(lrn.selection_log, lrn.maskable_vars):
-        w = ex.store.view(v).cpu().numpy()
-        cin = w.shape[2]
-        assert rec['nnz_target'] == int(cin * (1.0 - rec['ratio']))
-        assert np.all(rec['err'] < 1e-6)
-        # the search meets its target, or stops only once its bracket is below 1e-8 (:803): from 0.1 that takes more
-        # than 20 halvings.  A ratio-0 layer (target = Cin) always meets it.
-        if rec['ratio'] == 0.0:
-            assert rec['nnz'] == cin, v.name
-        if rec['nnz'] != rec['nnz_target']:
-            assert len(rec['search']) > 20, (v.name, rec['search'])
-        assert kept_channels(w) == rec['nnz'], v.name
-        # the channels the search dropped are zero; the kept ones were refit
-        assert np.all(w[:, :, rec['mask'] == 0, :] == 0)
-    # layer 0: ratio 0, still sampled, searched and refit — every channel kept, the weights changed
-    w0 = ex.store.view(lrn.maskable_vars[0]).cpu().numpy()
-    full0 = full_state[lrn.conv_ops_full[0].vars['kernel'].name]
-    assert lrn.prune_ratios[0] == 0.0 and lrn.selection_log[0]['nnz_target'] == w0.shape[2] == kept_channels(w0)
-    assert not np.array_equal(w0, full0)
 
 
 @pytest.mark.parametrize('poison', [False, True])

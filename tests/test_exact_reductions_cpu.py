@@ -1,25 +1,16 @@
 """The helpers of test_exact_reductions_gpu on the CPU: the per-tap DGEMM references against torch's float64 convolution
 on small integer cases, the weight-plane writers against the readers of test_tc_bench_layers_gpu, and the operand
 generator's bound and every-pixel-contributes construction."""
-import os
-import sys
 import types
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, 'tests')):
-    if p not in sys.path:
-        sys.path.insert(0, p)
-
-from pocketflow_b200 import ops  # noqa: E402
-from test_exact_reductions_gpu import (EXACT_BOUND, conv_dgrad_ref, conv_fwd_ref, conv_wgrad_ref, dw_dgrad_ref,  # noqa: E402
-                                       dw_fwd_ref, dw_wgrad_ref, every_pixel_contributes, int_values,
-                                       reduction_operands, split_terms, wgrad_density, write_dgrad_weight,
-                                       write_fwd_weight)
-from test_tc_bench_layers_gpu import dgrad_weight, fwd_weight  # noqa: E402
+from pocketflow_b200 import ops
+from support import (EXACT_BOUND, conv_dgrad_ref, conv_fwd_ref, conv_wgrad_ref, dgrad_weight, dw_dgrad_ref, dw_fwd_ref,
+                     dw_wgrad_ref, every_pixel_contributes, fwd_weight, int_values, reduction_operands, split_terms,
+                     wgrad_density, write_dgrad_weight, write_fwd_weight)
 
 
 def same_pads(size, r, st):

@@ -28,8 +28,6 @@ What is compared, and why not more:
 Every call of a wrapped entry point must have a replayed key, or one in SKIPPED with its reason; every other public
 entry point the step calls must be checked by test_nn_bench_layers_gpu or be in NOT_REPLAYED with its reason."""
 import gc
-import os
-import sys
 import time
 import types
 import zlib
@@ -38,19 +36,13 @@ import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, 'tests')):
-    if p not in sys.path:
-        sys.path.insert(0, p)
-
-from pocketflow_b200 import ops  # noqa: E402
-from test_nn_bench_layers_gpu import CLASSES, EXEMPT, RUNS, NnRecorder  # noqa: E402
-from test_tc_bench_layers_gpu import after_step, geom, run_workload  # noqa: E402
-from test_tc_variants_gpu import plan_key  # noqa: E402
+from pocketflow_b200 import ops
+from support import (CLASSES, EXACT_BOUND, EXEMPT, QUIET, RUNS, NnRecorder, after_step, conv_dgrad_ref, conv_fwd_ref,
+                     conv_wgrad_ref, dw_dgrad_ref, dw_fwd_ref, dw_wgrad_ref, every_pixel_contributes, geom, int_values,
+                     make, plan_key, prune_interior, reduction_operands, run_workload, split_terms, wgrad_density,
+                     write_dgrad_weight, write_fwd_weight)
 
 DEV = torch.device('cuda:0')
-EXACT_BOUND = 1 << 24          # integers below this add exactly in fp32 in any order (pinned on wgmma below)
-CHUNK_PIXELS = 1 << 20         # rows of one per-tap DGEMM in the references
 
 TC_NAMES = ('conv2d_tc_fwd', 'conv2d_tc_fwd_planes', 'conv2d_tc_fwd_ex', 'conv2d_tc_dgrad', 'conv2d_tc_dgrad_planes',
             'conv2d_tc_dgrad_ex', 'conv2d_tc_wgrad', 'conv2d_tc_wgrad_planes', 'conv2d_tc_wgrad_ex')
@@ -83,198 +75,6 @@ NOT_REPLAYED = {
 # the bar each weight gradient is held to by the bench-layer tests, relative to the largest sum of |terms|
 FLOAT_BAR = {'conv2d_tc_wgrad': 2e-5, 'conv2d_tc_wgrad_planes': 2e-5, 'conv2d_tc_wgrad_ex': 2e-5,
              'conv2d_wgrad': 1e-5, 'dwconv_wgrad': 1e-5}
-
-
-# ------------------------------------------------------------------------------------------------ references
-def dims(d):
-    """(n, h, w, c, k, r, s, p, q, sh, sw, pt, pl) of a descriptor or of such a tuple"""
-    return d if isinstance(d, tuple) else geom(d)
-
-
-def padded_hw(d):
-    n, h, w, c, k, r, s, p, q, sh, sw, pt, pl = dims(d)
-    return max((p - 1) * sh + r, pt + h), max((q - 1) * sw + s, pl + w)
-
-
-def pad_input(x, d):
-    """NHWC x inside a zero frame: top / left padding pt / pl, bottom / right as far as any window reaches"""
-    n, h, w, c, k, r, s, p, q, sh, sw, pt, pl = dims(d)
-    hp, wp = padded_hw(d)
-    xp = torch.zeros(x.shape[0], hp, wp, x.shape[3], dtype=x.dtype, device=x.device)
-    xp[:, pt:pt + h, pl:pl + w] = x
-    return xp
-
-
-def tap(xp, d, i, j):
-    """[n, p, q, c] view of padded input xp that filter tap (i, j) reads at every output pixel"""
-    n, h, w, c, k, r, s, p, q, sh, sw, pt, pl = dims(d)
-    return xp[:, i:i + (p - 1) * sh + 1:sh, j:j + (q - 1) * sw + 1:sw]
-
-
-def batch_chunks(d):
-    n, p, q = dims(d)[0], dims(d)[7], dims(d)[8]
-    step = max(1, CHUNK_PIXELS // max(p * q, 1))
-    return [(n0, min(n, n0 + step)) for n0 in range(0, n, step)]
-
-
-def conv_fwd_ref(x, w, d):
-    """y[n, p, q, k] = sum over taps of x_tap @ w[i, j]  (x NHWC, w HWIO), in x's dtype"""
-    n, h, wd, c, k, r, s, p, q = dims(d)[:9]
-    y = torch.zeros(n, p, q, k, dtype=x.dtype, device=x.device)
-    for n0, n1 in batch_chunks(d):
-        xp = pad_input(x[n0:n1], d)
-        for i in range(r):
-            for j in range(s):
-                y[n0:n1] += (tap(xp, d, i, j).reshape(-1, c) @ w[i, j]).view(n1 - n0, p, q, k)
-    return y
-
-
-def conv_dgrad_ref(dy, w, d):
-    """dx of y = conv(x, w): every tap scatters dy @ w[i, j]^T into its strided slice of the padded input"""
-    n, h, wd, c, k, r, s, p, q, sh, sw, pt, pl = dims(d)
-    dx = torch.zeros(n, h, wd, c, dtype=dy.dtype, device=dy.device)
-    for n0, n1 in batch_chunks(d):
-        hp, wp = padded_hw(d)
-        dxp = torch.zeros(n1 - n0, hp, wp, c, dtype=dy.dtype, device=dy.device)
-        g = dy[n0:n1].reshape(-1, k)
-        for i in range(r):
-            for j in range(s):
-                tap(dxp, d, i, j)[...] += (g @ w[i, j].t()).view(n1 - n0, p, q, c)
-        dx[n0:n1] = dxp[:, pt:pt + h, pl:pl + wd]
-    return dx
-
-
-def conv_wgrad_ref(x, dy, d, bounds=None):
-    """dw[i, j] = x_tap^T @ dy over the pixels (n, p, q) in row-major order; bounds = [0, b1, ..., Npix]: also the sum
-    over each pixel range [b_s, b_s+1), as [ranges, r, s, c, k].  Returns (dw, per-range sums or None)."""
-    n, h, wd, c, k, r, s, p, q = dims(d)[:9]
-    dw = torch.zeros(r, s, c, k, dtype=x.dtype, device=x.device)
-    parts = None if bounds is None else torch.zeros(len(bounds) - 1, r, s, c, k, dtype=x.dtype, device=x.device)
-    for n0, n1 in batch_chunks(d):
-        xp = pad_input(x[n0:n1], d)
-        g = dy[n0:n1].reshape(-1, k)
-        row0, row1 = n0 * p * q, n1 * p * q
-        for i in range(r):
-            for j in range(s):
-                xt = tap(xp, d, i, j).reshape(-1, c)
-                dw[i, j] += xt.t() @ g
-                if bounds is None:
-                    continue
-                for sp in range(len(bounds) - 1):
-                    a, b = max(bounds[sp], row0) - row0, min(bounds[sp + 1], row1) - row0
-                    if a < b:
-                        parts[sp, i, j] += xt[a:b].t() @ g[a:b]
-    return dw, parts
-
-
-def dw_fwd_ref(x, w, d):
-    """depthwise: y[n, p, q, c] = sum over taps of x_tap * w[i, j]  (w [r, s, c])"""
-    n, h, wd, c, k, r, s, p, q = dims(d)[:9]
-    y = torch.zeros(n, p, q, c, dtype=x.dtype, device=x.device)
-    for n0, n1 in batch_chunks(d):
-        xp = pad_input(x[n0:n1], d)
-        for i in range(r):
-            for j in range(s):
-                y[n0:n1] += tap(xp, d, i, j) * w[i, j]
-    return y
-
-
-def dw_dgrad_ref(dy, w, d):
-    n, h, wd, c, k, r, s, p, q, sh, sw, pt, pl = dims(d)
-    dx = torch.zeros(n, h, wd, c, dtype=dy.dtype, device=dy.device)
-    for n0, n1 in batch_chunks(d):
-        hp, wp = padded_hw(d)
-        dxp = torch.zeros(n1 - n0, hp, wp, c, dtype=dy.dtype, device=dy.device)
-        for i in range(r):
-            for j in range(s):
-                tap(dxp, d, i, j)[...] += dy[n0:n1] * w[i, j]
-        dx[n0:n1] = dxp[:, pt:pt + h, pl:pl + wd]
-    return dx
-
-
-def dw_wgrad_ref(x, dy, d):
-    n, h, wd, c, k, r, s, p, q = dims(d)[:9]
-    dw = torch.zeros(r, s, c, dtype=x.dtype, device=x.device)
-    for n0, n1 in batch_chunks(d):
-        xp = pad_input(x[n0:n1], d)
-        g = dy[n0:n1].reshape(-1, c)
-        for i in range(r):
-            for j in range(s):
-                dw[i, j] += (tap(xp, d, i, j).reshape(-1, c) * g).sum(0)
-    return dw
-
-
-def split_terms(f, a, b):
-    """f over operand planes a = [hi(, lo)], b = [hi(, lo)], without the lo.lo term the kernels drop:
-    f(a_hi, b_hi (+ b_lo)) + f(a_lo, b_hi).  With absolute=True-style inputs this is the largest sum of |terms|."""
-    bb = b[0] + b[1] if len(b) > 1 else b[0]
-    out = f(a[0], bb)
-    if len(a) > 1:
-        out = out + f(a[1], b[0])
-    return out
-
-
-# ------------------------------------------------------------------------------------------------ operands
-def int_values(shape, density, g, signed=True):
-    """float32 tensor of 0 and (+-)1, each entry non-zero with probability `density`"""
-    dev = g.device
-    v = (torch.rand(shape, generator=g, device=dev) < density).float()
-    if signed:
-        v = v * torch.where(torch.rand(shape, generator=g, device=dev) < 0.5, -1.0, 1.0)
-    return v
-
-
-def wgrad_density(npix, nterms):
-    """density of x and dy such that the expected sum of |terms| of a weight-gradient entry, npix * nterms * density^2,
-    stays near 2^22 (at most 1/2)"""
-    return min(0.5, (float(1 << 22) / (npix * nterms)) ** 0.5)
-
-
-def reduction_operands(xshape, yshape, x_planes, y_planes, density, g, x_signed=True):
-    """x [n, h, w, c] and dy [n, p, q, k] as lists of planes (one or two), integer valued, built so that every output
-    pixel contributes a non-zero term to the weight gradient: channel 0 of x is +-1 in its hi plane and 0 in its lo
-    plane everywhere, and every pixel of dy has one entry (at channel pixel % k) that is +-1 in hi and 0 in lo; so each
-    pixel with an in-bounds tap puts x_hi * dy_hi != 0 into entry (tap, 0, pixel % k)."""
-    xs = [int_values(xshape, density, g, x_signed) for _ in range(x_planes)]
-    ys = [int_values(yshape, density, g) for _ in range(y_planes)]
-    xs[0][..., 0] = torch.where(torch.rand(xshape[:3], generator=g, device=g.device) < 0.5, -1.0, 1.0) \
-        if x_signed else 1.0
-    for pl in xs[1:]:
-        pl[..., 0] = 0.0
-    n, p, q, k = yshape
-    kf = (torch.arange(n * p * q, device=g.device) % k).view(n, p, q, 1)
-    sign = torch.where(torch.rand(n, p, q, 1, generator=g, device=g.device) < 0.5, -1.0, 1.0)
-    ys[0].scatter_(3, kf, sign)
-    for pl in ys[1:]:
-        pl.scatter_(3, kf, torch.zeros_like(sign))
-    return xs, ys
-
-
-def every_pixel_contributes(xs, ys):
-    """the construction of reduction_operands holds: x channel 0 non-zero in hi and zero in lo at every position, and
-    every pixel of dy has an entry non-zero in hi and zero in lo"""
-    ok = bool((xs[0][..., 0] != 0).all()) and all(bool((pl[..., 0] == 0).all()) for pl in xs[1:])
-    carrier = ys[0] != 0
-    for pl in ys[1:]:
-        carrier &= pl == 0
-    return ok and bool(carrier.any(-1).all())
-
-
-# ------------------------------------------------------------------------------------------------ weight planes
-def write_fwd_weight(f_hi, f_lo, w_hi, w_lo):
-    """inverse of test_tc_bench_layers_gpu.fwd_weight: HWIO planes -> the K-major forward copy [k][Kpad] with columns
-    in (r, s, c) order; the Kpad columns stay as they are (zero in a fresh TcWeights)"""
-    r, s, c, k = w_hi.shape
-    for dst, src in ((f_hi, w_hi), (f_lo, w_lo)):
-        if dst is not None and src is not None:
-            dst.view(k, -1)[:, :r * s * c] = src.permute(3, 0, 1, 2).reshape(k, r * s * c).to(dst.dtype)
-
-
-def write_dgrad_weight(d_hi, d_lo, w_hi, w_lo):
-    """inverse of test_tc_bench_layers_gpu.dgrad_weight: HWIO planes -> the dgrad copy [c][Kpad_d], columns (r, s, k)"""
-    r, s, c, k = w_hi.shape
-    for dst, src in ((d_hi, w_hi), (d_lo, w_lo)):
-        dst.view(c, -1)[:, :r * s * k] = src.permute(2, 0, 1, 3).reshape(c, r * s * k).to(dst.dtype)
 
 
 def dv(t):
@@ -982,10 +782,10 @@ def test_compact_step_reductions_are_exact(net, learner, monkeypatch):
     """the compact fine-tune step as test_compact_train_gpu builds it: half of every interior kernel's input channels
     pruned, at batch 128"""
     from pocketflow_b200 import compact as C
-    from test_compact_train_gpu import make_learner, prune_interior
     t0 = time.time()
     torch.cuda.reset_peak_memory_stats()
-    lrn = make_learner(net, learner, batch_size=128)
+    mod, nflags = {'resnet50': ('resnet_at_ilsvrc12', dict(resnet_size=50)), 'mobilenet': ('mobilenet_at_ilsvrc12', {})}[net]
+    lrn = make(mod, learner, 128, **dict(QUIET, nb_classes=1001, **nflags))
     prune_interior(lrn, 0.5, 3)
     ex = lrn.sess_train
     images, labels = lrn.iterator_train.next_batch()

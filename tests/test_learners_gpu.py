@@ -1,6 +1,7 @@
 """Learner-level GPU tests through the plugin surface (create_learner / train_step / prune / evaluate):
 WeightSparseLearner (masks bit-exact vs the oracle inside a real training loop, pruned weights stay
 zero), NonUniformQuantLearner (codebook init + step loss vs the oracle), FullPrecLearner, checkpoints."""
+import functools
 import os
 
 import numpy as np
@@ -10,27 +11,15 @@ import torch
 from oracle import pf_oracle as O
 from oracle.step_oracle import StepOracle
 from pocketflow_b200.flags import FLAGS
+from support import make, rel
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 
 
-def rel(a, b):
-    return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
-
-
-def make(learner, **flags):
-    FLAGS.reset()
-    from pocketflow_b200.nets import resnet_at_cifar10 as R
-    from pocketflow_b200.learners.learner_utils import create_learner
-    import pocketflow_b200.learners.weight_sparsification.learner  # noqa: F401  (flag definitions)
-    import pocketflow_b200.learners.nonuniform_quantization.learner  # noqa: F401
-    import pocketflow_b200.learners.uniform_quantization.learner  # noqa: F401
-    import pocketflow_b200.learners.channel_pruning_gpu.learner  # noqa: F401
-    FLAGS.resnet_size, FLAGS.batch_size, FLAGS.learner = 8, 16, learner
-    for k, v in flags.items():
-        setattr(FLAGS, k, v)
-    return create_learner(None, R.ModelHelper())
+# ResNet-8 on CIFAR-10 at batch 16, the net module as last imported; MobileNet-v1 at batch 2
+resnet8 = functools.partial(make, 'resnet_at_cifar10', batch=16, reload=None, resnet_size=8)
+mobilenet = functools.partial(make, 'mobilenet_at_ilsvrc12', batch=2, nb_classes=1001)
 
 
 def test_create_learner_names():
@@ -45,7 +34,7 @@ def test_create_learner_names():
 
 
 def test_weight_sparse_learner_masks_bit_exact_in_training_loop():
-    lrn = make('weight-sparse', ws_prune_ratio=0.6, ws_prune_ratio_prtl='uniform', enbl_dst=False)
+    lrn = resnet8('weight-sparse', ws_prune_ratio=0.6, ws_prune_ratio_prtl='uniform', enbl_dst=False)
     ex = lrn.sess_train
     names = [v.name for v in lrn.maskable_vars]
     assert len(names) == 11 and all('kernel' in n for n in names)       # 10 convs + dense of ResNet-8
@@ -77,7 +66,7 @@ def test_weight_sparse_learner_masks_bit_exact_in_training_loop():
 
 
 def test_weight_sparse_heurist_protocol():
-    lrn = make('weight-sparse', ws_prune_ratio=0.5, ws_prune_ratio_prtl='heurist')
+    lrn = resnet8('weight-sparse', ws_prune_ratio=0.5, ws_prune_ratio_prtl='heurist')
     n = np.array([v.numel for v in lrn.maskable_vars], dtype=np.float64)
     r = np.array([x[1] for x in lrn.var_names_n_prune_ratios])
     np.testing.assert_allclose(r, O.ws_heurist_ratios(n, 0.5), rtol=1e-12)
@@ -91,7 +80,7 @@ def test_nonuniform_learner_step_matches_oracle(monkeypatch, mode):
     (gradient = alpha * segment sum of the kernel gradient over each centroid's members), 'both' trains everything.
     Quantile init exact, quantized kernels bit-exact, losses 1e-5, codebook / kernel updates vs the oracle step."""
     monkeypatch.setenv('PF_CONV_PATH', 'fp32')
-    lrn = make('non-uniform', nuql_weight_bits=4, enbl_dst=True, nuql_opt_mode=mode)
+    lrn = resnet8('non-uniform', nuql_weight_bits=4, enbl_dst=True, nuql_opt_mode=mode)
     ex = lrn.sess_train
     assert isinstance(ex.wq, __import__('pocketflow_b200.ops', fromlist=['x']).CodebookWeightQuantizer)
     state, tstate = ex.store.state_dict(), ex.teacher.store.state_dict()
@@ -138,7 +127,7 @@ def test_nonuniform_learner_step_matches_oracle(monkeypatch, mode):
 
 
 def test_full_prec_learner_and_checkpoint_roundtrip(tmp_path):
-    lrn = make('full-prec', save_path=str(tmp_path / 'models' / 'model.ckpt'))
+    lrn = resnet8('full-prec', save_path=str(tmp_path / 'models' / 'model.ckpt'))
     ex = lrn.sess_train
     losses = []
     for _ in range(8):
@@ -157,26 +146,11 @@ def test_full_prec_learner_and_checkpoint_roundtrip(tmp_path):
 
 
 def test_uniform_learner_trains_and_evaluates():
-    lrn = make('uniform', uql_weight_bits=8, uql_use_buckets=True, enbl_dst=True, summ_step=5, save_step=10 ** 9,
+    lrn = resnet8('uniform', uql_weight_bits=8, uql_use_buckets=True, enbl_dst=True, summ_step=5, save_step=10 ** 9,
                uql_save_quant_model_path='/tmp/pf_uql_test/model.ckpt')
     lrn.train(nb_iters=6)            # includes the CUDA-graph-free eager loop, logging, final save + evaluate
     r = lrn.sess_train.fetch_losses()
     assert np.isfinite(r['loss']) and lrn.sess_train.step_count == 6
-
-
-def make_mobilenet(learner, **flags):
-    FLAGS.reset()
-    import importlib
-    import pocketflow_b200.datasets.ilsvrc12_dataset as D
-    importlib.reload(D)
-    from pocketflow_b200.nets import mobilenet_at_ilsvrc12 as M
-    importlib.reload(M)
-    from pocketflow_b200.learners.learner_utils import create_learner
-    import pocketflow_b200.learners.channel_pruning_gpu.learner  # noqa: F401
-    FLAGS.batch_size, FLAGS.learner, FLAGS.nb_classes = 2, learner, 1001
-    for k, v in flags.items():
-        setattr(FLAGS, k, v)
-    return create_learner(None, M.ModelHelper())
 
 
 @pytest.mark.parametrize('conv_path', ['fp32', 'tc'])
@@ -185,7 +159,7 @@ def test_mobilenet_channel_pruned_gpu_learner_step(monkeypatch, conv_path):
     run of the selection phase), masked Momentum step; loss vs the oracle step with the same masks; pruned channels
     stay zero.  Both the exact-fp32 and the (default) tensor-core conv path."""
     monkeypatch.setenv('PF_CONV_PATH', conv_path)
-    lrn = make_mobilenet('chn-pruned-gpu', cpg_prune_ratio=0.5)
+    lrn = mobilenet('chn-pruned-gpu', cpg_prune_ratio=0.5)
     ex = lrn.sess_train
     assert len(lrn.maskable_vars) == 15 and sum(v.numel for v in lrn.maskable_vars) == 4165472
     assert all(v.name.startswith('pruned_model/') for v in lrn.maskable_vars)
@@ -239,7 +213,7 @@ def test_channel_selection_phase_matches_the_oracle(monkeypatch, tmp_path, conv_
     for idx in layers:
         ratios[idx] = '0.5'
     (tmp_path / 'ratios.txt').write_text(','.join(ratios) + '\n')
-    lrn = make_mobilenet('chn-pruned-gpu', cpg_prune_ratio_type='list', cpg_prune_ratio_file=str(tmp_path / 'ratios.txt'),
+    lrn = mobilenet('chn-pruned-gpu', cpg_prune_ratio_type='list', cpg_prune_ratio_file=str(tmp_path / 'ratios.txt'),
                          cpg_lrn_rate_pgd_init=1e-7)
     ex = lrn.sess_train
     lrn.init_from_full()
@@ -321,14 +295,14 @@ def test_exec_mode_eval_restores_the_saved_model(tmp_path, learner, path_flag, e
     from pocketflow_b200.datasets.abstract_dataset import POOL_SIZE
     flags = dict(extra, summ_step=10 ** 9, save_step=10 ** 9)
     flags[path_flag] = str(tmp_path / 'ckpt' / 'model.ckpt')
-    lrn = make(learner, **flags)
+    lrn = resnet8(learner, **flags)
     lrn.nb_iters_train = 6
     lrn.train(nb_iters=6)                                               # ends with save + evaluate
     first = lambda r: float(r[0] if isinstance(r, tuple) else r)
     trained = first(lrn.evaluate(nb_iters=POOL_SIZE))
     del lrn
     flags['exec_mode'] = 'eval'
-    fresh = make(learner, **flags)
+    fresh = resnet8(learner, **flags)
     restored = first(fresh.evaluate(nb_iters=POOL_SIZE))
     assert rel(restored, trained) <= 1e-6, (restored, trained)
     # and the default iteration count is the reference's ceil(nb_smpls_eval / batch_size_eval)
@@ -337,14 +311,14 @@ def test_exec_mode_eval_restores_the_saved_model(tmp_path, learner, path_flag, e
 
 def test_exec_mode_eval_without_a_checkpoint_raises(tmp_path):
     flags = dict(exec_mode='eval', save_path=str(tmp_path / 'none' / 'model.ckpt'))
-    lrn = make('full-prec', **flags)
+    lrn = resnet8('full-prec', **flags)
     with pytest.raises(ValueError):
         lrn.evaluate()
 
 
 def test_restore_refuses_a_checkpoint_of_another_scope(tmp_path):
     from pocketflow_b200.learners.abstract_learner import save_checkpoint
-    lrn = make('full-prec', save_path=str(tmp_path / 'm' / 'model.ckpt'))
+    lrn = resnet8('full-prec', save_path=str(tmp_path / 'm' / 'model.ckpt'))
     state = {('other/' + k): v for k, v in lrn.sess_train.store.state_dict().items()}
     save_checkpoint(FLAGS.save_path, state, 1)
     with pytest.raises(ValueError):
@@ -359,7 +333,7 @@ def test_weight_sparse_layerwise_regression_matches_the_oracle(monkeypatch, conv
     against the oracle driven on the same mini-batches."""
     from oracle.step_oracle import cpg_layer_regression
     monkeypatch.setenv('PF_CONV_PATH', conv_path)
-    lrn = make('weight-sparse', ws_prune_ratio=0.5, ws_prune_ratio_prtl='uniform', enbl_dst=True, ws_lrn_rate_rg=3e-3)
+    lrn = resnet8('weight-sparse', ws_prune_ratio=0.5, ws_prune_ratio_prtl='uniform', enbl_dst=True, ws_lrn_rate_rg=3e-3)
     ex = lrn.sess_train
     nb = 2
     lrn.pr_prune([0.5] * len(lrn.maskable_vars))

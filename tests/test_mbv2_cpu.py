@@ -14,6 +14,7 @@ import pytest
 from pocketflow_b200 import graph as G
 from pocketflow_b200.flags import FLAGS
 from pocketflow_b200.nets import mobilenet_v2 as M2
+from support import expected_contributions, grad_inputs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _spec = importlib.util.spec_from_file_location('make_plan_snapshot',
@@ -187,15 +188,14 @@ def test_v2_inference_graph_dropout_is_an_alias():
 
 
 def test_v2_gradient_buffers_hold_exactly_the_consumers_contributions():
-    import test_planner_cpu as P
     ex = v2_executor(1.0)
     memo, state = {}, {ex.gkey(ex.loss.ce[1]): {'loss'}}
     for op in reversed(ex.ops):
         if op.type == 'Placeholder' or ex.gkey(op.output) not in state:
             continue
         if not (op.type in ('Reshape', 'Identity') or op in ex.fused_into):
-            assert state[ex.gkey(op.output)] == P.expected_contributions(ex, op.output, memo), op.name
-        for t in P.grad_inputs(ex, op):
+            assert state[ex.gkey(op.output)] == expected_contributions(ex, op.output, memo), op.name
+        for t in grad_inputs(ex, op):
             k = ex.gkey(t)
             state[k] = (state[k] | {op}) if k in state else {op}
 

@@ -1,29 +1,20 @@
 """MobileNet-v2 on the GPU: the fused linear-bottleneck BN + residual kernel (pf_bn_apply_add / _eval), the dropout
 kernels and their Philox stream, layer-local step parity of every learner on v2 at 224x224 against the oracle, the
 benchmarked batch under PF_POISON=1 with its CUDA-graph replay, and a TF-slim-named checkpoint round trip."""
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if ROOT not in sys.path:
-    sys.path.insert(0, ROOT)
-
-from oracle import pf_oracle as O  # noqa: E402
-from oracle.mbv2_oracle import DropoutStepOracle  # noqa: E402
-from pocketflow_b200 import ops  # noqa: E402
-from pocketflow_b200.flags import FLAGS  # noqa: E402
+from oracle import pf_oracle as O
+from oracle.mbv2_oracle import DropoutStepOracle
+from pocketflow_b200 import ops
+from pocketflow_b200.flags import FLAGS
+from support import check_selection, ref_mask, rel
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
 DEV = torch.device('cuda', 0)
-
-
-def rel(a, b):
-    return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
 
 
 def split_np(v):
@@ -80,32 +71,6 @@ def test_bn_apply_add_with_one_block_grid(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ dropout
-MASK32 = 0xffffffff
-
-
-def philox4x32_10(ctr, key):
-    """numpy restatement of Philox4x32-10 (Salmon et al., SC'11): ctr [..., 4] uint32, key (k0, k1)"""
-    c = [ctr[..., i].astype(np.uint64) for i in range(4)]
-    k0, k1 = np.uint64(key[0]), np.uint64(key[1])
-    m0, m1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57)
-    for r in range(10):
-        if r:
-            k0, k1 = (k0 + np.uint64(0x9E3779B9)) & np.uint64(MASK32), (k1 + np.uint64(0xBB67AE85)) & np.uint64(MASK32)
-        p0, p1 = m0 * c[0], m1 * c[2]
-        hi0, lo0 = p0 >> np.uint64(32), p0 & np.uint64(MASK32)
-        hi1, lo1 = p1 >> np.uint64(32), p1 & np.uint64(MASK32)
-        c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
-    return np.stack(c, -1).astype(np.uint32)
-
-
-def ref_mask(n, keep, seed, rank, step, stream=0):
-    """counter (element group [2 words], step [low word], stream), key (seed, rank)"""
-    g = np.arange((n + 3) // 4, dtype=np.uint64)
-    ctr = np.stack([g & np.uint64(MASK32), g >> np.uint64(32), np.full_like(g, step & MASK32),
-                    np.full_like(g, stream)], -1).astype(np.uint32)
-    w = philox4x32_10(ctr, (seed, rank)).reshape(-1)[:n]
-    u = ((w & np.uint32(0x7fffff)) | np.uint32(0x3f800000)).view(np.float32) - np.float32(1.0)
-    return np.floor(np.float32(keep) + u).astype(np.float32)
 
 
 def test_dropout_stream_is_philox4x32_10_and_keeps_keep_prob():
@@ -435,7 +400,6 @@ def test_v2_channel_pruned_rmt_selection_and_masked_steps(tmp_path):
     """chn-pruned-rmt on v2: its selection executors sample conv inputs that the linear-bottleneck fusion may hold only as
     operand planes; every sampled patch x W must reproduce the full model's output (err < 1e-6), the kept counts meet
     their targets, and masked steps follow"""
-    from test_cpr_gpu import check_selection
     lrn = make_v2('chn-pruned-rmt', cpr_nb_smpls=4, cpr_nb_crops_per_smpl=4, cpr_ista_nb_iters=30, cpr_lstsq_nb_iters=5,
                   cpr_save_path_ws=str(tmp_path / 'ws' / 'model.ckpt'), summ_step=10 ** 9, save_step=10 ** 9)
     ex = lrn.sess_train

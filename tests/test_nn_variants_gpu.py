@@ -18,6 +18,7 @@ import torch.nn.functional as F
 
 from oracle import pf_oracle as O
 from pocketflow_b200 import ops
+from support import bn_chain, fq_chain, pool_dx_ref, pool_ref, rel_err, sms, split_planes
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0')
@@ -30,15 +31,6 @@ WORST = {}                        # (family, form) -> worst error relative to it
 
 def note(family, form, err):
     WORST[(family, form)] = max(WORST.get((family, form), 0.0), err)
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def rel_err(got, ref):
-    assert torch.isfinite(got).all(), 'non-finite output'
-    return ((got.double() - ref).abs().max() / ref.abs().max()).item()
 
 
 # ------------------------------------------------------------------------------------------ depthwise
@@ -186,27 +178,6 @@ def test_rows_and_one_output_kernels_agree_bit_for_bit(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------ batch-norm
-def bn_chain(x, mean, rstd, gamma, beta, act):
-    """act(((x - mean) * rstd) * gamma + beta), each op rounded to fp32 on its own (eager torch)"""
-    y = ((x - mean) * rstd) * gamma + beta
-    if act >= 1:
-        y = torch.clamp_min(y, 0.0)
-    if act == 2:
-        y = torch.clamp_max(y, 6.0)
-    return y
-
-
-def fq_chain(y, mn, mx, bits):
-    """the activation fake-quant op chain of oracle/pf_oracle.uniform_quantize in fp32 torch, range (mn, mx) given"""
-    alpha = (mx - mn) + torch.tensor(1e-10, dtype=torch.float32, device=y.device)
-    k = torch.tensor(float(O.uq_k(bits)), dtype=torch.float32, device=y.device)
-    lv = torch.round(((y - mn) / alpha) * k)
-    return alpha * (lv / k) + mn, lv
-
-
-def split_planes(t):
-    hi = t.reshape(-1).to(torch.bfloat16)
-    return hi, (t.reshape(-1) - hi.float()).to(torch.bfloat16)
 
 
 def bn_splits(m, c):
@@ -406,30 +377,6 @@ def test_bn_apply_quant_matches_the_numpy_oracle():
 
 
 # ------------------------------------------------------------------------------------------ max-pool
-def pool_ref(x, k, st, pt, pb, P, Q):
-    """(y, first-max argmax code r * k + q, float64 dx of dy routed to it) with an unfold of the -inf padded input"""
-    n, h, w, c = x.shape
-    pr = (Q - 1) * st + k - w - pt
-    xp = F.pad(x.permute(0, 3, 1, 2), (pt, pr, pt, pb), value=float('-inf'))
-    cols = F.unfold(xp, k, stride=st).view(n, c, k * k, P * Q)
-    y = cols.max(2).values
-    idx = torch.arange(k * k, device=x.device).view(1, 1, -1, 1)
-    at_max = cols == y.unsqueeze(2)
-    am = torch.where(at_max, idx, k * k).min(2).values                          # first maximum, row-major
-    ties = (at_max.sum(2) > 1).float().mean().item()
-    return y.view(n, c, P, Q).permute(0, 2, 3, 1), am.view(n, c, P, Q).permute(0, 2, 3, 1), xp.shape, ties
-
-
-def pool_dx_ref(dy, am, k, st, pt, P, Q, n, h, w, c, hp, wp):
-    oh = torch.arange(P, device=dy.device).view(1, P, 1, 1)
-    ow = torch.arange(Q, device=dy.device).view(1, 1, Q, 1)
-    ih = oh * st + am // k
-    iw = ow * st + am % k
-    flat = ((torch.arange(n, device=dy.device).view(n, 1, 1, 1) * hp + ih) * wp + iw) * c + \
-        torch.arange(c, device=dy.device).view(1, 1, 1, c)
-    dxp = torch.zeros(n * hp * wp * c, dtype=torch.float64, device=dy.device)
-    dxp.index_add_(0, flat.reshape(-1), dy.double().reshape(-1))
-    return dxp.view(n, hp, wp, c)[:, pt:pt + h, pt:pt + w, :]
 
 
 # (id, n, h, w, c, k, stride, pad_t, pad_b, input)

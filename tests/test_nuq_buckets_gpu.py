@@ -9,6 +9,7 @@ from oracle import nuq_bucket_oracle as B
 from oracle import pf_oracle as O
 from pocketflow_b200 import ops
 from pocketflow_b200.flags import FLAGS
+from support import rel
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -169,10 +170,6 @@ def make(**flags):
     for k, v in dict(dict(nuql_use_buckets=True, summ_step=10 ** 9, save_step=10 ** 9), **flags).items():
         setattr(FLAGS, k, v)
     return create_learner(None, R.ModelHelper())
-
-
-def rel(a, b):
-    return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
 
 
 @pytest.mark.parametrize('mode,bucket_type', [('weights', 'channel'), ('cluster', 'channel'), ('both', 'channel'),

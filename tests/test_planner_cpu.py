@@ -13,6 +13,7 @@ import torch
 from pocketflow_b200 import graph as G
 from pocketflow_b200.engine import Executor
 from pocketflow_b200.flags import FLAGS
+from support import expected_contributions, grad_inputs
 
 
 def build(net, **flags):
@@ -33,39 +34,6 @@ def build(net, **flags):
             loss, _ = mh.calc_loss(lab, out, tv)
     return Executor(g, im, out, torch.device('cpu'), train=True, loss=loss, labels=lab,
                     optimizer=dict(kind='momentum', momentum=0.9))
-
-
-def grad_inputs(ex, op):
-    """Tensors whose gradient buffer op's backward WRITES (mirrors Executor.loss_and_backward)."""
-    if op.type in ('Placeholder', 'Reshape', 'Identity') or op in ex.fused_into:
-        return []
-    ins = op.inputs if op.type == 'Add' else op.inputs[:1]
-    out = []
-    for t in ins:
-        if t.op.type == 'Placeholder':
-            continue
-        if op.type == 'Add' and ex.gkey(t) is ex.gkey(op.output):
-            continue                                   # shared buffer: the Add's backward is a no-op for this input
-        out.append(t)
-    return out
-
-
-def expected_contributions(ex, t, memo):
-    """The set of WRITER ops whose contributions make up dL/dt."""
-    if t in memo:
-        return memo[t]
-    s = set()
-    for c in ex._consumers(t):
-        if c.type in ('Reshape', 'Identity') or c in ex.fused_into:
-            s |= expected_contributions(ex, c.output, memo)              # pass-through: same gradient
-        elif c.type == 'Add' and ex.gkey(t) is ex.gkey(c.output):
-            s |= expected_contributions(ex, c.output, memo)              # identity: shares the Add output's gradient
-        else:
-            s.add(c)
-    if t is ex.loss.ce[1] or (t in ex.alias and False):
-        s.add('loss')
-    memo[t] = s
-    return s
 
 
 @pytest.mark.parametrize('net,flags', [('resnet_at_cifar10', dict(resnet_size=20, batch_size=4)),

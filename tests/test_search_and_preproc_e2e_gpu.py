@@ -8,6 +8,7 @@ import importlib.util
 import os
 
 import pytest
+from support import make
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -38,9 +39,9 @@ def test_nuq_rl_bit_search_through_the_real_learner():
     (restore, per-layer bit-widths, codebooks re-fitted by the quantile initialisation, fine-tune, evaluate)."""
     import numpy as np
     from pocketflow_b200.flags import FLAGS
-    from test_learners_gpu import make
-    lrn = make('non-uniform', nuql_enbl_rl_agent=True, nuql_nb_rlouts=4, nuql_tune_global_steps=2, nuql_equivalent_bits=4,
-               nuql_w_bit_min=2, nuql_w_bit_max=6, nb_smpls_eval=64, batch_size_eval=16, enbl_dst=False)
+    lrn = make('resnet_at_cifar10', 'non-uniform', 16, reload=None, resnet_size=8, nuql_enbl_rl_agent=True,
+               nuql_nb_rlouts=4, nuql_tune_global_steps=2, nuql_equivalent_bits=4, nuql_w_bit_min=2, nuql_w_bit_max=6,
+               nb_smpls_eval=64, batch_size_eval=16, enbl_dst=False)
     ex = lrn.sess_train
     bits = lrn.optimal_w_bit_list
     assert len(bits) == len(ex.wq_ops) and all(2 <= b <= 6 for b in bits)

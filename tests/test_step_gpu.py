@@ -8,13 +8,10 @@ import torch
 from oracle.step_oracle import StepOracle
 from oracle import pf_oracle as O
 from pocketflow_b200.flags import FLAGS
+from support import rel
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-
-
-def rel(a, b):
-    return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
 
 
 def make_uq_learner(resnet_size=8, batch=16, w_bits=8, a_bits=8, dst=True, buckets=True):

@@ -14,14 +14,11 @@ import torch
 import torch.nn.functional as F
 
 from pocketflow_b200 import ops
+from support import rel_err, sms
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0')
 HW = 8                            # 8 x 8 images: 64 GEMM rows per image
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def tile_count(which):
@@ -54,11 +51,6 @@ def dgrad_ref(dy, w, r, shape):
     x = torch.zeros(shape, dtype=torch.float64, device=DEV, requires_grad=True)
     conv_ref(x, w, r).backward(dy)
     return x.grad
-
-
-def rel_err(got, ref):
-    assert torch.isfinite(got).all(), 'non-finite output'
-    return ((got.double() - ref).abs().max() / ref.abs().max()).item()
 
 
 def split_planes(t):

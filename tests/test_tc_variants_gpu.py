@@ -22,43 +22,12 @@ import torch
 import torch.nn.functional as F
 
 from pocketflow_b200 import ops
+from support import KEY_FIELDS, TC_REQUIRED, plan_key, rel_err, sms
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0')
 S_A = 0.0173                      # value of one activation level
 
-# plan key: (feed, pass, classes, bn, aff, ring, b_stationary, a_fp32) — pass 0 fwd, 1 dgrad, 2 wgrad
-KEY_FIELDS = ('feed', 'pass', 'classes', 'bn', 'aff', 'ring', 'b_stationary', 'a_fp32')
-
-
-def plan_key(plan):
-    return tuple(plan[f] for f in KEY_FIELDS)
-
-
-def _required():
-    req = set()
-    for bn in (16, 32, 64, 128):
-        for aff in (0, 1, 2):
-            req.add((1, 0, 0, bn, aff, 0, 0, 0))               # TMA fwd: split / act levels / weight levels
-        req.add((1, 1, 0, bn, 0, 0, 0, 0))                     # TMA unit-stride dgrad
-        for stat in (0, 1):
-            for fp32 in (0, 1):
-                req.add((0, 0, 0, bn, 0, 0, stat, fp32))       # cp.async fwd: streamed / stationary weights
-                req.add((0, 1, 0, bn, 0, 0, stat, fp32))       # cp.async dgrad (unit stride)
-        req.add((0, 1, 1, bn, 0, 0, 0, 0))                     # strided dgrad by pixel-parity classes
-        req.add((0, 1, 0, bn, 0, 0, 0, 0))                     # strided dgrad, classes off
-    for aff in (0, 2):
-        req.add((1, 0, 0, 64, aff, 2, 0, 0))                   # residual ring, depth 2
-        req.add((1, 0, 0, 64, aff, 4, 0, 0))                   # residual ring, depth 4
-    req.add((1, 1, 0, 64, 0, 2, 0, 0))                         # dgrad accumulate through the ring
-    for bn in (64, 128):
-        req.update({(1, 2, 0, bn, 0, 0, 0, 0), (1, 2, 0, bn, 1, 0, 0, 0), (0, 2, 0, bn, 0, 0, 0, 0)})
-    return req
-
-
-# Every variant the launchers can produce for the operand forms below.  cp.async kernels never get a ring on sm_90:
-# beside a 128 KB ring the shared memory holds fewer than two stages at BN >= 64 (pf_conv_tc.cu: launch_persist).
-REQUIRED = frozenset(_required())
 SEEN = {}                         # plan key -> first case id that produced it
 RAN = set()
 WORST = {}                        # (pass, operand form) -> worst error relative to max|ref|
@@ -66,10 +35,6 @@ WORST = {}                        # (pass, operand form) -> worst error relative
 
 def note(pass_, form, err):
     WORST[(pass_, form)] = max(WORST.get((pass_, form), 0.0), err)
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.fixture(autouse=True)
@@ -119,11 +84,6 @@ def wgrad_ref(x, dy, case):
     w = torch.zeros(r, s, c, k, dtype=torch.float64, device=DEV, requires_grad=True)
     conv_ref(x, w, case).backward(dy)
     return w.grad
-
-
-def rel_err(got, ref):
-    assert torch.isfinite(got).all(), 'non-finite output'
-    return ((got.double() - ref).abs().max() / ref.abs().max()).item()
 
 
 # ------------------------------------------------------------------------------------------ operands
@@ -501,5 +461,5 @@ def test_every_variant_was_reached():
     print('variant combinations reached (%d): ' % len(SEEN) + ', '.join(
         '%s=%s' % (dict(zip(KEY_FIELDS, k)), v) for k, v in sorted(SEEN.items())))
     print('worst error / max|ref|: ' + ', '.join('%s %s %.2e' % (p, f, e) for (p, f), e in sorted(WORST.items())))
-    missing = REQUIRED - set(SEEN)
+    missing = TC_REQUIRED - set(SEEN)
     assert not missing, 'variants never reached: %s' % sorted(missing)
