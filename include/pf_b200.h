@@ -443,6 +443,34 @@ int pf_conv2d_tc_dgrad_ex(const pf_conv_desc* d, const pf_tc_act* dy, const pf_t
                           void* stream);
 int pf_conv2d_tc_wgrad_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_act* dy, float* ws_dev, float* dw_dev,
                           void* stream);
+/* ---- u8 x u8 inference forward (pf_conv_tma.cu; reference: learners/uniform_quantization/utils.py:92-104, 163-199,
+ * the conv of the fake-quantized weight and activation) ----
+ * The TMA-fed ping-pong forward with BOTH operands as the uniform quantizers' own unsigned levels, one byte each:
+ *   x->plane0 = u8 activation levels q_a in [0, k_a] (layout of the NHWC tensor), x->plane1 = NULL, x->hdr = {scale =
+ *   alpha_a / k_a, nplanes = 1} and x->csum / x->nseg = ceil(Cin / 128) per-pixel channel-segment level sums, all written
+ *   by pf_bn_eval_levels_u8;  w->plane0 = u8 weight levels q_w in [0, k_w], K-major [Cout][R*S*Cin] (row pitch R*S*Cin),
+ *   w->plane1 = NULL, w->alpha / w->beta = the weight quantizer's bucket scales (per layer, or per output channel with
+ *   w->per_channel = 1), w->bits = log2(k_w + 1) <= 8.
+ * One u8 x u8 -> s32 wgmma per 32-wide k-slice gives S[m,n] = sum_K q_a q_w exactly (K * 255^2 < 2^31 for K < 33,000);
+ * the epilogue computes
+ *   y[m,n] = (scale * alpha_n / k_w) * S[m,n] + (scale * beta_n) * J[m],   J[m] = sum_K q_a (from csum),
+ * rounding only there, then bias, ReLU (relu != 0), the residual (residual_dev) and, with bn != NULL, the folded inference
+ * batch norm as pf_conv2d_tc_fwd_bn applies it.  A header with nplanes != 1 (the activation's minimum was not 0, so
+ * its values are not scale * level) makes every output NaN.  Requires pf_conv2d_u8_supported(d): Cin % 64 == 0,
+ * Cout % 64 == 0, strides <= 8, filters <= 16 x 16; there is no other kernel for u8 operands. */
+int pf_conv2d_u8_supported(const pf_conv_desc* d);
+int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, const float* bias_dev, int relu,
+                     const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn, void* stream);
+/* producer of the u8 operand (reference: utils/external/resnet_model.py:55-62 inference BN, then
+ * learners/uniform_quantization/utils.py:51-79 with the range of this batch): y = act(bn(x)) with the moving statistics
+ * (pf_bn_apply_eval's op chain), quantized per tensor, written as levels rint(((y - min) / alpha) * k) into levels_dev
+ * (m * c bytes) + hdr + csum (m * ceil(c / 128) floats).  have_range = 0: range_enc_dev[0..1] is reset and filled with
+ * min / max of y first (a pass of its own: the whole range is needed before any level); 1: it already holds them (a
+ * pf_bn_apply_eval of the same x with minmax_enc_dev = range_enc_dev).  C a power of two >= 16, bits 1..8. */
+int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
+                         float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
+                         uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
+                         float* csum_dev, void* stream);
 /* host-side decisions of the most recent tensor-core conv launch (fwd / dgrad / wgrad, either feed), recorded by the
  * launcher from the values it launches with, so that tests can tell which kernel variant a call exercised.  One
  * process-wide record, not synchronised: read it from the thread that launched.  Returns PF_ERR_INVALID_ARG when

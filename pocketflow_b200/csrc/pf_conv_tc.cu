@@ -1098,6 +1098,29 @@ int pf_conv2d_tc_fwd_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_w
   return conv_tma_launch(0, g, *x, *w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who);
 }
 
+int pf_conv2d_u8_supported(const pf_conv_desc* d) {
+  TcGeom g;
+  if (!d || tc_geom(d, &g, "pf_conv2d_u8_supported")) return 0;
+  return conv_tma_u8_eligible(g);
+}
+
+int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, const float* bias_dev, int relu,
+                     const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn, void* stream) {
+  const char* who = "pf_conv2d_u8_fwd";
+  PF_REQUIRE(x && w && x->plane0 && x->hdr && x->csum && w->plane0 && w->alpha && w->beta && y_dev, "%s: null pointer", who);
+  PF_REQUIRE(x->plane1 == nullptr && w->plane1 == nullptr, "%s: u8 operands have one plane", who);
+  PF_REQUIRE(x->nseg == (d ? (d->c + 127) / 128 : 0), "%s: nseg must be ceil(Cin / 128)", who);
+  TcGeom g;
+  int rc = tc_geom(d, &g, who);
+  if (rc) return rc;
+  PF_REQUIRE(conv_tma_u8_eligible(g), "%s: needs Cin %% 64 == 0, Cout %% 64 == 0, strides <= 8 and filters <= 16", who);
+  PF_REQUIRE((((uintptr_t)x->plane0 | (uintptr_t)w->plane0 | (uintptr_t)y_dev | (uintptr_t)residual_dev |
+               (uintptr_t)bias_dev | (uintptr_t)w->alpha | (uintptr_t)w->beta) & 15) == 0 &&
+                 ((uintptr_t)x->hdr & 7) == 0,
+             "%s: 16-byte alignment required (header: 8)", who);
+  return conv_tma_launch(0, g, *x, *w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who, bn, true);
+}
+
 int pf_conv2d_tc_dgrad_ex(const pf_conv_desc* d, const pf_tc_act* dy, const pf_tc_wt* wd, int accumulate, float* dx_dev,
                           void* stream) {
   const char* who = "pf_conv2d_tc_dgrad_ex";

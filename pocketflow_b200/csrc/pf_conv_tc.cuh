@@ -104,10 +104,11 @@ __device__ __forceinline__ void wg_tile_to_smem(float (&acc)[BN / 2], float* acc
 // the convolution of the fake-quantized tensors is   s_a s_c * sum_k j (n - centre)  +  s_a o_c * J[m],
 // J[m] = sum of the activation levels under the filter window of output row m (computed by the row's thread from
 // per-pixel channel sums and handed in as `my_j`).  AFF 1: only the scalar s_a (weight gradient: j (x) dy).
-// BNO (forward, AFF 0 only): after the fp32 store to `out`, the same register value also goes through the inference
+// BNO (forward; AFF 0, or AFF 2 of the u8 kernel): after the fp32 store to `out`, the same register value also goes through the inference
 // batch norm `bn` (pf_b200.h: pf_tc_bn_out) with pf_bn_apply_eval's op chain, and is stored as split-bf16 planes and /
 // or fp32: the BN pass that would re-read `out` is folded into this one.  The tile's column constants come in `aff_tab`
-// (bn_table: rstd, mean, gamma, beta of column c at c, BN + c, 2 BN + c, 3 BN + c), formed by the kernel before the
+// (bn_table: rstd, mean, gamma, beta of column c at c, BN + c, 2 BN + c, 3 BN + c; with AFF 2 they follow e1 / e2
+// at aff_tab + 512), formed by the kernel before the
 // epilogue: __frsqrt_rn has a called slow path, which inside the chunk loop would make ptxas save the loop's live
 // registers to local memory.  BNO loads the residual at each chunk instead of one chunk ahead (the second buffer would
 // not fit the registers beside the constants), and stores `out` with evict-first stores: nothing reads it soon, while
@@ -208,12 +209,13 @@ __device__ __forceinline__ void epilogue_tile_t(const float* __restrict__ acc, i
       e2 = make_float4(fmaf(aff.w_centre, sx, be.x) * a_s, fmaf(aff.w_centre, sy, be.y) * a_s,
                        fmaf(aff.w_centre, sz, be.z) * a_s, fmaf(aff.w_centre, sw_, be.w) * a_s);
     }
-    float4 brs, bmu, bga, bbe;                   // BNO: the columns' batch-norm constants
+    float4 brs, bmu, bga, bbe;                   // BNO: the columns' batch-norm constants (after e1 / e2 with AFF 2)
     if (BNO && cok) {
-      brs = *reinterpret_cast<const float4*>(aff_tab + cv);
-      bmu = *reinterpret_cast<const float4*>(aff_tab + BN + cv);
-      bga = *reinterpret_cast<const float4*>(aff_tab + 2 * BN + cv);
-      bbe = *reinterpret_cast<const float4*>(aff_tab + 3 * BN + cv);
+      const float* bt = AFF == 2 ? aff_tab + 512 : aff_tab;
+      brs = *reinterpret_cast<const float4*>(bt + cv);
+      bmu = *reinterpret_cast<const float4*>(bt + BN + cv);
+      bga = *reinterpret_cast<const float4*>(bt + 2 * BN + cv);
+      bbe = *reinterpret_cast<const float4*>(bt + 3 * BN + cv);
     }
     if (EXTRA == 1 && !BNO && c0 + c_step < BN) load_extra(c0 + c_step, xb);
     if (EXTRA == 1 && BNO) load_extra(c0, xa);
@@ -292,7 +294,7 @@ __device__ __forceinline__ void epilogue_rows(const float* acc, int c_begin, int
                                               const float* __restrict__ bias, int relu, int n0, int BN, int Ng,
                                               int lane, uint8_t* ring, const EpiAff& aff, float my_j, float* jrow,
                                               const float* aff_tab, int ring_depth, const pf_tc_bn_out& bn) {
-  static_assert(!BNO || AFF == 0, "the folded batch norm is an inference-mode (split-bf16 operand) epilogue");
+  static_assert(!BNO || AFF != 1, "the folded batch norm is an inference-mode (forward) epilogue");
   const int pitch = acc_pitch(BN);
   if (extra && ring && ring_depth == 2) epilogue_tile_t<2, AFF, 2, BNO>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
   else if (extra && ring) epilogue_tile_t<2, AFF, kRingDepth, BNO>(acc, pitch, my_row_off, rowoff, out, extra, bias, relu, n0, BN, Ng, lane, ring, aff, my_j, jrow, c_begin, c_step, aff_tab, bn);
@@ -338,9 +340,11 @@ void record_plan(const pf_tc_plan& p);
 // ---- TMA-fed kernels (pf_conv_tma.cu)
 void conv_tma_set_feed(int mode);
 bool conv_tma_eligible(int pass, const TcGeom& g);      // pass: 0 fwd, 1 dgrad, 2 wgrad
+bool conv_tma_u8_eligible(const TcGeom& g);             // pf_conv2d_u8_fwd
+// u8: forward with unsigned 8-bit activation and weight levels (pf_conv2d_u8_fwd)
 int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_wt& w, float* out, int accumulate,
                     const float* bias, int relu, const float* residual, cudaStream_t st, const char* who,
-                    const pf_tc_bn_out* bn = nullptr);
+                    const pf_tc_bn_out* bn = nullptr, bool u8 = false);
 int conv_tma_wgrad_launch(const TcGeom& g, const pf_tc_act& x, const pf_tc_act& dy, int BN, int pps, int splits,
                           float* partial, cudaStream_t st, const char* who);
 

@@ -11,7 +11,11 @@
 //     warp), stages are as deep as shared memory allows (up to 8);
 //   * an operand that is a <= 8-bit fake-quantized tensor arrives as its INTEGER LEVELS (exact in bf16): one plane
 //     instead of hi + lo.  MMAs per k-slice: levels x levels 1, levels x split 2, split x split 3; the per-channel
-//     scale, and the rank-1 term that the weight offset contributes, are applied by the epilogue (pf_conv_tc.cuh).
+//     scale, and the rank-1 term that the weight offset contributes, are applied by the epilogue (pf_conv_tc.cuh);
+//   * the u8 forward (pf_conv2d_u8_fwd, inference): both operands are the quantizers' own UNSIGNED 8-bit levels, one
+//     byte per element, K-major.  A k-stage is still 64 channels of one tap, now 64-byte rows (SWIZZLE_64B boxes and
+//     descriptors), and a k-slice is one u8 x u8 -> s32 wgmma of k = 32: the integer sum of level products is exact,
+//     and the same AFF 2 epilogue (weight centre 0) turns it into the fake-quantized model's output.
 #include <cuda.h>
 
 #include "pf_conv_tc.cuh"
@@ -22,7 +26,6 @@ using namespace pftma;
 
 constexpr int kTmaMaxStages = 8;
 constexpr int kTmaThreads = (kMmaWarps + 1) * 32;     // wgrad: warps 0-7 MMA warpgroups + epilogue, warp 8 TMA producer
-constexpr uint32_t kATileBytes = TM * 128;
 
 struct TmaP {
   int M, Ng, BN, nk, n_tiles, total_tiles;
@@ -94,20 +97,21 @@ __device__ __forceinline__ void conv_tma_epilogue_chunked(float (&acc)[2][64], c
   }
 }
 
-template <int AFF, int BN, int NA, int NB, bool BNO>
+template <int AFF, int BN, int NA, int NB, bool BNO, bool U8>
 __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, uint32_t stage_bytes,
                                                   uint32_t n_stages, uint64_t* full_bar, uint64_t* empty_bar,
                                                   uint64_t* ml_bar, uint64_t* epi_bar, int* tab_n0, float* out,
                                                   const float* bias, const float* residual) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = warp >> 2, q = warp & 3, wtid = tid & 127;   // epilogue rows [32 q, 32 q + 32) of the tile
-  const uint32_t b_bytes = (uint32_t)BN * 128u;
+  constexpr uint32_t kRow = U8 ? 64u : 128u, kATile = TM * kRow;   // bytes of one tile row / of the A tile
+  const uint32_t b_bytes = (uint32_t)BN * kRow;
   float* acc_s = reinterpret_cast<float*>(smem + p.stage_budget);
   long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(p.chunked ? 32 : BN));
   float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
   // AFF == 2: e1[256], e2[256] of the staged tile's columns; BNO: the folded batch norm's constants of them (bn_table)
   float* aff_tab = jrow_all + kMmaWarps * 32;
-  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : (BNO ? 4 * kMaxBN : 0)));
+  uint8_t* ring_all = reinterpret_cast<uint8_t*>(aff_tab + (AFF == 2 ? 2 * 256 : 0) + (BNO ? 4 * kMaxBN : 0));
   long long* rowoff = rowoff_all + warp * 32;
   float* jrow = jrow_all + warp * 32;
   uint8_t* ring = p.ring ? ring_all + (size_t)warp * p.ring * kRingSlotBytes : nullptr;
@@ -118,25 +122,36 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
     const uint32_t turn_ph = (uint32_t)(wg == 1 ? j : j - 1) & 1u;
     // ---- mainloop
     if (wait_turn) mbar_wait_bounded(&ml_bar[wg], turn_ph);
-    float acc[2][BN / 2];
+    std::conditional_t<U8, int, float> acc[2][BN / 2];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0;
     uint32_t s = it % n_stages, ph = (it / n_stages) & 1u, prev = 0;
     for (int ks = 0; ks < p.nk; ++ks) {
       mbar_wait_bounded(&full_bar[s], ph);                               // TMA bytes have landed
-      const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), a1 = a0 + kATileBytes;
-      const uint32_t b0 = a0 + (uint32_t)NA * kATileBytes, b1 = b0 + b_bytes;
+      const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), a1 = a0 + kATile;
+      const uint32_t b0 = a0 + (uint32_t)NA * kATile, b1 = b0 + b_bytes;
       wgmma_fence();
+      if constexpr (U8) {
+        // two k32 slices of 32 bytes per 64-byte row; 8-row groups 512 bytes apart
 #pragma unroll
-      for (int kk = 0; kk < BK / 16; ++kk) {
-        const uint64_t db0 = make_smem_desc(b0 + kk * 32, 16, 1024), db1 = make_smem_desc(b1 + kk * 32, 16, 1024);
+        for (int kk = 0; kk < 2; ++kk) {
+          const uint64_t db = make_smem_desc(b0 + kk * 32, 16, 512, kSwizzle64B);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {                                    // rows [64 h, 64 h + 64): 8 KB per plane
-          const uint32_t ha = (uint32_t)h * 64 * 128 + kk * 32;
-          wg_mma_kslice<BN, 0, NA, NB>(acc[h], make_smem_desc(a0 + ha, 16, 1024), make_smem_desc(a1 + ha, 16, 1024),
-                                       db0, db1);
+          for (int h = 0; h < 2; ++h)                                    // rows [64 h, 64 h + 64): 4 KB
+            WgmmaU8<BN>::mma(acc[h], make_smem_desc(a0 + (uint32_t)h * 64 * 64 + kk * 32, 16, 512, kSwizzle64B), db);
+        }
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk) {
+          const uint64_t db0 = make_smem_desc(b0 + kk * 32, 16, 1024), db1 = make_smem_desc(b1 + kk * 32, 16, 1024);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {                                  // rows [64 h, 64 h + 64): 8 KB per plane
+            const uint32_t ha = (uint32_t)h * 64 * 128 + kk * 32;
+            wg_mma_kslice<BN, 0, NA, NB>(acc[h], make_smem_desc(a0 + ha, 16, 1024), make_smem_desc(a1 + ha, 16, 1024),
+                                         db0, db1);
+          }
         }
       }
       wgmma_commit();
@@ -189,7 +204,7 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
     }
     if (wait_turn) mbar_wait_bounded(&epi_bar[wg], turn_ph);            // the staging tile is this warpgroup's
     constexpr bool TAB = AFF == 2 || BNO;
-    if constexpr (BN == 128 && AFF == 0 && !BNO) {
+    if constexpr (BN == 128 && AFF == 0 && !BNO && !U8) {
       if (p.chunked) {
         conv_tma_epilogue_chunked(acc, p, acc_s, n0, off, rowoff, out, bias, wg, q, lane);
         __syncwarp();
@@ -203,7 +218,10 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
     if (AFF == 2 && tab_was != n0) {
       // per-column constants of this tile's columns, when they differ from the staged table's (with one n-tile per
       // row of tiles this runs once per CTA):  e1[c] = s_a * alpha_c / k_w ,  e2[c] = s_a * (centre * alpha_c / k_w + beta_c)
-      const float a_s = p.aff.a_scale ? __ldg(p.aff.a_scale) : 1.f;
+      float a_s = p.aff.a_scale ? __ldg(p.aff.a_scale) : 1.f;
+      // u8 levels stand for scale * level only when the tensor's minimum is 0 (header: 1 plane); otherwise the
+      // activation offset has no term here, and the output is NaN rather than silently wrong
+      if (U8 && __ldg(&p.a_hdr->nplanes) != 1) a_s = __int_as_float(0x7fc00000);
       for (int c = wtid; c < BN; c += 128) {
         const bool cok = n0 + c < p.Ng;
         const int bi = p.aff.per_channel ? n0 + c : 0;
@@ -213,7 +231,7 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
         aff_tab[256 + c] = fmaf(p.aff.w_centre, sx, be) * a_s;
       }
     }
-    if (BNO && tab_was != n0) bn_table(p.bn, aff_tab, n0, BN, p.Ng, wtid, 128);
+    if (BNO && tab_was != n0) bn_table(p.bn, aff_tab + (AFF == 2 ? 512 : 0), n0, BN, p.Ng, wtid, 128);
     named_bar_sync(2 + wg, 128);                       // the staged tile (and table) are visible to the warpgroup
     if (TAB && tab_was != n0 && wtid == 0) *reinterpret_cast<volatile int*>(tab_n0) = n0;
     epilogue_rows<AFF, BNO>(acc_s + (size_t)(32 * q) * acc_pitch(BN), 0, 32, off, rowoff, out, extra, bias, p.relu, n0,
@@ -223,7 +241,7 @@ __device__ __forceinline__ void conv_tma_consumer(const TmaP& p, uint8_t* smem, 
   }
 }
 
-template <int AFF, int BN, bool BNO = false>
+template <int AFF, int BN, bool BNO = false, bool U8 = false>
 __global__ void __launch_bounds__(kPingPongThreads, 1)
 conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                 const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
@@ -237,8 +255,9 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
   int na = p.na;
   if (p.a_hdr) na = (__ldg(&p.a_hdr->nplanes) == 2) ? 2 : 1;
   const int nb = p.nb;
-  const uint32_t b_bytes = (uint32_t)BN * 128u;
-  const uint32_t stage_bytes = (uint32_t)na * kATileBytes + (uint32_t)nb * b_bytes;
+  constexpr uint32_t kRow = U8 ? 64u : 128u, kATile = TM * kRow;
+  const uint32_t b_bytes = (uint32_t)BN * kRow;
+  const uint32_t stage_bytes = (uint32_t)na * kATile + (uint32_t)nb * b_bytes;
   const uint32_t n_stages = min((uint32_t)kTmaMaxStages, (uint32_t)p.stage_budget / stage_bytes);
 
   if (tid == 0) {
@@ -279,10 +298,10 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
           const int r = (int)fdiv((uint32_t)tap, p.d_s), q = tap - r * p.S;
           const uint32_t ow = (uint32_t)(p.flip ? p.S - 1 - q : q), oh = (uint32_t)(p.flip ? p.R - 1 - r : r);
           const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-          const uint32_t sb = sa + (uint32_t)na * kATileBytes;
+          const uint32_t sb = sa + (uint32_t)na * kATile;
           mbar_arrive_expect_tx(&full_bar[s], stage_bytes);
           load_im2col(sa, &tmA0, &full_bar[s], cb * BK, cw, ch, img, ow, oh);
-          if (na == 2) load_im2col(sa + kATileBytes, &tmA1, &full_bar[s], cb * BK, cw, ch, img, ow, oh);
+          if (na == 2) load_im2col(sa + kATile, &tmA1, &full_bar[s], cb * BK, cw, ch, img, ow, oh);
           load_2d(sb, &tmB0, &full_bar[s], ks * BK, n0);
           if (nb == 2) load_2d(sb + b_bytes, &tmB1, &full_bar[s], ks * BK, n0);
           if (++s == n_stages) { s = 0; ph ^= 1u; }
@@ -294,14 +313,18 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant_
     // the plane counts are fixed for the whole launch: one straight-line mainloop per combination
     setmaxnreg_inc<kConsumerRegs>();
 #define PF_TMA_CONSUMER(NA_, NB_)                                                                                    \
-  conv_tma_consumer<AFF, BN, NA_, NB_, BNO>(p, smem, stage_bytes, n_stages, full_bar, empty_bar, ml_bar, epi_bar,     \
-                                            &tab_n0, out, bias, residual)
-    if (na == 2) {
-      if (nb == 2) PF_TMA_CONSUMER(2, 2);
-      else PF_TMA_CONSUMER(2, 1);
+  conv_tma_consumer<AFF, BN, NA_, NB_, BNO, U8>(p, smem, stage_bytes, n_stages, full_bar, empty_bar, ml_bar, epi_bar, \
+                                                &tab_n0, out, bias, residual)
+    if constexpr (U8) {
+      PF_TMA_CONSUMER(1, 1);
     } else {
-      if (nb == 2) PF_TMA_CONSUMER(1, 2);
-      else PF_TMA_CONSUMER(1, 1);
+      if (na == 2) {
+        if (nb == 2) PF_TMA_CONSUMER(2, 2);
+        else PF_TMA_CONSUMER(2, 1);
+      } else {
+        if (nb == 2) PF_TMA_CONSUMER(1, 2);
+        else PF_TMA_CONSUMER(1, 1);
+      }
     }
 #undef PF_TMA_CONSUMER
   }
@@ -489,6 +512,11 @@ bool conv_tma_eligible(int pass, const TcGeom& g) {
   return g.C % 64 == 0 && g.K % 64 == 0 && g.sh <= 8 && g.sw <= 8;
 }
 
+// the u8 forward has no cp.async sibling: only the shape decides
+bool conv_tma_u8_eligible(const TcGeom& g) {
+  return g.C % 64 == 0 && g.K % 64 == 0 && g.sh <= 8 && g.sw <= 8 && g.R <= 16 && g.S <= 16;
+}
+
 static int pick_bn(int Ng) {
   int BN = Ng >= 128 ? 128 : (Ng >= 64 ? 64 : (Ng >= 32 ? 32 : 16));
   const int forced = env_int("PF_TC_BN", 0);
@@ -508,7 +536,7 @@ static int pick_bn(int Ng) {
 // pass 0: fwd (a = x planes, b = [Cout][Kpad] weights); pass 1: unit-stride dgrad (a = dy planes, b = [Cin][Kpad_d])
 int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_wt& w, float* out, int accumulate,
                     const float* bias, int relu, const float* residual, cudaStream_t st, const char* who,
-                    const pf_tc_bn_out* bn) {
+                    const pf_tc_bn_out* bn, bool u8) {
   TmaP p;
   memset(&p, 0, sizeof(p));
   const int CC = pass == 0 ? g.C : g.K;
@@ -535,7 +563,8 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   p.accumulate = accumulate;
   p.relu = relu;
   const int m_tiles = (p.M + TM - 1) / TM;
-  const int BN = pick_bn(p.Ng);
+  // u8: the tile widths that have an s32 wgmma instantiated (output channels are multiples of 64)
+  const int BN = u8 ? (p.Ng >= 128 ? 128 : 64) : pick_bn(p.Ng);
   p.BN = BN;
   p.n_tiles = (p.Ng + BN - 1) / BN;
   p.total_tiles = m_tiles * p.n_tiles;
@@ -547,8 +576,12 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   p.na = a.plane1 ? 2 : 1;
   p.nb = w.plane1 ? 2 : 1;
   p.a_hdr = a.hdr;
-  PF_REQUIRE(a.hdr == nullptr || a.plane1 != nullptr, "%s: an operand with a device header needs both planes", who);
+  PF_REQUIRE(a.hdr == nullptr || a.plane1 != nullptr || u8, "%s: an operand with a device header needs both planes",
+             who);
   int aff = 0;
+  PF_REQUIRE(!u8 || (pass == 0 && w.alpha != nullptr && a.hdr != nullptr && a.plane1 == nullptr && w.plane1 == nullptr &&
+                      p.Ng % 64 == 0),
+             "%s: u8 operands are a forward pass of activation levels with a header and weight levels", who);
   if (w.alpha) {
     PF_REQUIRE(w.beta != nullptr && w.bits >= 1 && w.bits <= 8, "%s: weight levels need alpha, beta and 1..8 bits", who);
     PF_REQUIRE(a.csum != nullptr && a.nseg >= 1, "%s: weight levels need the operand's channel sums", who);
@@ -557,7 +590,7 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     p.aff.w_beta = w.beta;
     p.aff.per_channel = w.per_channel;
     p.aff.w_rk = 1.f / (float)((1 << w.bits) - 1);
-    p.aff.w_centre = (float)(1 << (w.bits - 1));
+    p.aff.w_centre = u8 ? 0.f : (float)(1 << (w.bits - 1));      // u8 weight levels are stored as they are
     p.aff.a_scale = a.hdr ? &a.hdr->scale : nullptr;
     p.csum = a.csum;
     p.nseg = a.nseg;
@@ -565,12 +598,14 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
     aff = 1;
     p.aff.a_scale = &a.hdr->scale;
   }
-  PF_REQUIRE(bn == nullptr || (pass == 0 && aff == 0), "%s: the folded batch norm needs a split-bf16 forward", who);
+  PF_REQUIRE(bn == nullptr || (pass == 0 && (aff == 0 || u8)), "%s: the folded batch norm needs a split-bf16 or u8 forward",
+             who);
   if (bn) p.bn = *bn;
   // ---- shared memory: [stages][accumulator tile, row offsets, J, column constants][residual ring]
-  const int stage_max = p.na * (int)kATileBytes + p.nb * BN * 128;
+  const int row_bytes = u8 ? 64 : 128;                  // one k-stage row: 64 channels of bf16 or of u8
+  const int stage_max = (p.na * TM + p.nb * BN) * row_bytes;
   const bool has_extra = residual != nullptr || accumulate;
-  const int aff_tab_bytes = aff == 2 ? 2 * 256 * 4 : (bn ? 4 * kMaxBN * 4 : 0);   // the tile's per-column constants
+  const int aff_tab_bytes = (aff == 2 ? 2 * 256 * 4 : 0) + (bn ? 4 * kMaxBN * 4 : 0);   // the tile's per-column constants
   const int epi_bytes = epi_fixed_bytes(BN) + aff_tab_bytes;
   // the residual / accumulate operand streams through a per-warp cp.async ring of 4 (else 2) 4 KB chunks when the
   // pipeline keeps enough stages beside it: 3, or nk + 1 for the short reductions of the 1x1 layers (a 64 -> 256 layer
@@ -611,12 +646,22 @@ int conv_tma_launch(int pass, const TcGeom& g, const pf_tc_act& a, const pf_tc_w
   if (p.total_tiles == 0) return PF_OK;
   // ---- tensor maps
   alignas(64) CUtensorMap tA0, tA1, tB0, tB1;
+  const int Kpad = pad64(Kdim);
+  if (u8) {
+    PF_TMA_ENCODE(encode_im2col_u8(&tA0, a.plane0, g.N, Hs, Ws, CC, p.base_w, p.base_h, Wo, Ho, p.str_w, p.str_h, BK, TM), who);
+    PF_TMA_ENCODE(encode_2d_u8(&tB0, w.plane0, (uint64_t)Kpad, (uint64_t)p.Ng, (uint64_t)Kpad, BK, (uint32_t)BN), who);
+    auto kern = BN == 128 ? (bn ? conv_tma_kernel<2, 128, true, true> : conv_tma_kernel<2, 128, false, true>)
+                          : (bn ? conv_tma_kernel<2, 64, true, true> : conv_tma_kernel<2, 64, false, true>);
+    PF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, kPingPongThreads, smem, st>>>(tA0, tA0, tB0, tB0, out, bias, residual, p);
+    PF_CHECK_LAUNCH(who);
+    return PF_OK;
+  }
   PF_TMA_ENCODE(encode_im2col_bf16(&tA0, a.plane0, g.N, Hs, Ws, CC, p.base_w, p.base_h, Wo, Ho, p.str_w, p.str_h, BK, TM), who);
   if (a.plane1)
     PF_TMA_ENCODE(encode_im2col_bf16(&tA1, a.plane1, g.N, Hs, Ws, CC, p.base_w, p.base_h, Wo, Ho, p.str_w, p.str_h, BK, TM), who);
   else
     tA1 = tA0;
-  const int Kpad = pad64(Kdim);
   PF_TMA_ENCODE(encode_2d_bf16(&tB0, w.plane0, (uint64_t)Kpad, (uint64_t)p.Ng, (uint64_t)Kpad, BK, (uint32_t)BN), who);
   if (w.plane1)
     PF_TMA_ENCODE(encode_2d_bf16(&tB1, w.plane1, (uint64_t)Kpad, (uint64_t)p.Ng, (uint64_t)Kpad, BK, (uint32_t)BN), who);

@@ -378,6 +378,91 @@ bn_apply_levels_kernel(const float* __restrict__ x, int64_t total, int C, int cs
   }
 }
 
+// The u8 operand of pf_conv2d_u8_fwd (inference): y = act(bn(x)) with the moving statistics (pf_bn_apply_eval's op
+// chain, rstd formed in the kernel), quantized with the per-tensor range of THIS batch, written as unsigned 8-bit levels
+// rint(((y - min) / alpha) * k) — the levels act_quant rebuilds its values from — plus the per-pixel channel-segment
+// level sums (csum, as bn_apply_levels_kernel writes them) and the header {alpha / k, 1}.  The range needs a grid-wide
+// reduction before any level is written, so this runs twice: RANGE = min / max of y into range_enc (ordered-uint, as
+// pf_bn_apply_eval accumulates it), then the levels.  A range that does not start at 0 (an activation offset the u8
+// convolution has no term for) is recorded as header {1, 0}.  Channel-stationary grid (host: chan_grid), C a power of
+// two >= 16.  HBM traffic: 4 B read per element and pass, 1 B written.
+template <bool RANGE>
+__global__ void __launch_bounds__(NT)
+bn_eval_levels_u8_kernel(const float* __restrict__ x, int64_t total, int C, int cshift, const float* __restrict__ mean,
+                         const float* __restrict__ var, float eps, const float* __restrict__ gamma,
+                         const float* __restrict__ beta, int act, uint32_t* __restrict__ range_enc, int q_bits,
+                         uint8_t* __restrict__ levels, pf_tc_act_hdr* __restrict__ hdr, float* __restrict__ csum,
+                         int nseg) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nvec = total >> 2;
+  const int64_t stride = (int64_t)gridDim.x * NT;
+  const int64_t first = (int64_t)blockIdx.x * NT + threadIdx.x;
+  const uint32_t c = (uint32_t)((first << 2) & (int64_t)(C - 1));
+  const float4 mu = __ldg(reinterpret_cast<const float4*>(mean + c));
+  float4 rs = __ldg(reinterpret_cast<const float4*>(var + c));
+  rs.x = __frsqrt_rn(__fadd_rn(rs.x, eps)); rs.y = __frsqrt_rn(__fadd_rn(rs.y, eps));
+  rs.z = __frsqrt_rn(__fadd_rn(rs.z, eps)); rs.w = __frsqrt_rn(__fadd_rn(rs.w, eps));
+  const float4 ga = __ldg(reinterpret_cast<const float4*>(gamma + c));
+  const float4 be = __ldg(reinterpret_cast<const float4*>(beta + c));
+  auto bn4 = [&](float4 v) {
+    return make_float4(pf_bn_act(v.x, mu.x, rs.x, ga.x, be.x, act), pf_bn_act(v.y, mu.y, rs.y, ga.y, be.y, act),
+                       pf_bn_act(v.z, mu.z, rs.z, ga.z, be.z, act), pf_bn_act(v.w, mu.w, rs.w, ga.w, be.w, act));
+  };
+  if (RANGE) {
+    __shared__ float s_mn[NT / 32], s_mx[NT / 32];
+    float mn = INFINITY, mx = -INFINITY;
+    for (int64_t i = first; i < nvec; i += stride) {
+      const float4 y = bn4(pf_ld_stream(x + (i << 2)));
+      mn = fminf(fminf(mn, y.x), fminf(y.y, fminf(y.z, y.w)));
+      mx = fmaxf(fmaxf(mx, y.x), fmaxf(y.y, fmaxf(y.z, y.w)));
+    }
+    mn = pf_warp_min(mn);
+    mx = pf_warp_max(mx);
+    if (lane == 0) {
+      s_mn[threadIdx.x >> 5] = mn;
+      s_mx[threadIdx.x >> 5] = mx;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      mn = lane < NT / 32 ? s_mn[lane] : INFINITY;
+      mx = lane < NT / 32 ? s_mx[lane] : -INFINITY;
+      mn = pf_warp_min(mn);
+      mx = pf_warp_max(mx);
+      if (lane == 0 && mn <= mx) {
+        atomicMin(range_enc, pf_enc(mn));
+        atomicMax(range_enc + 1, pf_enc(mx));
+      }
+    }
+    return;
+  }
+  const float qmn = pf_dec(__ldg(range_enc)), qmx = pf_dec(__ldg(range_enc + 1));
+  const float q_alpha = __fadd_rn(__fsub_rn(qmx, qmn), 1e-10f);
+  const float q_k = pf_uq_kf(q_bits), q_ra = __frcp_rn(q_alpha);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    hdr->scale = qmn == 0.f ? __fdiv_rn(q_alpha, q_k) : 1.f;
+    hdr->nplanes = qmn == 0.f ? 1 : 0;
+  }
+  const int L = min(C >> 2, 32);                       // lanes per channel segment
+  const int64_t wbase = first - lane;
+  for (int64_t i = first; wbase + (i - first) < nvec; i += stride) {   // warp-uniform trip count (segment shuffles)
+    const bool valid = i < nvec;
+    float part = 0.f;
+    if (valid) {
+      const float4 y = bn4(pf_ld_stream(x + (i << 2)));
+      const float lx = pf_quant_level(y.x, q_alpha, qmn, q_k, q_ra), ly = pf_quant_level(y.y, q_alpha, qmn, q_k, q_ra);
+      const float lz = pf_quant_level(y.z, q_alpha, qmn, q_k, q_ra), lw = pf_quant_level(y.w, q_alpha, qmn, q_k, q_ra);
+      *reinterpret_cast<uint32_t*>(levels + (i << 2)) =
+          (uint32_t)lx | ((uint32_t)ly << 8) | ((uint32_t)lz << 16) | ((uint32_t)lw << 24);
+      part = (lx + ly) + (lz + lw);
+    }
+    for (int o = L >> 1; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if (valid && (lane & (L - 1)) == 0) {
+      const int64_t e = i << 2;
+      csum[(e >> cshift) * nseg + (int)((e & (int64_t)(C - 1)) >> 7)] = part;
+    }
+  }
+}
+
 // BN backward, phase 1: per channel sum(dz) and sum(dz * xhat), dz = dy masked by the activation.
 __global__ void __launch_bounds__(NT)
 bn_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__ x, int M, int C,
@@ -977,6 +1062,43 @@ int pf_bn_apply_quant_levels(const float* x_dev, int64_t m, int c, const float* 
                                                                         beta_dev, act, y_dev, plane0_dev, plane1_dev,
                                                                         range_enc_dev, bits, hdr_dev, csum_dev, nseg);
   PF_CHECK_LAUNCH("pf_bn_apply_quant_levels");
+  return PF_OK;
+}
+
+int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
+                         float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
+                         uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
+                         float* csum_dev, void* stream) {
+  const char* who = "pf_bn_eval_levels_u8";
+  PF_REQUIRE(m > 0 && c >= 16 && (c & (c - 1)) == 0, "%s: C must be a power of two >= 16 (got %d)", who, c);
+  PF_REQUIRE(act >= 0 && act <= 2, "%s: act must be 0 (none), 1 (relu) or 2 (relu6)", who);
+  PF_REQUIRE(bits >= 1 && bits <= 8, "%s: u8 levels need 1..8 bits", who);
+  PF_REQUIRE(eps >= 0.f, "%s: eps < 0", who);
+  PF_REQUIRE(x_dev && moving_mean_dev && moving_var_dev && gamma_dev && beta_dev && range_enc_dev && levels_dev && hdr_dev &&
+                 csum_dev, "%s: null pointer", who);
+  PF_REQUIRE((((uintptr_t)x_dev | (uintptr_t)moving_mean_dev | (uintptr_t)moving_var_dev | (uintptr_t)gamma_dev |
+               (uintptr_t)beta_dev) & 15) == 0 && (((uintptr_t)levels_dev | (uintptr_t)hdr_dev) & 7) == 0,
+             "%s: fp32 tensors must be 16-byte aligned, levels / header 8-byte aligned", who);
+  const int64_t total = m * c;
+  int cshift = 0;
+  while ((1 << cshift) < c) ++cshift;
+  const int nseg = (c + 127) / 128;
+  const unsigned grid = chan_grid(total >> 2, c);
+  PF_REQUIRE(((int64_t)grid * NT) % (c >> 2) == 0, "%s: C = %d too large for the channel-stationary grid", who, c);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* lv = reinterpret_cast<uint8_t*>(levels_dev);
+  if (!have_range) {
+    const int rc = pf_minmax_reset(range_enc_dev, 1, stream);
+    if (rc) return rc;
+    bn_eval_levels_u8_kernel<true><<<grid, NT, 0, st>>>(x_dev, total, c, cshift, moving_mean_dev, moving_var_dev, eps,
+                                                        gamma_dev, beta_dev, act, range_enc_dev, bits, lv, hdr_dev,
+                                                        csum_dev, nseg);
+    PF_CHECK_LAUNCH(who);
+  }
+  bn_eval_levels_u8_kernel<false><<<grid, NT, 0, st>>>(x_dev, total, c, cshift, moving_mean_dev, moving_var_dev, eps,
+                                                       gamma_dev, beta_dev, act, range_enc_dev, bits, lv, hdr_dev, csum_dev,
+                                                       nseg);
+  PF_CHECK_LAUNCH(who);
   return PF_OK;
 }
 

@@ -73,13 +73,15 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 
 // ---- wgmma descriptors
 // Shared-memory matrix descriptor: start address, LBO, SBO in 16-byte units; bits 62-63 layout type
-// 1 = SWIZZLE_128B (tile base 1024-byte aligned).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// 1 = SWIZZLE_128B (tile base 1024-byte aligned), 2 = SWIZZLE_64B (tile base 512-byte aligned).
+constexpr uint32_t kSwizzle128B = 1, kSwizzle64B = 2;
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                                   uint32_t layout = kSwizzle128B) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
+  d |= (uint64_t)layout << 62;
   return d;
 }
 
@@ -103,6 +105,15 @@ __device__ __forceinline__ void wgmma_wait(float (&d)[H][R]) {
   for (int h = 0; h < H; ++h)
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[h][i])::"memory");
+}
+// the same for an s32 accumulator of H row blocks (u8 x u8 MMAs)
+template <int N, int H, int R>
+__device__ __forceinline__ void wgmma_wait(int (&d)[H][R]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+#pragma unroll
+  for (int h = 0; h < H; ++h)
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[h][i])::"memory");
 }
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 operands from shared memory, fp32 accumulator in registers.
@@ -218,6 +229,54 @@ template <> struct Wgmma<256> {
   }
 };
 
+// D[64 x N] += A[64 x 32] * B[N x 32]^T with unsigned 8-bit operands from shared memory (both K-major: the only
+// layout integer wgmma takes) and s32 accumulators in registers; the fragment layout is Wgmma's.  Exact: every product
+// is below 2^16, so a sum of K products stays below 2^31 for K < 33,000.
+template <int N>
+struct WgmmaU8;
+template <> struct WgmmaU8<64> {
+  __device__ __forceinline__ static void mma(int (&d)[32], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p;\n}\n"
+        :
+          "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(a), "l"(b), "r"(1)
+        : "memory");
+  }
+};
+template <> struct WgmmaU8<128> {
+  __device__ __forceinline__ static void mma(int (&d)[64], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p;\n}\n"
+        :
+          "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(a), "l"(b), "r"(1)
+        : "memory");
+  }
+};
+
 // the accumulator fragment of one m64 x N warpgroup tile -> fp32 rows [row0, row0 + 64) of a shared-memory tile
 template <int N>
 __device__ __forceinline__ void wgmma_store_acc(const float (&d)[N / 2], float* tile, int pitch, int row0, int wtid) {
@@ -227,6 +286,19 @@ __device__ __forceinline__ void wgmma_store_acc(const float (&d)[N / 2], float* 
   for (int j = 0; j < N / 8; ++j) {
     *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
     *reinterpret_cast<float2*>(r0 + 8 * pitch + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// the same for an s32 accumulator, each value rounded to fp32 once on the way
+template <int N>
+__device__ __forceinline__ void wgmma_store_acc(const int (&d)[N / 2], float* tile, int pitch, int row0, int wtid) {
+  const int w = wtid >> 5, l = wtid & 31;
+  float* r0 = tile + (size_t)(row0 + 16 * w + (l >> 2)) * pitch + 2 * (l & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(__int2float_rn(d[4 * j]), __int2float_rn(d[4 * j + 1]));
+    *reinterpret_cast<float2*>(r0 + 8 * pitch + 8 * j) =
+        make_float2(__int2float_rn(d[4 * j + 2]), __int2float_rn(d[4 * j + 3]));
   }
 }
 

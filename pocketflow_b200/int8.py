@@ -1,0 +1,308 @@
+"""Uniformly quantized models at inference on the 8-bit integer tensor cores.
+
+The uniform-quantization learner (`--learner uniform`) trains a network whose convolutions see fake-quantized operands:
+weights w_q = alpha_w[n] * q_w / k_w + beta_w[n] with levels q_w in [0, k_w] (one (alpha, beta) per layer, or per
+output channel with `channel` buckets), and every ReLU / ReLU6 output a_q = alpha_a * q_a / k_a + beta_a with its range
+taken from the current batch (learners/uniform_quantization/utils.py).  Evaluated as it is trained, such a model still
+runs in fp32 on split-bf16 operands.  This module runs it as integers where it can: a convolution whose weights have
+<= 8 bits and whose input is a quantized ReLU / ReLU6 output with <= 8 bits computes
+
+    y[m, n] = (alpha_a alpha_w[n] / (k_a k_w)) * sum_K q_a q_w  +  (alpha_a beta_w[n] / k_a) * sum_K q_a
+
+(beta_a = min(act) = 0 after a ReLU) with one u8 x u8 -> s32 tensor-core MMA per 32-wide k-slice, exact, and the
+rank-1 term from the activation's per-pixel level sums (pf_conv2d_u8_fwd).  The batch norm + ReLU that produces its
+input writes the u8 levels instead of split-bf16 planes (pf_bn_eval_levels_u8).
+
+Which convolutions run as integers is decided from what the graph and the quantizer settings show (`select`): weight
+bits, the producer of the input and its activation bits, and the shape the u8 kernel takes (Cin and Cout multiples of
+64).  Every other layer keeps the fake-quant inference kernels: the stem and the dense layer, first and last layers
+unless all layers are quantized, depthwise convolutions, `split` buckets.
+
+    im = IntModel.from_checkpoint(graph, images, logits, state, cfg)   # the learner's checkpoint (unquantized weights)
+    logits = im.forward(images_tensor)
+    im.export(path)                                                    # integer checkpoint + sidecar
+    im2 = IntModel.load(graph, images, logits, path)
+`graph` / `images` / `logits` are the network's inference graph (compact.build_eval_graph); `cfg` the quantizer settings
+(`config_from_flags`).
+"""
+import json
+import os
+
+import numpy as np
+
+from . import compact
+
+F32 = np.float32
+SIDECAR_VERSION = 1
+CFG_KEYS = ('weight_bits', 'activation_bits', 'quantize_all_layers', 'use_buckets', 'bucket_type', 'bucket_size')
+
+
+def config_from_flags():
+    """The uniform learner's quantizer settings (its --uql_* flags)."""
+    from .flags import FLAGS
+    import pocketflow_b200.learners.uniform_quantization.learner  # noqa: F401  (defines the --uql_* flags)
+    return dict(weight_bits=int(FLAGS.uql_weight_bits), activation_bits=int(FLAGS.uql_activation_bits),
+                quantize_all_layers=bool(FLAGS.uql_quantize_all_layers), use_buckets=bool(FLAGS.uql_use_buckets),
+                bucket_type=str(FLAGS.uql_bucket_type), bucket_size=int(FLAGS.uql_bucket_size))
+
+
+def quant_marks(graph, cfg):
+    """(quantized Conv2D / MatMul / depthwise ops, quantized Relu / Relu6 ops) of `graph`, as the learner marks them
+    (UniformQuantization.search_matmul_op / search_activation_op)."""
+    from .learners.uniform_quantization.utils import UniformQuantization
+    uq = UniformQuantization(graph, cfg['bucket_size'], cfg['use_buckets'], cfg['bucket_type'])
+    mm = uq.search_matmul_op(cfg['quantize_all_layers'])
+    acts = [op for op in uq.search_activation_op() if op.type in ('Relu', 'Relu6')]
+    return list(mm), acts
+
+
+def weight_levels(kernel, bits, per_channel):
+    """The weight quantizer's levels and scales of one kernel (the arithmetic of oracle.pf_oracle.uniform_quantize):
+    alpha = (max - min) + 1e-10, beta = min per bucket, q = rint(((w - beta) / alpha) * k) in fp32.  Returns
+    (levels uint8 with the kernel's shape, alpha [buckets], beta [buckets])."""
+    w = np.ascontiguousarray(kernel, F32)
+    cols = w.reshape(-1, w.shape[-1]) if per_channel else w.reshape(-1, 1)
+    mx, mn = cols.max(axis=0), cols.min(axis=0)
+    alpha = (mx - mn).astype(F32) + F32(1e-10)
+    beta = mn.astype(F32)
+    k = F32(2 ** bits - 1)
+    q = np.rint((((cols - beta) / alpha).astype(F32) * k).astype(F32))
+    return q.astype(np.uint8).reshape(w.shape), alpha.astype(F32), beta
+
+
+def dequantize(levels, alpha, beta, bits):
+    """alpha * (q / k) + beta in fp32, op by op (uq_inv_scale): the fake-quantized weight the levels stand for."""
+    q = np.asarray(levels, F32)
+    cols = q.reshape(-1, alpha.shape[0])
+    k = F32(2 ** bits - 1)
+    return ((alpha * (cols / k).astype(F32)).astype(F32) + beta).astype(F32).reshape(q.shape)
+
+
+def _conv_desc(op):
+    from . import ops
+    n, h, w, c = op.inputs[0].shape
+    _, p, q, k = op.output.shape
+    (kh, kw), (sh, sw), (pt, pl) = op.attrs['ksize'], op.attrs['strides'], op.attrs['pad']
+    return ops.conv_desc(n, h, w, c, k, kh, kw, p, q, sh, sw, pt, pl)
+
+
+def select(graph, logits, cfg):
+    """[(op name, None or the reason it keeps the fake-quant kernels)] for every Conv2D / MatMul / depthwise op in
+    graph order; None = it runs on the u8 kernel."""
+    from . import ops
+    mm, acts = quant_marks(graph, cfg)
+    mm, acts = set(mm), set(acts)
+    out = []
+    for op in compact.reachable_ops(graph, logits):
+        if op.type not in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative'):
+            continue
+        x = op.inputs[0]
+        why = None
+        if op not in mm:
+            why = 'weights not quantized (first / last layer)'
+        elif op.type == 'DepthwiseConv2dNative':
+            why = 'depthwise convolution'
+        elif op.type == 'MatMul':
+            why = 'dense layer'
+        elif cfg['use_buckets'] and cfg['bucket_type'] != 'channel':
+            why = '%s buckets' % cfg['bucket_type']
+        elif cfg['weight_bits'] > 8:
+            why = 'weight bits %d > 8' % cfg['weight_bits']
+        elif x.op not in acts or x.op.inputs[0].op.type != 'FusedBatchNorm' or len(x.op.inputs[0].consumers) != 1:
+            why = 'input is not a quantized batch norm + ReLU output'
+        elif cfg['activation_bits'] > 8:
+            why = 'activation bits %d > 8' % cfg['activation_bits']
+        else:
+            c = x.shape[-1]
+            if c < 16 or c & (c - 1):
+                why = 'input channels %d not a power of two' % c
+            elif not ops.conv2d_u8_supported(_conv_desc(op)):
+                why = 'shape %d -> %d channels (the u8 kernel needs multiples of 64)' % (c, op.output.shape[-1])
+        out.append((op.name, why))
+    return out
+
+
+def report_lines(sel):
+    """What tools/export_uq_int8.py prints: one line per layer."""
+    lines = ['%s: %s' % (name, 'u8 x u8 tensor cores' if why is None else 'fake-quant (%s)' % why) for name, why in sel]
+    n = sum(1 for _, why in sel if why is None)
+    lines.append('%d of %d layers run as integers' % (n, len(sel)))
+    return lines
+
+
+def _specs(graph, cfg, exclude=()):
+    """the Executor's weight_quant / act_quant specs of the fake-quant model, less the weight quantizers of `exclude`"""
+    mm, acts = quant_marks(graph, cfg)
+    mm = [op for op in mm if op.name not in exclude]
+    wq = dict(kind='uniform', ops=mm, bits=[cfg['weight_bits']] * len(mm), use_buckets=cfg['use_buckets'],
+              bucket_type=cfg['bucket_type'], bucket_size=cfg['bucket_size']) if mm else None
+    aq = dict(ops=acts, bits=[cfg['activation_bits']] * len(acts)) if acts else None
+    return wq, aq
+
+
+def _load(ex, state):
+    """Load an inference executor's parameters and prepare its tensor-core weight copies from the QUANTIZED kernels:
+    an inference executor prepares them once, when its store is loaded, and the weight quantizer has not run by then."""
+    ex.store.load_state_dict(state, strict=True)
+    if ex.wq is not None:
+        ex.wq.forward()
+    ex.prepare_static_weights()
+
+
+def fake_quant_executor(graph, images, logits, state, cfg, device):
+    """The fake-quantized model as the learner evaluates it, on `graph` in inference mode (engine.Executor)."""
+    from .engine import Executor
+    wq, aq = _specs(graph, cfg)
+    ex = Executor(graph, images, logits, device, train=False, weight_quant=wq, act_quant=aq)
+    _load(ex, state)
+    return ex
+
+
+class _U8Bn:
+    """The batch norm + quantized ReLU feeding u8 convolutions: writes the u8 levels, header and channel sums (and,
+    first, what its fake-quant lowering writes when other readers need the fp32 tensor or split-bf16 planes)."""
+
+    def __init__(self, ex, op, base, others):
+        import torch
+        self.ex, self.op, self.base, self.others = ex, op, base, others
+        st = ex.store
+        c = op.output.shape[-1]
+        self.m, self.c = op.output.numel // c, c
+        self.args = (st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance']), op.attrs['epsilon'],
+                     st.view(op.vars['gamma']), st.view(op.vars['beta']), ex.fused_act.get(op, 0))
+        self.bits = ex.act_quant['bits'][base.aq]
+        self.levels = torch.empty(op.output.numel, dtype=torch.uint8, device=ex.device)
+        self.hdr = torch.zeros(2, dtype=torch.int32, device=ex.device)
+        self.csum = torch.empty(self.m * ((c + 127) // 128), dtype=torch.float32, device=ex.device)
+
+    def forward(self, training):
+        from . import ops
+        if self.others:
+            self.base.forward(training)
+        with self.ex.timed('act_quant'):
+            ops.bn_eval_levels_u8(self.ex.T(self.op.inputs[0]), self.m, self.c, *self.args, self.bits, self.base.slot,
+                                  self.levels, self.hdr, self.csum, have_range=self.others)
+
+
+class _U8Conv:
+    """A convolution on the u8 kernel, from the levels of its input's producer and its own weight levels."""
+
+    def __init__(self, ex, op, bn, levels, alpha, beta, bits):
+        from .engine import _TcConv
+        import torch
+        self.ex, self.op, self.bn, self.bits = ex, op, bn, bits
+        self.d = ex.desc[op]
+        dev = ex.device
+        self.wl = torch.from_numpy(np.ascontiguousarray(levels.reshape(-1, levels.shape[-1]).T)).to(dev)
+        self.alpha = torch.from_numpy(np.ascontiguousarray(alpha, F32)).to(dev)
+        self.beta = torch.from_numpy(np.ascontiguousarray(beta, F32)).to(dev)
+        tc = ex.conv[op]
+        assert isinstance(tc, _TcConv), op.name
+        self.res, self.bn_out = tc.res, tc.bn_out
+
+    def prepare_weights(self):
+        """the levels are uploaded once"""
+
+    def forward(self):
+        from . import ops
+        ex, op = self.ex, self.op
+        bias = ex.store.view(op.vars['bias']) if 'bias' in op.vars else None
+        res = ex.T(self.res) if self.res is not None else None
+        with ex.timed('conv_fwd'):
+            ops.conv2d_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.bn.csum, self.wl, self.alpha, self.beta,
+                              self.bits, ex.buf[op.output], bias, op in ex.fused_act, res, self.bn_out)
+
+
+class IntModel:
+    """A uniformly quantized model whose eligible convolutions run on the u8 tensor cores (engine.Executor in inference
+    mode, with those convolutions and the batch norms feeding them lowered to the u8 kernels)."""
+
+    def __init__(self, graph, images, logits, cfg, state, wlevels, device=None):
+        """state: {variable name: fp32 array} of every variable but the integer layers' kernels; wlevels: {conv op
+        name: (levels uint8 HWIO, alpha, beta)} of the integer layers"""
+        import torch
+        from .engine import Executor
+        self.graph, self.images, self.logits, self.cfg = graph, images, logits, dict(cfg)
+        self.sel = select(graph, logits, cfg)
+        ints = [name for name, why in self.sel if why is None]
+        if sorted(ints) != sorted(wlevels):
+            raise ValueError('the weight levels do not cover the integer layers: %s' % sorted(set(ints) ^ set(wlevels)))
+        self.wlevels = wlevels
+        self.state = dict(state)
+        bits = cfg['weight_bits']
+        byname = {op.name: op for op in compact.reachable_ops(graph, logits)}
+        full = dict(state)
+        for name, (lv, al, be) in wlevels.items():                 # the executor's copy: the fake-quantized kernel
+            full[byname[name].vars['kernel'].name] = dequantize(lv, al, be, bits)
+        self.device = device or torch.device('cuda', torch.cuda.current_device())
+        wq, aq = _specs(graph, cfg, exclude=set(ints))
+        self.ex = ex = Executor(graph, images, logits, self.device, train=False, weight_quant=wq, act_quant=aq)
+        _load(ex, full)
+        u8_readers = {}
+        for name in ints:
+            op = byname[name]
+            u8_readers.setdefault(ex._root(op.inputs[0]).op, []).append(op)
+        for bn, readers in u8_readers.items():
+            fp_readers = [c for c in ex.ops if c in ex.tc and c not in readers and ex.planes_of(c.inputs[0]) is not None
+                          and ex._root(c.inputs[0]).op is bn]
+            others = ex.bn_need_f32.get(bn, True) or bool(fp_readers)
+            ex.batch_norm[bn] = _U8Bn(ex, bn, ex.batch_norm[bn], others)
+        for name in ints:
+            op = byname[name]
+            lv, al, be = wlevels[name]
+            ex.conv[op] = _U8Conv(ex, op, ex.batch_norm[ex._root(op.inputs[0]).op], lv, al, be, bits)
+
+    @classmethod
+    def from_checkpoint(cls, graph, images, logits, state, cfg, device=None):
+        """From the uniform learner's checkpoint (unquantized weights under any one scope, compact.map_state)."""
+        full = compact.map_state(graph, compact.reachable_ops(graph, logits), state)
+        per_channel = cfg['use_buckets'] and cfg['bucket_type'] == 'channel'
+        byname = {op.name: op for op in compact.reachable_ops(graph, logits)}
+        wlevels = {}
+        for name, why in select(graph, logits, cfg):
+            if why is None:
+                kname = byname[name].vars['kernel'].name
+                wlevels[name] = weight_levels(full.pop(kname), cfg['weight_bits'], per_channel)
+        return cls(graph, images, logits, cfg, full, wlevels, device)
+
+    def forward(self, images=None):
+        """Logits (device tensor, the executor's own buffer) of `images` (or of what the input buffer holds)."""
+        if images is not None:
+            self.ex.buf[self.images].copy_(images)
+        return self.ex.forward(training=False)
+
+    def export(self, path):
+        """Write the integer checkpoint `path`.npz (the other variables in fp32 under their names; per integer layer
+        `<kernel>/levels` uint8 HWIO, `<kernel>/alpha` and `<kernel>/beta`) and the sidecar `path`.int8.json (quantizer
+        settings and the layer selection).  Returns the checkpoint's file name."""
+        os.makedirs(os.path.dirname(path) or '.', exist_ok=True)
+        byname = {op.name: op for op in compact.reachable_ops(self.graph, self.logits)}
+        arrays = {k.replace('/', '|'): v for k, v in self.state.items()}
+        for name, (lv, al, be) in self.wlevels.items():
+            k = byname[name].vars['kernel'].name[:-2]
+            arrays[(k + '/levels').replace('/', '|')] = lv
+            arrays[(k + '/alpha').replace('/', '|')] = al
+            arrays[(k + '/beta').replace('/', '|')] = be
+        fn = path + '.npz'
+        np.savez(fn, **arrays)
+        with open(path + '.int8.json', 'w') as f:
+            json.dump(dict(version=SIDECAR_VERSION, config=self.cfg, layers=[[n, w] for n, w in self.sel]), f)
+        return fn
+
+    @classmethod
+    def load(cls, graph, images, logits, path, device=None):
+        """Rebuild the integer model from what export(path) wrote."""
+        with open(path + '.int8.json') as f:
+            rec = json.load(f)
+        if rec.get('version') != SIDECAR_VERSION:
+            raise ValueError('%s.int8.json: unsupported sidecar version %r' % (path, rec.get('version')))
+        cfg = {k: rec['config'][k] for k in CFG_KEYS}
+        d = np.load(path + '.npz')
+        arrays = {k.replace('|', '/'): d[k] for k in d.files}
+        byname = {op.name: op for op in compact.reachable_ops(graph, logits)}
+        wlevels = {}
+        for name, why in rec['layers']:
+            if why is None:
+                k = byname[name].vars['kernel'].name[:-2]
+                wlevels[name] = (arrays.pop(k + '/levels'), arrays.pop(k + '/alpha'), arrays.pop(k + '/beta'))
+        return cls(graph, images, logits, cfg, arrays, wlevels, device)

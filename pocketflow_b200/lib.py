@@ -73,6 +73,10 @@ SIGNATURES = {
     'pf_conv2d_tc_dgrad_ex': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
     'pf_conv2d_tc_wgrad_ex': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_conv2d_tc_last_plan': (c_i32, [c_vp]),
+    'pf_conv2d_u8_supported': (c_i32, [c_vp]),
+    'pf_conv2d_u8_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    'pf_bn_eval_levels_u8': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp,
+                                     c_vp, c_vp]),
     'pf_tc_probe': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32] + [ctypes.c_uint32] * 6 + [c_vp]),
     'pf_dwconv_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_dwconv_dgrad': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),

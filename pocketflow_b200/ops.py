@@ -1139,6 +1139,39 @@ def conv2d_tc_wgrad_ex(d, x_act, dy_act, ws, dw):
                                                  _stream()), 'pf_conv2d_tc_wgrad_ex')
 
 
+def conv2d_u8_supported(d):
+    """the shapes pf_conv2d_u8_fwd runs: Cin and Cout multiples of 64, strides <= 8, filters <= 16 x 16"""
+    return bool(_lib.load().pf_conv2d_u8_supported(ctypes.byref(d)))
+
+
+def conv2d_u8_fwd(d, x_levels, hdr, csum, w_levels, alpha, beta, bits, y, bias=None, relu=False, residual=None,
+                  bn_out=None):
+    """y = the fake-quantized conv from u8 levels (pf_conv2d_u8_fwd): x_levels uint8 [N, H, W, Cin] with its header and
+    channel sums (bn_eval_levels_u8), w_levels uint8 [Cout, R*S*Cin], alpha / beta the weight bucket scales ([1] per
+    layer or [Cout] per channel); bn_out: a TcBnOut folded into the epilogue"""
+    if x_levels.dtype != torch.uint8 or w_levels.dtype != torch.uint8:
+        raise ValueError('conv2d_u8_fwd: the levels are uint8 tensors')
+    _check_f32(csum, alpha, beta, y, bias, residual)
+    act = _lib.TcAct(x_levels.data_ptr(), 0, hdr.data_ptr(), csum.data_ptr(), (d.c + 127) // 128, 0)
+    wt = _lib.TcWt(w_levels.data_ptr(), 0, alpha.data_ptr(), beta.data_ptr(), int(alpha.numel() > 1), int(bits))
+    _lib.check(_lib.load().pf_conv2d_u8_fwd(ctypes.byref(d), ctypes.byref(act), ctypes.byref(wt), _p(bias),
+                                            int(bool(relu)), _p(residual), _p(y),
+                                            ctypes.byref(bn_out) if bn_out is not None else None, _stream()),
+               'pf_conv2d_u8_fwd')
+
+
+def bn_eval_levels_u8(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, bits, rng, levels, hdr, csum, have_range=False):
+    """u8 levels of Q(act(bn(x))) with the moving statistics and this batch's range (pf_bn_eval_levels_u8): levels
+    uint8 [m * c], hdr int32 [2] (pf_tc_act_hdr), csum float32 [m * ceil(c / 128)], rng int32 [2] (the range, ordered
+    encoding); have_range: rng already holds the range of act(bn(x))"""
+    if levels.dtype != torch.uint8:
+        raise ValueError('bn_eval_levels_u8: levels must be uint8')
+    _check_f32(x, mov_mean, mov_var, gamma, beta, csum)
+    _lib.check(_lib.load().pf_bn_eval_levels_u8(_p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma), _p(beta),
+                                                int(act), int(bits), _p(rng), int(bool(have_range)), _p(levels), _p(hdr),
+                                                _p(csum), _stream()), 'pf_bn_eval_levels_u8')
+
+
 def conv2d_tc_last_plan():
     """Host-side plan of the most recent tensor-core conv launch (pf_tc_plan) as a dict: which feed, pass and kernel
     variant ran, and with what tile width, ring depth, stages, grid and split-K."""

@@ -1,0 +1,100 @@
+#!/usr/bin/env python
+"""Per-layer times of the u8 x u8 convolutions of an integer model against the fake-quant convolutions they replace.
+
+Every convolution that the integer model (pocketflow_b200/int8.py) runs on the u8 kernel is launched alone, n times
+between CUDA events, as is the same layer of the fake-quantized model (split-bf16 operands, three MMAs per k-slice),
+both on the inputs a forward of the seed-initialised model left in their buffers.  Each line gives both times and the
+u8 kernel's lower bound: the larger of the FLOP bound (2 M N K at the u8 data-sheet rate, 1,979 dense TOPS) and the byte
+bound (u8 operands read once, fp32 output written once, at 3.35 TB/s).
+
+    python tools/bench_int8.py --net resnet_at_ilsvrc12 --resnet_size 50 --batch_size_eval 128 --json out.json
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tools'))
+
+U8_OPS_PER_S = 1979e12
+HBM_BYTES_PER_S = 3.35e12
+
+
+def parse(argv=None):
+    p = argparse.ArgumentParser(description=__doc__.split('\n\n')[0])
+    p.add_argument('--net', default='resnet_at_ilsvrc12')
+    p.add_argument('--resnet_size', type=int, default=None)
+    p.add_argument('--mobilenet_version', type=int, default=None)
+    p.add_argument('--batch_size_eval', type=int, default=128)
+    p.add_argument('--launches', type=int, default=50, help='launches per timed layer')
+    p.add_argument('--json', default=None)
+    return p.parse_args(argv)
+
+
+def _ms(fn, n, torch):
+    for _ in range(3):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(n):
+        fn()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b) / n
+
+
+def main(argv=None):
+    args = parse(argv)
+    import torch
+    from export_uq_int8 import gpu_name, load_state, setup
+    from pocketflow_b200 import compact, int8
+    args.ckpt_dir = None
+    for k, v in dict(uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel',
+                     uql_bucket_size=256, uql_quantize_all_layers=False).items():
+        setattr(args, k, v)
+    graph, images, logits, cfg = setup(args)
+    state = load_state(args, graph, logits)
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    im = int8.IntModel.from_checkpoint(graph, images, logits, state, cfg, dev)
+    fq = int8.fake_quant_executor(graph, images, logits, compact.map_state(graph, compact.reachable_ops(graph, logits),
+                                                                           state), cfg, dev)
+    x = torch.randn(images.shape, generator=torch.Generator().manual_seed(0)).to(dev)
+    im.forward(x)
+    fq.buf[images].copy_(x)
+    fq.forward(training=False)
+    torch.cuda.synchronize()
+    fq_conv = {op.name: lo for op, lo in fq.conv.items()}
+    rows, tot = [], dict(u8=0.0, fq=0.0, bound=0.0)
+    for op, lo in im.ex.conv.items():
+        if not isinstance(lo, int8._U8Conv):
+            continue
+        d = lo.d
+        m, k, n = d.n * d.p * d.q, d.r * d.s * d.c, d.k
+        flop_s = 2.0 * m * n * k / U8_OPS_PER_S
+        byte_s = (d.n * d.h * d.w * d.c + n * k + 4 * m * n) / HBM_BYTES_PER_S
+        t_u8 = _ms(lo.forward, args.launches, torch)
+        t_fq = _ms(fq_conv[op.name].forward, args.launches, torch)
+        bound = max(flop_s, byte_s) * 1e3
+        rows.append(dict(op=op.name, m=m, n=n, k=k, u8_ms=t_u8, fake_quant_ms=t_fq, bound_ms=bound,
+                         bound_by='flops' if flop_s >= byte_s else 'bytes', u8_share_of_bound=bound / t_u8))
+        for key, v in (('u8', t_u8), ('fq', t_fq), ('bound', bound)):
+            tot[key] += v
+        print('%-48s M %7d N %5d K %5d | u8 %.4f ms  fake-quant %.4f ms | bound %.4f ms (%s) = %.0f %% of u8'
+              % (op.name, m, n, k, t_u8, t_fq, bound, rows[-1]['bound_by'], 100 * bound / t_u8))
+    print('all %d u8 layers: u8 %.3f ms, fake-quant %.3f ms, bound %.3f ms' % (len(rows), tot['u8'], tot['fq'],
+                                                                              tot['bound']))
+    res = dict(net=args.net, resnet_size=args.resnet_size, batch=args.batch_size_eval, layers=rows, totals=tot,
+               gpu=gpu_name(torch))
+    print('gpu: ' + res['gpu'])
+    if args.json:
+        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+        with open(args.json, 'w') as f:
+            json.dump(res, f, indent=1)
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())

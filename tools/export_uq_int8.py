@@ -1,0 +1,149 @@
+#!/usr/bin/env python
+"""Export a uniformly quantized model as an integer model, and time it against the fake-quantized model.
+
+The latest checkpoint of a `--learner uniform` run (npz or TF bundle) is turned into an integer model
+(pocketflow_b200/int8.py): u8 weight levels with their per-layer or per-channel alpha / beta for every convolution that
+runs on the u8 x u8 tensor cores, every other variable (batch-norm constants included) in fp32, plus a sidecar JSON of
+the quantizer settings and the layer selection.  Each layer is reported with the path it runs on, and why.  Then the
+inference forward of both models is timed as CUDA-graph replays at --batch_size_eval, alternating in one process.
+
+    python tools/export_uq_int8.py --net resnet_at_ilsvrc12 --resnet_size 50 --ckpt_dir ./uql_quant_models \\
+        --uql_weight_bits 8 --uql_activation_bits 8 --uql_use_buckets --batch_size_eval 128 --out ./rn50_int8/model
+
+Without --ckpt_dir the model keeps its seed initialisation (for speed measurements only).
+"""
+import argparse
+import importlib
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tools'))
+
+
+def parse(argv=None):
+    p = argparse.ArgumentParser(description=__doc__.split('\n\n')[0])
+    p.add_argument('--net', default='resnet_at_ilsvrc12', help='pocketflow_b200.nets module with a ModelHelper')
+    p.add_argument('--resnet_size', type=int, default=None)
+    p.add_argument('--mobilenet_version', type=int, default=None)
+    p.add_argument('--ckpt_dir', default=None, help='directory of the uniform learner\'s checkpoint (default: seed init)')
+    p.add_argument('--out', default='./models_uq_int8/model', help='integer checkpoint path prefix')
+    p.add_argument('--uql_weight_bits', type=int, default=8)
+    p.add_argument('--uql_activation_bits', type=int, default=8)
+    p.add_argument('--uql_use_buckets', action='store_true')
+    p.add_argument('--uql_bucket_type', default='channel', choices=('channel', 'split'))
+    p.add_argument('--uql_bucket_size', type=int, default=256)
+    p.add_argument('--uql_quantize_all_layers', action='store_true')
+    p.add_argument('--batch_size_eval', type=int, default=100)
+    p.add_argument('--nb_repts_warmup', type=int, default=20, help='graph replays before timing')
+    p.add_argument('--nb_repts', type=int, default=50, help='graph replays per timed window')
+    p.add_argument('--nb_rounds', type=int, default=5, help='alternating (fake-quant, integer) timed windows')
+    p.add_argument('--no_time', action='store_true', help='export only')
+    p.add_argument('--json', default=None, help='write the measurements here')
+    return p.parse_args(argv)
+
+
+def setup(args):
+    """(graph, images, logits, quantizer config) of the net's inference graph at --batch_size_eval"""
+    from pocketflow_b200 import compact, int8
+    from pocketflow_b200.flags import FLAGS
+    net = importlib.import_module('pocketflow_b200.nets.' + args.net)           # defines the net's flags
+    import pocketflow_b200.learners.uniform_quantization.learner  # noqa: F401  (the --uql_* flags)
+    FLAGS.reset()
+    if args.resnet_size is not None:
+        FLAGS.resnet_size = args.resnet_size
+    if args.mobilenet_version is not None:
+        FLAGS.mobilenet_version = args.mobilenet_version
+    FLAGS.batch_size_eval = args.batch_size_eval
+    for k in ('uql_weight_bits', 'uql_activation_bits', 'uql_use_buckets', 'uql_bucket_type', 'uql_bucket_size',
+              'uql_quantize_all_layers'):
+        setattr(FLAGS, k, getattr(args, k))
+    graph, images, logits = compact.build_eval_graph(net.ModelHelper(), args.batch_size_eval)
+    return graph, images, logits, int8.config_from_flags()
+
+
+def load_state(args, graph, logits):
+    from pocketflow_b200 import compact
+    from pocketflow_b200.learners.abstract_learner import latest_checkpoint, load_checkpoint
+    if args.ckpt_dir:
+        fn = latest_checkpoint(args.ckpt_dir) if os.path.isdir(args.ckpt_dir) else None
+        if fn is None:
+            raise ValueError('no checkpoint found in ' + args.ckpt_dir)
+        print('quantized model restored from ' + fn)
+        return load_checkpoint(fn)
+    rng = np.random.default_rng(1)
+    return {v.name: v.initializer(rng, v.shape) for op in compact.reachable_ops(graph, logits) for v in op.vars.values()}
+
+
+def gpu_name(torch):
+    try:
+        return subprocess.check_output(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm',
+                                        '--format=csv,noheader'], text=True).strip()
+    except (OSError, subprocess.CalledProcessError):
+        return torch.cuda.get_device_name(0)
+
+
+def main(argv=None):
+    args = parse(argv)
+    import torch
+    from export_chn_pruned import _capture, _replay_ms
+    from pocketflow_b200 import compact, int8
+    graph, images, logits, cfg = setup(args)
+    state = load_state(args, graph, logits)
+    for line in int8.report_lines(int8.select(graph, logits, cfg)):
+        print(line)
+    if not torch.cuda.is_available():
+        raise RuntimeError('the integer model runs on the GPU: no CUDA device found')
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    im = int8.IntModel.from_checkpoint(graph, images, logits, state, cfg, dev)
+    print('integer model written to ' + im.export(args.out) + ' (+ %s.int8.json)' % args.out)
+    if args.no_time:
+        return 0
+    fq = int8.fake_quant_executor(graph, images, logits, compact.map_state(graph, compact.reachable_ops(graph, logits),
+                                                                           state), cfg, dev)
+    x = torch.randn(images.shape, generator=torch.Generator().manual_seed(0)).to(dev)
+    fq.buf[images].copy_(x)
+    im.ex.buf[images].copy_(x)
+    g_fq = _capture(lambda: fq.forward(training=False), torch)
+    g_int = _capture(lambda: im.ex.forward(training=False), torch)
+    g_fq.replay()
+    g_int.replay()
+    torch.cuda.synchronize()
+    lf, li = fq.T(fq.logits_t).float(), im.ex.T(im.logits).float()
+    diff = float((lf - li).abs().max() / lf.abs().max().clamp_min(1e-30))
+    agree = float((lf.argmax(1) == li.argmax(1)).float().mean())
+    for _ in range(args.nb_repts_warmup):
+        g_fq.replay()
+        g_int.replay()
+    ms = {'fake_quant': [], 'integer': []}
+    for _ in range(args.nb_rounds):
+        ms['fake_quant'].append(_replay_ms(g_fq, args.nb_repts, torch))
+        ms['integer'].append(_replay_ms(g_int, args.nb_repts, torch))
+    bs = args.batch_size_eval
+    res = dict(net=args.net, resnet_size=args.resnet_size, batch=bs, config=cfg,
+               int_layers=sum(1 for _, w in im.sel if w is None), layers=len(im.sel), logits_max_rel_diff=diff,
+               top1_agreement=agree)
+    for arm, v in ms.items():
+        ips = sorted(bs / (t / 1e3) for t in v)
+        res[arm] = dict(ms_per_batch=sorted(v), images_per_s_min=ips[0], images_per_s_median=float(np.median(ips)),
+                        images_per_s_max=ips[-1])
+        print('%-10s inference forward: %.3f ms / batch of %d | images/s min %.0f median %.0f max %.0f'
+              % (arm, float(np.median(v)), bs, ips[0], float(np.median(ips)), ips[-1]))
+    print('logits: max |fake-quant - integer| / max |fake-quant| = %.3e, top-1 agreement %.4f' % (diff, agree))
+    res['gpu'] = gpu_name(torch)
+    print('gpu: ' + res['gpu'])
+    if args.json:
+        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+        with open(args.json, 'w') as f:
+            json.dump(res, f, indent=1)
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())
