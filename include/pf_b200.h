@@ -529,6 +529,21 @@ enum {
   PF_DW_WGRAD_GENERIC
 };
 int pf_dwconv_last_variant(void);
+/* u8 forward of the integer inference model (reference: learners/uniform_quantization/utils.py:92-104, 163-199, the
+ * depthwise conv of the fake-quantized weight and activation), on CUDA cores:
+ *   x->plane0 = u8 activation levels q_a [N,H,W,C], x->hdr = {scale = alpha_a / k_a, nplanes = 1} as
+ *   pf_bn_eval_levels_u8 writes them (x->plane1 = NULL; x->csum is not read);  w->plane0 = u8 weight levels q_w [R*S][C]
+ *   (the [R,S,C,1] kernel's layout), w->plane1 = NULL, w->alpha / w->beta = the weight quantizer's bucket scales ([C]
+ *   with w->per_channel = 1, else [1]), w->bits = log2(k_w + 1) in 1..8.
+ * Per output pixel and channel, S = sum_taps q_a q_w and J = sum_taps q_a are exact integers (padding taps are level 0,
+ * the value 0 of an activation whose range starts at 0), and
+ *   y = (scale * alpha_c / k_w) * S + (scale * beta_c) * J
+ * is rounded once, in fp32.  A header with nplanes != 1 makes every output NaN.  Requires pf_dwconv_u8_supported(d):
+ * k == c, C % 16 == 0 (16 channels per 128-bit load), C <= 65536, r * s <= 9, strides 1 or 2, zero padding, fewer than
+ * 2^31 input and output elements; 3 x 3 filters with equal strides run a row-blocked kernel, the rest one pixel per
+ * item. */
+int pf_dwconv_u8_supported(const pf_conv_desc* d);
+int pf_dwconv_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, float* y_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * a13 The HBM-bound layers between the convolutions (pf_nn.cu); tensors viewed as [m, c], c % 4 == 0.

@@ -544,6 +544,175 @@ dw3x3s2_dgrad_block_kernel(const float* __restrict__ dy, const float* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// u8 forward of the integer inference model (pf_dwconv_u8_fwd): activation and weights are the uniform quantizers'
+// unsigned levels, one byte each, so one 128-bit load holds 16 channels of a pixel and a thread works on 16 channels.
+// Per output, S = sum_taps q_a q_w and J = sum_taps q_a are exact integers (S <= 9 * 255^2 < 2^20, J <= 9 * 255 < 2^12)
+// and share one 32-bit accumulator, S in bits 0..19 and J in bits 20..31; the affine epilogue is the only rounding:
+//   y = fma(S, e1, J * e2),   e1 = (alpha_c * (1 / k_w)) * s_a,   e2 = beta_c * s_a,   s_a = alpha_a / k_a (header)
+// (the u8 tensor-core convolution's epilogue with weight centre 0).  A header with nplanes != 1 makes s_a NaN.
+struct DwU8Epi {
+  const float* alpha;      // weight bucket scales: [C] with per_channel, else [1]
+  const float* beta;
+  const pf_tc_act_hdr* hdr;
+  int per_channel;
+  float rk;                // 1 / (2^bits - 1)
+};
+
+constexpr int kU8Ch = 16;                 // channels per thread
+constexpr uint32_t kJOne = 1u << 20;      // J's unit in the shared accumulator
+constexpr int kU8RB = 2;                  // output rows per item of the 3 x 3 kernel
+constexpr int kU8NT = 128, kU8MinBlocks = 3;   // <= 168 registers: 12 warps per SM
+
+// the 16 (S, J) accumulators of one output pixel through the epilogue, as four streaming float4 stores
+__device__ __forceinline__ void dw_u8_store(const uint32_t (&acc)[kU8Ch], const DwU8Epi& e, float a_s, int c,
+                                            float* __restrict__ out) {
+#pragma unroll
+  for (int v = 0; v < kU8Ch / 4; ++v) {
+    float4 al, be;
+    if (e.per_channel) {
+      al = __ldg(reinterpret_cast<const float4*>(e.alpha + c + 4 * v));
+      be = __ldg(reinterpret_cast<const float4*>(e.beta + c + 4 * v));
+    } else {
+      const float a0 = __ldg(e.alpha), b0 = __ldg(e.beta);
+      al = make_float4(a0, a0, a0, a0);
+      be = make_float4(b0, b0, b0, b0);
+    }
+    const float a4[4] = {al.x, al.y, al.z, al.w}, b4[4] = {be.x, be.y, be.z, be.w};
+    float o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t t = acc[4 * v + k];
+      const float e1 = (a4[k] * e.rk) * a_s, e2 = b4[k] * a_s;
+      o[k] = fmaf((float)(t & (kJOne - 1)), e1, (float)(t >> 20) * e2);
+    }
+    pf_st_stream(out + 4 * v, make_float4(o[0], o[1], o[2], o[3]));
+  }
+}
+
+// 16 channels of three horizontally adjacent taps (a, b, c: one uint4 each) regrouped per channel: byte q of out[k] is
+// tap q of channel k (byte 3 is a copy of byte 0, for the caller to mask or multiply by a zero weight byte)
+__device__ __forceinline__ void dw_u8_taps3(const uint4& a, const uint4& b, const uint4& c, uint32_t (&out)[kU8Ch]) {
+  const uint32_t av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w}, cv[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t lo = __byte_perm(av[i], bv[i], 0x5140), hi = __byte_perm(av[i], bv[i], 0x7362);
+    out[4 * i + 0] = __byte_perm(lo, cv[i], 0x0410);
+    out[4 * i + 1] = __byte_perm(lo, cv[i], 0x0532);
+    out[4 * i + 2] = __byte_perm(hi, cv[i], 0x0610);
+    out[4 * i + 3] = __byte_perm(hi, cv[i], 0x0732);
+  }
+}
+
+// Items are (image, block of RB output rows, column, 16 channels), in a grid-stride loop whose stride is a multiple of
+// C / 16, so a thread's channels never change and its 3 x 16 packed weight words (byte q = w[r][q][c], byte 3 = 0) are
+// formed once.  An item streams the (RB - 1) * ST + 3 input rows its outputs share, row-blocked as the fp32 stride-1
+// kernel above; each row's three taps of a channel sit in one word, so one dp4a with the weights of row r adds a row's
+// three products to S, and one dp4a with 0x00010101 gives the row's level sum for J.
+template <int ST, int RB>
+__global__ void __launch_bounds__(kU8NT, kU8MinBlocks)
+dw3x3_u8_fwd_rows_kernel(const uint8_t* __restrict__ x, const uint8_t* __restrict__ w, DwU8Epi e, DwGeom g,
+                         float* __restrict__ y) {
+  const uint32_t C16 = (uint32_t)(g.C / kU8Ch), PB = (uint32_t)(g.P + RB - 1) / RB;
+  const uint32_t total = (uint32_t)g.N * PB * g.Q * C16;
+  const uint32_t lanes = (gridDim.x * kU8NT) / C16 * C16;
+  const uint32_t tid = blockIdx.x * kU8NT + threadIdx.x;
+  if (tid >= lanes) return;
+  const int c = (int)(tid % C16) * kU8Ch;
+  uint32_t wp[3][kU8Ch];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const uint8_t* wr = w + (size_t)(3 * r) * g.C + c;
+    dw_u8_taps3(__ldg(reinterpret_cast<const uint4*>(wr)), __ldg(reinterpret_cast<const uint4*>(wr + g.C)),
+                __ldg(reinterpret_cast<const uint4*>(wr + 2 * g.C)), wp[r]);
+#pragma unroll
+    for (int k = 0; k < kU8Ch; ++k) wp[r][k] &= 0x00ffffffu;
+  }
+  const float a_s = __ldg(&e.hdr->nplanes) == 1 ? __ldg(&e.hdr->scale) : __int_as_float(0x7fc00000);
+  for (uint32_t i = tid; i < total; i += lanes) {
+    const uint32_t pix = i / C16;
+    const uint32_t t1 = pix / (uint32_t)g.Q;
+    const int ow = (int)(pix - t1 * (uint32_t)g.Q);
+    const int n = (int)(t1 / PB);
+    const int oh0 = (int)(t1 - (uint32_t)n * PB) * RB;
+    const int ih0 = oh0 * ST - g.pt, iw0 = ow * ST - g.pl;
+    const uint8_t* xn = x + (size_t)n * g.H * g.W * g.C + c;
+    uint32_t acc[RB][kU8Ch];
+#pragma unroll
+    for (int j = 0; j < RB; ++j)
+#pragma unroll
+      for (int k = 0; k < kU8Ch; ++k) acc[j][k] = 0u;
+#pragma unroll
+    for (int rr = 0; rr < (RB - 1) * ST + 3; ++rr) {
+      const int ih = ih0 + rr;
+      const bool okh = ih >= 0 && ih < g.H;
+      uint4 xv[3];
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const int iw = iw0 + q;
+        const bool ok = okh && iw >= 0 && iw < g.W;
+        xv[q] = ok ? __ldg(reinterpret_cast<const uint4*>(xn + ((size_t)ih * g.W + iw) * g.C)) : make_uint4(0u, 0u, 0u, 0u);
+      }
+      uint32_t xp[kU8Ch];
+      dw_u8_taps3(xv[0], xv[1], xv[2], xp);
+#pragma unroll
+      for (int k = 0; k < kU8Ch; ++k) {
+        const uint32_t rs = __dp4a(xp[k], 0x00010101u, 0u) << 20;
+#pragma unroll
+        for (int j = 0; j < RB; ++j) {
+          const int r = rr - j * ST;
+          if (r >= 0 && r < 3) acc[j][k] = __dp4a(xp[k], wp[r][k], acc[j][k] + rs);
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < RB; ++j)
+      if (oh0 + j < g.P) dw_u8_store(acc[j], e, a_s, c, y + (((size_t)n * g.P + oh0 + j) * g.Q + ow) * g.C + c);
+  }
+}
+
+// any other filter of <= kMaxTaps taps and either stride: one output pixel x 16 channels per item, tap by tap;
+// q_a * (q_w + 2^20) adds the product to S and q_a to J in one multiply-add
+__global__ void __launch_bounds__(kU8NT, kU8MinBlocks)
+dw_u8_fwd_kernel(const uint8_t* __restrict__ x, const uint8_t* __restrict__ w, DwU8Epi e, DwGeom g,
+                 float* __restrict__ y) {
+  const uint32_t C16 = (uint32_t)(g.C / kU8Ch);
+  const uint32_t total = (uint32_t)g.N * g.P * g.Q * C16;
+  const uint32_t lanes = (gridDim.x * kU8NT) / C16 * C16;
+  const uint32_t tid = blockIdx.x * kU8NT + threadIdx.x;
+  if (tid >= lanes) return;
+  const int c = (int)(tid % C16) * kU8Ch;
+  const float a_s = __ldg(&e.hdr->nplanes) == 1 ? __ldg(&e.hdr->scale) : __int_as_float(0x7fc00000);
+  for (uint32_t i = tid; i < total; i += lanes) {
+    const uint32_t pix = i / C16;
+    const uint32_t t1 = pix / (uint32_t)g.Q;
+    const int ow = (int)(pix - t1 * (uint32_t)g.Q);
+    const int n = (int)(t1 / (uint32_t)g.P);
+    const int oh = (int)(t1 - (uint32_t)n * (uint32_t)g.P);
+    const uint8_t* xn = x + (size_t)n * g.H * g.W * g.C + c;
+    uint32_t acc[kU8Ch];
+#pragma unroll
+    for (int k = 0; k < kU8Ch; ++k) acc[k] = 0u;
+    for (int r = 0; r < g.R; ++r) {
+      const int ih = oh * g.sh - g.pt + r;
+      if (ih < 0 || ih >= g.H) continue;
+      for (int s = 0; s < g.S; ++s) {
+        const int iw = ow * g.sw - g.pl + s;
+        if (iw < 0 || iw >= g.W) continue;
+        const uint4 xv = __ldg(reinterpret_cast<const uint4*>(xn + ((size_t)ih * g.W + iw) * g.C));
+        const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w + (size_t)(r * g.S + s) * g.C + c));
+        const uint32_t xa[4] = {xv.x, xv.y, xv.z, xv.w}, wa[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+        for (int k = 0; k < kU8Ch; ++k) {
+          const uint32_t qa = (xa[k >> 2] >> (8 * (k & 3))) & 0xffu, qw = (wa[k >> 2] >> (8 * (k & 3))) & 0xffu;
+          acc[k] += qa * (qw + kJOne);
+        }
+      }
+    }
+    dw_u8_store(acc, e, a_s, c, y + (size_t)pix * g.C + c);
+  }
+}
+
 inline bool dw_rows_enabled() {           // PF_DW_ROWS=0: the one-output-per-thread kernels everywhere (read per launch)
   const char* v = getenv("PF_DW_ROWS");
   return !(v && v[0] == '0');
@@ -689,5 +858,48 @@ int pf_dwconv_wgrad(const pf_conv_desc* d, const float* x_dev, const float* dy_d
 }
 
 int pf_dwconv_last_variant(void) { return g_last_variant; }
+
+int pf_dwconv_u8_supported(const pf_conv_desc* d) {
+  if (!d || d->n <= 0 || d->h <= 0 || d->w <= 0 || d->c <= 0 || d->r <= 0 || d->s <= 0 || d->p <= 0 || d->q <= 0 ||
+      d->pad_t < 0 || d->pad_l < 0)
+    return 0;
+  return d->k == d->c && d->c % kU8Ch == 0 && d->c <= 65536 && d->r * d->s <= kMaxTaps && (d->stride_h == 1 || d->stride_h == 2) &&
+         (d->stride_w == 1 || d->stride_w == 2) && (int64_t)d->n * d->h * d->w * d->c < (1ll << 31) &&
+         (int64_t)d->n * d->p * d->q * d->c < (1ll << 31);
+}
+
+int pf_dwconv_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, float* y_dev, void* stream) {
+  const char* who = "pf_dwconv_u8_fwd";
+  PF_REQUIRE(d && x && w && x->plane0 && x->hdr && w->plane0 && w->alpha && w->beta && y_dev, "%s: null pointer", who);
+  PF_REQUIRE(x->plane1 == nullptr && w->plane1 == nullptr, "%s: u8 operands have one plane", who);
+  PF_REQUIRE(w->bits >= 1 && w->bits <= 8, "%s: u8 weight levels need 1..8 bits", who);
+  PF_REQUIRE(pf_dwconv_u8_supported(d),
+             "%s: needs depth multiplier 1, C %% 16 == 0, at most %d taps, strides 1 or 2 and < 2^31 elements", who,
+             kMaxTaps);
+  PF_REQUIRE((((uintptr_t)x->plane0 | (uintptr_t)w->plane0 | (uintptr_t)y_dev) & 15) == 0 &&
+                 (!w->per_channel || (((uintptr_t)w->alpha | (uintptr_t)w->beta) & 15) == 0) &&
+                 ((uintptr_t)x->hdr & 7) == 0,
+             "%s: 16-byte alignment required (per-channel scales: 16, header: 8)", who);
+  const DwGeom g{d->n, d->h, d->w, d->c, d->r, d->s, d->p, d->q, d->stride_h, d->stride_w, d->pad_t, d->pad_l};
+  const DwU8Epi e{w->alpha, w->beta, x->hdr, w->per_channel ? 1 : 0, 1.f / (float)((1 << w->bits) - 1)};
+  const uint8_t* xl = reinterpret_cast<const uint8_t*>(x->plane0);
+  const uint8_t* wl = reinterpret_cast<const uint8_t*>(w->plane0);
+  const int64_t c16 = g.C / kU8Ch;
+  cudaStream_t st = (cudaStream_t)stream;
+  // at least C / 16 threads take items (the grid-stride loop keeps each thread on its channels)
+  auto grid = [&](int64_t items) {
+    const int64_t want = ((items > c16 ? items : c16) + kU8NT - 1) / kU8NT, cap = (int64_t)PF_NUM_SMS * 16;
+    return (unsigned)(want < cap ? want : cap);
+  };
+  if (g.R == 3 && g.S == 3 && g.sh == g.sw && g.P >= kU8RB) {
+    const int64_t items = (int64_t)g.N * ((g.P + kU8RB - 1) / kU8RB) * g.Q * c16;
+    if (g.sh == 1) dw3x3_u8_fwd_rows_kernel<1, kU8RB><<<grid(items), kU8NT, 0, st>>>(xl, wl, e, g, y_dev);
+    else dw3x3_u8_fwd_rows_kernel<2, kU8RB><<<grid(items), kU8NT, 0, st>>>(xl, wl, e, g, y_dev);
+  } else {
+    dw_u8_fwd_kernel<<<grid((int64_t)g.N * g.P * g.Q * c16), kU8NT, 0, st>>>(xl, wl, e, g, y_dev);
+  }
+  PF_CHECK_LAUNCH(who);
+  return PF_OK;
+}
 
 }  // extern "C"

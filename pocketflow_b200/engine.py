@@ -809,6 +809,8 @@ class Executor:
                            for op in self.ops if op.type == 'FusedBatchNorm'}
         self.conv = {op: (_StemConv if op in self.im2col else _TcConv if op in self.tc else _ConvLowering)(self, op)
                      for op in self.ops if op.type in ('Conv2D', 'MatMul')}
+        # depthwise convolutions run pf_dwconv_fwd unless a lowering is registered here (int8.IntModel's u8 layers)
+        self.dwconv = {}
 
     def _plan_bn_add(self):
         """Linear bottleneck: a BatchNorm without activation whose only consumer is a residual Add (MobileNet-v2's
@@ -1088,6 +1090,9 @@ class Executor:
             if ty in ('Conv2D', 'MatMul'):
                 self.conv[op].forward()
             elif ty == 'DepthwiseConv2dNative':
+                if op in self.dwconv:
+                    self.dwconv[op].forward()
+                    continue
                 with self.timed('dwconv'):
                     ops.dwconv_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), self.buf[op.output])
             elif ty == 'FusedBatchNorm':

@@ -18,6 +18,11 @@ bits, the producer of the input and its activation bits, and the shape the u8 ke
 64).  Every other layer keeps the fake-quant inference kernels: the stem and the dense layer, first and last layers
 unless all layers are quantized, depthwise convolutions, `split` buckets.
 
+With `cfg['int8_depthwise']` (opt-in; `config_from_flags` leaves it out) the depthwise convolutions that meet the same
+conditions run on u8 levels too (pf_dwconv_u8_fwd, CUDA cores: exact window sums S = sum q_a q_w and J = sum q_a per
+channel, then the same affine epilogue), fed by the same batch norm + ReLU level producer.  Their sidecar carries
+version 2, which loaders before this option refuse.
+
     im = IntModel.from_checkpoint(graph, images, logits, state, cfg)   # the learner's checkpoint (unquantized weights)
     logits = im.forward(images_tensor)
     im.export(path)                                                    # integer checkpoint + sidecar
@@ -33,7 +38,8 @@ import numpy as np
 from . import compact
 
 F32 = np.float32
-SIDECAR_VERSION = 1
+SIDECAR_VERSION = 2          # written when depthwise layers run as integers; version 1 otherwise
+SIDECAR_VERSIONS = (1, 2)    # what load() reads
 CFG_KEYS = ('weight_bits', 'activation_bits', 'quantize_all_layers', 'use_buckets', 'bucket_type', 'bucket_size')
 
 
@@ -88,19 +94,21 @@ def _conv_desc(op):
 
 def select(graph, logits, cfg):
     """[(op name, None or the reason it keeps the fake-quant kernels)] for every Conv2D / MatMul / depthwise op in
-    graph order; None = it runs on the u8 kernel."""
+    graph order; None = it runs on a u8 kernel.  Depthwise ops are considered only with cfg['int8_depthwise']."""
     from . import ops
     mm, acts = quant_marks(graph, cfg)
     mm, acts = set(mm), set(acts)
+    depthwise = bool(cfg.get('int8_depthwise', False))
     out = []
     for op in compact.reachable_ops(graph, logits):
         if op.type not in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative'):
             continue
         x = op.inputs[0]
+        dw = op.type == 'DepthwiseConv2dNative'
         why = None
         if op not in mm:
             why = 'weights not quantized (first / last layer)'
-        elif op.type == 'DepthwiseConv2dNative':
+        elif dw and not depthwise:
             why = 'depthwise convolution'
         elif op.type == 'MatMul':
             why = 'dense layer'
@@ -114,7 +122,14 @@ def select(graph, logits, cfg):
             why = 'activation bits %d > 8' % cfg['activation_bits']
         else:
             c = x.shape[-1]
-            if c < 16 or c & (c - 1):
+            if dw and (c < 16 or c & (c - 1)):
+                why = 'input channels %d: the level producer needs a power of two >= 16' % c
+            elif dw:
+                if not ops.dwconv_u8_supported(_conv_desc(op)):
+                    (kh, kw), (sh, sw) = op.attrs['ksize'], op.attrs['strides']
+                    why = 'depthwise %dx%d stride %dx%d over %d channels (the u8 depthwise kernel needs C %% 16 == 0, ' \
+                          '<= 9 taps, strides 1 or 2)' % (kh, kw, sh, sw, c)
+            elif c < 16 or c & (c - 1):
                 why = 'input channels %d not a power of two' % c
             elif not ops.conv2d_u8_supported(_conv_desc(op)):
                 why = 'shape %d -> %d channels (the u8 kernel needs multiples of 64)' % (c, op.output.shape[-1])
@@ -124,7 +139,11 @@ def select(graph, logits, cfg):
 
 def report_lines(sel):
     """What tools/export_uq_int8.py prints: one line per layer."""
-    lines = ['%s: %s' % (name, 'u8 x u8 tensor cores' if why is None else 'fake-quant (%s)' % why) for name, why in sel]
+    def path(name, why):
+        if why is not None:
+            return 'fake-quant (%s)' % why
+        return 'u8 depthwise (CUDA cores)' if name.rsplit('/', 1)[-1] == 'depthwise' else 'u8 x u8 tensor cores'
+    lines = ['%s: %s' % (name, path(name, why)) for name, why in sel]
     n = sum(1 for _, why in sel if why is None)
     lines.append('%d of %d layers run as integers' % (n, len(sel)))
     return lines
@@ -213,6 +232,27 @@ class _U8Conv:
                               self.bits, ex.buf[op.output], bias, op in ex.fused_act, res, self.bn_out)
 
 
+class _U8DwConv:
+    """A depthwise convolution on pf_dwconv_u8_fwd, from the levels of its input's producer and its own weight levels
+    (registered in the executor's `dwconv` table, which its forward consults before pf_dwconv_fwd)."""
+
+    def __init__(self, ex, op, bn, levels, alpha, beta, bits):
+        import torch
+        self.ex, self.op, self.bn, self.bits = ex, op, bn, bits
+        self.d = ex.desc[op]
+        dev = ex.device
+        self.wl = torch.from_numpy(np.ascontiguousarray(levels.reshape(-1, levels.shape[-2]))).to(dev)   # [R*S, C]
+        self.alpha = torch.from_numpy(np.ascontiguousarray(alpha, F32)).to(dev)
+        self.beta = torch.from_numpy(np.ascontiguousarray(beta, F32)).to(dev)
+
+    def forward(self):
+        from . import ops
+        ex = self.ex
+        with ex.timed('dwconv'):
+            ops.dwconv_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.wl, self.alpha, self.beta, self.bits,
+                              ex.buf[self.op.output])
+
+
 class IntModel:
     """A uniformly quantized model whose eligible convolutions run on the u8 tensor cores (engine.Executor in inference
     mode, with those convolutions and the batch norms feeding them lowered to the u8 kernels)."""
@@ -243,14 +283,22 @@ class IntModel:
             op = byname[name]
             u8_readers.setdefault(ex._root(op.inputs[0]).op, []).append(op)
         for bn, readers in u8_readers.items():
-            fp_readers = [c for c in ex.ops if c in ex.tc and c not in readers and ex.planes_of(c.inputs[0]) is not None
-                          and ex._root(c.inputs[0]).op is bn]
-            others = ex.bn_need_f32.get(bn, True) or bool(fp_readers)
+            if bn in ex.xplanes:     # it writes operand planes: other planes readers, or fp32 readers the plan found
+                fp_readers = [c for c in ex.ops if c in ex.tc and c not in readers
+                              and ex.planes_of(c.inputs[0]) is not None and ex._root(c.inputs[0]).op is bn]
+                others = ex.bn_need_f32[bn] or bool(fp_readers)
+            else:                    # fp32 only (it feeds depthwise layers): does anything but the u8 layers read it?
+                ts = [bn.output] + [c.output for c in ex._consumers(bn.output) if ex.fused_into.get(c) is bn]
+                others = any(c not in readers and ex.fused_into.get(c) is not bn for t in ts for c in ex._consumers(t))
             ex.batch_norm[bn] = _U8Bn(ex, bn, ex.batch_norm[bn], others)
         for name in ints:
             op = byname[name]
             lv, al, be = wlevels[name]
-            ex.conv[op] = _U8Conv(ex, op, ex.batch_norm[ex._root(op.inputs[0]).op], lv, al, be, bits)
+            bn = ex.batch_norm[ex._root(op.inputs[0]).op]
+            if op.type == 'DepthwiseConv2dNative':
+                ex.dwconv[op] = _U8DwConv(ex, op, bn, lv, al, be, bits)
+            else:
+                ex.conv[op] = _U8Conv(ex, op, bn, lv, al, be, bits)
 
     @classmethod
     def from_checkpoint(cls, graph, images, logits, state, cfg, device=None):
@@ -285,8 +333,9 @@ class IntModel:
             arrays[(k + '/beta').replace('/', '|')] = be
         fn = path + '.npz'
         np.savez(fn, **arrays)
+        version = SIDECAR_VERSION if any(byname[n].type == 'DepthwiseConv2dNative' for n in self.wlevels) else 1
         with open(path + '.int8.json', 'w') as f:
-            json.dump(dict(version=SIDECAR_VERSION, config=self.cfg, layers=[[n, w] for n, w in self.sel]), f)
+            json.dump(dict(version=version, config=self.cfg, layers=[[n, w] for n, w in self.sel]), f)
         return fn
 
     @classmethod
@@ -294,9 +343,12 @@ class IntModel:
         """Rebuild the integer model from what export(path) wrote."""
         with open(path + '.int8.json') as f:
             rec = json.load(f)
-        if rec.get('version') != SIDECAR_VERSION:
-            raise ValueError('%s.int8.json: unsupported sidecar version %r' % (path, rec.get('version')))
+        if rec.get('version') not in SIDECAR_VERSIONS:
+            raise ValueError('%s.int8.json: unsupported sidecar version %r (this loader reads %s)'
+                             % (path, rec.get('version'), ', '.join(map(str, SIDECAR_VERSIONS))))
         cfg = {k: rec['config'][k] for k in CFG_KEYS}
+        if rec['config'].get('int8_depthwise'):
+            cfg['int8_depthwise'] = True
         d = np.load(path + '.npz')
         arrays = {k.replace('|', '/'): d[k] for k in d.files}
         byname = {op.name: op for op in compact.reachable_ops(graph, logits)}

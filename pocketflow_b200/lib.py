@@ -83,6 +83,8 @@ SIGNATURES = {
     'pf_dwconv_wgrad_workspace_bytes': (c_i64, [c_vp]),
     'pf_dwconv_wgrad': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_dwconv_last_variant': (c_i32, []),
+    'pf_dwconv_u8_supported': (c_i32, [c_vp]),
+    'pf_dwconv_u8_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_train_stats': (c_i32, [c_vp, c_i64, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_eval_prepare': (c_i32, [c_vp, c_i32, c_f32, c_vp, c_vp]),
     'pf_bn_apply': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),

@@ -1245,6 +1245,24 @@ def dwconv_last_variant():
     return DW_VARIANTS[v - 1] if v else None
 
 
+def dwconv_u8_supported(d):
+    """the shapes pf_dwconv_u8_fwd runs: depth multiplier 1, C % 16 == 0, <= 9 taps, strides 1 or 2"""
+    return bool(_lib.load().pf_dwconv_u8_supported(ctypes.byref(d)))
+
+
+def dwconv_u8_fwd(d, x_levels, hdr, w_levels, alpha, beta, bits, y):
+    """y = the fake-quantized depthwise conv from u8 levels (pf_dwconv_u8_fwd): x_levels uint8 [N, H, W, C] with its
+    header (bn_eval_levels_u8), w_levels uint8 [R*S, C], alpha / beta the weight bucket scales ([1] per layer or [C]
+    per channel)"""
+    if x_levels.dtype != torch.uint8 or w_levels.dtype != torch.uint8:
+        raise ValueError('dwconv_u8_fwd: the levels are uint8 tensors')
+    _check_f32(alpha, beta, y)
+    act = _lib.TcAct(x_levels.data_ptr(), 0, hdr.data_ptr(), 0, 0, 0)
+    wt = _lib.TcWt(w_levels.data_ptr(), 0, alpha.data_ptr(), beta.data_ptr(), int(alpha.numel() > 1), int(bits))
+    _lib.check(_lib.load().pf_dwconv_u8_fwd(ctypes.byref(d), ctypes.byref(act), ctypes.byref(wt), _p(y), _stream()),
+               'pf_dwconv_u8_fwd')
+
+
 def preprocess_images(crops_u8, desc, out, mean=(123.68, 116.78, 103.94)):
     """ILSVRC-12 preprocessing of a packed mini-batch on the device (pf_preprocess_images): crops_u8 = uint8 CUDA buffer
     holding every decoded crop back to back, desc = uint8 CUDA view of n pf_img_desc records

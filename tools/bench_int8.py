@@ -7,6 +7,10 @@ both on the inputs a forward of the seed-initialised model left in their buffers
 u8 kernel's lower bound: the larger of the FLOP bound (2 M N K at the u8 data-sheet rate, 1,979 dense TOPS) and the byte
 bound (u8 operands read once, fp32 output written once, at 3.35 TB/s).
 
+The integer model is built with its depthwise layers on u8 levels too (cfg['int8_depthwise']): each is timed the same
+way against pf_dwconv_fwd on the fake-quant model's fp32 input, with the byte bound of each (u8: 1 B read per input
+element, 4 B written per output; fp32: 4 B and 4 B) and the u8 kernel's share of its own.
+
     python tools/bench_int8.py --net resnet_at_ilsvrc12 --resnet_size 50 --batch_size_eval 128 --json out.json
 """
 import argparse
@@ -54,6 +58,7 @@ def main(argv=None):
     for k, v in dict(uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel',
                      uql_bucket_size=256, uql_quantize_all_layers=False).items():
         setattr(args, k, v)
+    args.int8_depthwise = True
     graph, images, logits, cfg = setup(args)
     state = load_state(args, graph, logits)
     dev = torch.device('cuda', 0)
@@ -86,8 +91,28 @@ def main(argv=None):
               % (op.name, m, n, k, t_u8, t_fq, bound, rows[-1]['bound_by'], 100 * bound / t_u8))
     print('all %d u8 layers: u8 %.3f ms, fake-quant %.3f ms, bound %.3f ms' % (len(rows), tot['u8'], tot['fq'],
                                                                               tot['bound']))
+    from pocketflow_b200 import ops
+    dw_rows, dw_tot = [], dict(u8=0.0, fp32=0.0, bound=0.0, fp32_bound=0.0)
+    for op, lo in im.ex.dwconv.items():
+        d = lo.d
+        nin, nout = d.n * d.h * d.w * d.c, d.n * d.p * d.q * d.c
+        bound = (nin + d.r * d.s * d.c + 4 * nout) / HBM_BYTES_PER_S * 1e3
+        bound32 = (4 * nin + 4 * d.r * d.s * d.c + 4 * nout) / HBM_BYTES_PER_S * 1e3
+        x32, w32, y32 = fq.T(op.inputs[0]), fq.kernel_of(op), fq.buf[op.output]
+        t_u8 = _ms(lo.forward, args.launches, torch)
+        t_32 = _ms(lambda: ops.dwconv_fwd(d, x32, w32, y32), args.launches, torch)
+        dw_rows.append(dict(op=op.name, h=d.h, w=d.w, c=d.c, stride=d.stride_h, u8_ms=t_u8, fp32_ms=t_32,
+                            bound_ms=bound, fp32_bound_ms=bound32, u8_share_of_bound=bound / t_u8,
+                            fp32_share_of_bound=bound32 / t_32))
+        for key, v in (('u8', t_u8), ('fp32', t_32), ('bound', bound), ('fp32_bound', bound32)):
+            dw_tot[key] += v
+        print('%-48s %4dx%-4d C %4d s%d | u8 %.4f ms (%.0f %% of its byte bound)  fp32 %.4f ms (%.0f %%)'
+              % (op.name, d.h, d.w, d.c, d.stride_h, t_u8, 100 * bound / t_u8, t_32, 100 * bound32 / t_32))
+    if dw_rows:
+        print('all %d u8 depthwise layers: u8 %.3f ms (bound %.3f), pf_dwconv_fwd %.3f ms (bound %.3f)'
+              % (len(dw_rows), dw_tot['u8'], dw_tot['bound'], dw_tot['fp32'], dw_tot['fp32_bound']))
     res = dict(net=args.net, resnet_size=args.resnet_size, batch=args.batch_size_eval, layers=rows, totals=tot,
-               gpu=gpu_name(torch))
+               depthwise=dw_rows, depthwise_totals=dw_tot, gpu=gpu_name(torch))
     print('gpu: ' + res['gpu'])
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

@@ -39,10 +39,12 @@ def parse(argv=None):
     p.add_argument('--uql_bucket_type', default='channel', choices=('channel', 'split'))
     p.add_argument('--uql_bucket_size', type=int, default=256)
     p.add_argument('--uql_quantize_all_layers', action='store_true')
+    p.add_argument('--int8_depthwise', action='store_true',
+                   help='depthwise layers on u8 levels too (pf_dwconv_u8_fwd); also times the integer model without them')
     p.add_argument('--batch_size_eval', type=int, default=100)
     p.add_argument('--nb_repts_warmup', type=int, default=20, help='graph replays before timing')
     p.add_argument('--nb_repts', type=int, default=50, help='graph replays per timed window')
-    p.add_argument('--nb_rounds', type=int, default=5, help='alternating (fake-quant, integer) timed windows')
+    p.add_argument('--nb_rounds', type=int, default=5, help='alternating (fake-quant, integer[, ...]) timed windows')
     p.add_argument('--no_time', action='store_true', help='export only')
     p.add_argument('--json', default=None, help='write the measurements here')
     return p.parse_args(argv)
@@ -64,7 +66,10 @@ def setup(args):
               'uql_quantize_all_layers'):
         setattr(FLAGS, k, getattr(args, k))
     graph, images, logits = compact.build_eval_graph(net.ModelHelper(), args.batch_size_eval)
-    return graph, images, logits, int8.config_from_flags()
+    cfg = int8.config_from_flags()
+    if getattr(args, 'int8_depthwise', False):
+        cfg['int8_depthwise'] = True
+    return graph, images, logits, cfg
 
 
 def load_state(args, graph, logits):
@@ -110,21 +115,26 @@ def main(argv=None):
     x = torch.randn(images.shape, generator=torch.Generator().manual_seed(0)).to(dev)
     fq.buf[images].copy_(x)
     im.ex.buf[images].copy_(x)
-    g_fq = _capture(lambda: fq.forward(training=False), torch)
-    g_int = _capture(lambda: im.ex.forward(training=False), torch)
-    g_fq.replay()
-    g_int.replay()
+    arms = {'fake_quant': fq, 'integer': im.ex}
+    if cfg.get('int8_depthwise'):             # the same integer model with its depthwise layers on the fake-quant path
+        nodw = {k: v for k, v in cfg.items() if k != 'int8_depthwise'}
+        im_nodw = int8.IntModel.from_checkpoint(graph, images, logits, state, nodw, dev)
+        im_nodw.ex.buf[images].copy_(x)
+        arms = {'fake_quant': fq, 'integer_no_depthwise': im_nodw.ex, 'integer': im.ex}
+    graphs = {arm: _capture(lambda ex=ex: ex.forward(training=False), torch) for arm, ex in arms.items()}
+    for gr in graphs.values():
+        gr.replay()
     torch.cuda.synchronize()
     lf, li = fq.T(fq.logits_t).float(), im.ex.T(im.logits).float()
     diff = float((lf - li).abs().max() / lf.abs().max().clamp_min(1e-30))
     agree = float((lf.argmax(1) == li.argmax(1)).float().mean())
     for _ in range(args.nb_repts_warmup):
-        g_fq.replay()
-        g_int.replay()
-    ms = {'fake_quant': [], 'integer': []}
+        for gr in graphs.values():
+            gr.replay()
+    ms = {arm: [] for arm in graphs}
     for _ in range(args.nb_rounds):
-        ms['fake_quant'].append(_replay_ms(g_fq, args.nb_repts, torch))
-        ms['integer'].append(_replay_ms(g_int, args.nb_repts, torch))
+        for arm, gr in graphs.items():
+            ms[arm].append(_replay_ms(gr, args.nb_repts, torch))
     bs = args.batch_size_eval
     res = dict(net=args.net, resnet_size=args.resnet_size, batch=bs, config=cfg,
                int_layers=sum(1 for _, w in im.sel if w is None), layers=len(im.sel), logits_max_rel_diff=diff,
@@ -133,7 +143,7 @@ def main(argv=None):
         ips = sorted(bs / (t / 1e3) for t in v)
         res[arm] = dict(ms_per_batch=sorted(v), images_per_s_min=ips[0], images_per_s_median=float(np.median(ips)),
                         images_per_s_max=ips[-1])
-        print('%-10s inference forward: %.3f ms / batch of %d | images/s min %.0f median %.0f max %.0f'
+        print('%-20s inference forward: %.3f ms / batch of %d | images/s min %.0f median %.0f max %.0f'
               % (arm, float(np.median(v)), bs, ips[0], float(np.median(ips)), ips[-1]))
     print('logits: max |fake-quant - integer| / max |fake-quant| = %.3e, top-1 agreement %.4f' % (diff, agree))
     res['gpu'] = gpu_name(torch)
