@@ -456,9 +456,12 @@ int pf_conv2d_tc_wgrad_ex(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc
  *   y[m,n] = (scale * alpha_n / k_w) * S[m,n] + (scale * beta_n) * J[m],   J[m] = sum_K q_a (from csum),
  * rounding only there, then bias, ReLU (relu != 0), the residual (residual_dev) and, with bn != NULL, the folded inference
  * batch norm as pf_conv2d_tc_fwd_bn applies it.  A header with nplanes != 1 (the activation's minimum was not 0, so
- * its values are not scale * level) makes every output NaN.  Requires pf_conv2d_u8_supported(d): Cin % 64 == 0,
- * Cout % 64 == 0, strides <= 8, filters <= 16 x 16; there is no other kernel for u8 operands. */
+ * its values are not scale * level) makes every output NaN.  The shape picks the kernel: where
+ * pf_conv2d_u8_supported(d) holds (Cin % 64 == 0, Cout % 64 == 0, strides <= 8, filters <= 16 x 16) the TMA-fed one,
+ * otherwise a cp.async-fed one (pf_conv_tc.cu) with the same arithmetic, which needs Cin % 16 == 0, Cout % 16 == 0 and
+ * R*S*Cin <= 32768; pf_conv2d_u8_narrow_supported(d) tells whether either kernel takes d. */
 int pf_conv2d_u8_supported(const pf_conv_desc* d);
+int pf_conv2d_u8_narrow_supported(const pf_conv_desc* d);
 int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, const float* bias_dev, int relu,
                      const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn, void* stream);
 /* producer of the u8 operand (reference: utils/external/resnet_model.py:55-62 inference BN, then
@@ -466,7 +469,9 @@ int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* 
  * (pf_bn_apply_eval's op chain), quantized per tensor, written as levels rint(((y - min) / alpha) * k) into levels_dev
  * (m * c bytes) + hdr + csum (m * ceil(c / 128) floats).  have_range = 0: range_enc_dev[0..1] is reset and filled with
  * min / max of y first (a pass of its own: the whole range is needed before any level); 1: it already holds them (a
- * pf_bn_apply_eval of the same x with minmax_enc_dev = range_enc_dev).  C a power of two >= 16, bits 1..8. */
+ * pf_bn_apply_eval of the same x with minmax_enc_dev = range_enc_dev).  C a multiple of 16 (a power of two, or not:
+ * each runs a kernel of its own, with the same levels and sums), bits 1..8.  x and the four per-channel vectors
+ * 16-byte aligned, levels_dev and hdr_dev 8-byte aligned. */
 int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
                          float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
                          uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,

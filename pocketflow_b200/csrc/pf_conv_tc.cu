@@ -774,6 +774,249 @@ int launch_tc(const TcGeom& g, const float* src, const void* a_hi, const void* a
   return launch_persist<MODE>(g, p, src, a_hi, a_lo, b_hi, b_lo, out, bias, residual, st, who, bn);
 }
 
+// ---------------------------------------------------------------------------------------------
+// u8 forward for the shapes the TMA-fed u8 kernel does not take (Cin or Cout a multiple of 16 but not of 64): both
+// operands are the quantizers' unsigned 8-bit levels (pf_conv2d_u8_fwd), activations [N, H, W, Cin], weights
+// [Cout][R*S*Cin].  The structure is conv_tc_persist_kernel's with pre-made operands: warps 8-15 copy each k-stage with
+// cp.async straight into 128B-swizzled tiles (one 16-byte chunk = 16 channels of one filter tap, so any Cin % 16 == 0
+// decodes per chunk; chunks past R*S*Cin are zero-filled), warps 0-7 are two m64 warpgroups.  A k-stage is 128 levels
+// per row, i.e. four k32 slices at the 32-byte steps the bf16 kernel's k16 slices take; each slice is one
+// u8 x u8 -> s32 wgmma, so S = sum q_a q_w is exact.  The epilogue is the TMA u8 kernel's: AFF 2 with weight centre 0
+// (the rank-1 term from the channel sums J), bias, ReLU, residual and optionally the folded inference batch norm.
+constexpr int BKU = 128;                         // u8 levels per k-stage and row
+struct U8P {
+  TcGeom g;
+  int M, Ng, Kdim, nk, n_stages, n_tiles, total_tiles, relu, nseg;
+  FastDiv d_hw, d_w, d_c, d_s, d_ntiles;
+  EpiAff aff;
+  const pf_tc_act_hdr* hdr;
+  const float* csum;
+};
+
+// J of one GEMM row: the sum of the stored activation levels under the row's filter window (origin
+// (oh0, ow0), R x S taps) from the per-pixel channel-segment sums `cimg` of the row's image (src_h x src_w pixels x
+// nseg).  The (tap, segment) terms are independent loads, issued four at a time (branch-free; the terms are integers
+// below 2^24, so the order of the additions does not change the result).  The TMA-fed u8 kernel forms the same sum in
+// its consumer.
+__device__ __forceinline__ float window_level_sum(const float* __restrict__ cimg, int nseg, int R, int S, FastDiv d_s,
+                                                  int src_h, int src_w, int oh0, int ow0) {
+  const int total = R * S * nseg;
+  auto term = [&](int u) -> float {
+    if (u >= total) return 0.f;
+    const int t = u / nseg, g = u - t * nseg;
+    const int r = (int)fdiv((uint32_t)t, d_s), s_ = t - r * S;
+    const int ih = oh0 + r, iw = ow0 + s_;
+    const bool ok = (unsigned)ih < (unsigned)src_h && (unsigned)iw < (unsigned)src_w;
+    return ok ? __ldg(cimg + ((size_t)ih * src_w + iw) * nseg + g) : 0.f;
+  };
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+  for (int u = 0; u < total; u += 4) {
+    const float v0 = term(u), v1 = term(u + 1), v2 = term(u + 2), v3 = term(u + 3);
+    a0 += v0; a1 += v1; a2 += v2; a3 += v3;
+  }
+  return (a0 + a1) + (a2 + a3);
+}
+
+template <int BN, bool BNO>
+__global__ void __launch_bounds__(kThreadsP, 1)
+conv_u8_persist_kernel(const uint8_t* __restrict__ a_g, const uint8_t* __restrict__ b_g, float* __restrict__ out,
+                       const float* __restrict__ bias, const float* __restrict__ residual,
+                       const __grid_constant__ U8P p, const __grid_constant__ pf_tc_bn_out bn) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  const TcGeom& g = p.g;
+  constexpr uint32_t a_bytes = TM * BKU, b_bytes = (uint32_t)BN * BKU, stage_bytes = a_bytes + b_bytes;
+  float* acc_s = reinterpret_cast<float*>(smem + (size_t)p.n_stages * stage_bytes);
+  long long* rowoff_all = reinterpret_cast<long long*>(acc_s + TM * acc_pitch(BN));
+  float* jrow_all = reinterpret_cast<float*>(rowoff_all + kMmaWarps * 32);
+  float* aff_tab = jrow_all + kMmaWarps * 32;    // e1 at c, e2 at 256 + c; BNO: bn_table at 512
+  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int s = 0; s < p.n_stages; ++s) {
+      mbar_init(&full_bar[s], kProdWarps * 32);
+      mbar_init(&empty_bar[s], kMmaWarps);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const int first_tile = blockIdx.x, tile_step = gridDim.x;
+
+  if (warp >= kMmaWarps) {
+    // ============ producers: thread = 16-byte chunk l8 of rows rgrp + 32 i (A) and rgrp + 32 j < BN (B) ============
+    const int pt_ = tid - kMmaWarps * 32;
+    const int l8 = pt_ & 7, rgrp = pt_ >> 3;
+    const uint32_t chunk_off = (((uint32_t)l8) ^ (uint32_t)(rgrp & 7)) << 4;
+    uint32_t it = 0;
+    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
+      const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
+      const int n0 = (tile - mt * p.n_tiles) * BN;
+      // this thread's rows of A: (image, window origin), or -1 past the last row
+      int img[4], oh[4], ow[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int m = mt * TM + rgrp + 32 * i;
+        img[i] = -1;
+        if (m < p.M) {
+          img[i] = (int)fdiv((uint32_t)m, p.d_hw);
+          const int rem = m - img[i] * g.P * g.Q;
+          const int y = (int)fdiv((uint32_t)rem, p.d_w);
+          oh[i] = y * g.sh - g.pt;
+          ow[i] = (rem - y * g.Q) * g.sw - g.pl;
+        }
+      }
+      for (int ks = 0; ks < p.nk; ++ks, ++it) {
+        const uint32_t s = it % (uint32_t)p.n_stages;
+        mbar_wait(&empty_bar[s], ((it / (uint32_t)p.n_stages) & 1u) ^ 1u);
+        const int kk = ks * BKU + l8 * 16;
+        const bool kok = kk < p.Kdim;
+        const int tap = (int)fdiv((uint32_t)kk, p.d_c), c = kk - tap * g.C;
+        const int r = (int)fdiv((uint32_t)tap, p.d_s), q = tap - r * g.S;
+        const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes), sb = sa + a_bytes;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int ih = oh[i] + r, iw = ow[i] + q;
+          const bool ok = kok && img[i] >= 0 && (unsigned)ih < (unsigned)g.H && (unsigned)iw < (unsigned)g.W;
+          const size_t o = ok ? (((size_t)img[i] * g.H + ih) * g.W + iw) * g.C + c : 0;
+          const uint32_t dst = sa + (uint32_t)(rgrp + 32 * i) * BKU + chunk_off;
+          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(a_g + o), "r"(ok ? 16u : 0u) : "memory");
+        }
+        for (int br = rgrp; br < BN; br += 32) {
+          const bool ok = kok && n0 + br < p.Ng;
+          const size_t o = ok ? (size_t)(n0 + br) * p.Kdim + kk : 0;
+          const uint32_t dst = sb + (uint32_t)br * BKU + chunk_off;
+          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(b_g + o), "r"(ok ? 16u : 0u) : "memory");
+        }
+        // the barrier arrival fires when every cp.async issued so far by this thread has landed
+        asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[s])) : "memory");
+      }
+    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+  } else {
+    // ============================ MMA warpgroups + epilogue (warps 0-7) ============================
+    const int wg = warp >> 2;
+    long long* rowoff = rowoff_all + warp * 32;
+    float* jrow = jrow_all + warp * 32;
+    // u8 levels stand for scale * level only when the tensor's minimum is 0 (header: 1 plane); otherwise the output
+    // is NaN rather than silently wrong
+    float a_s = __ldg(&p.hdr->scale);
+    if (__ldg(&p.hdr->nplanes) != 1) a_s = __int_as_float(0x7fc00000);
+    uint32_t it = 0;
+    for (int tile = first_tile; tile < p.total_tiles; tile += tile_step) {
+      const int mt = (int)fdiv((uint32_t)tile, p.d_ntiles);
+      const int n0 = (tile - mt * p.n_tiles) * BN;
+      int acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < p.nk; ++ks, ++it) {
+        const uint32_t s = it % (uint32_t)p.n_stages;
+        mbar_wait(&full_bar[s], (it / (uint32_t)p.n_stages) & 1u);
+        fence_proxy_async_smem();              // cp.async writes -> visible to the tensor core (async proxy)
+        const uint32_t base = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t a0 = base + (uint32_t)wg * 64 * BKU, b0 = base + a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BKU / 32; ++kk)
+          WgmmaU8<BN>::mma(acc, make_smem_desc(a0 + kk * 32, 16, 1024), make_smem_desc(b0 + kk * 32, 16, 1024));
+        wgmma_commit();
+        wgmma_wait<1>(acc);                    // the previous stage's MMAs have completed: release it
+        if (ks > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = s;
+      }
+      wgmma_wait<0>(acc);
+      if (p.nk > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      const int m = mt * TM + (warp & 3) * 32 + lane;
+      long long off = -1;
+      float my_j = 0.f;
+      if (m < p.M) {
+        off = (long long)m * p.Ng;
+        const int im = (int)fdiv((uint32_t)m, p.d_hw);
+        const int rem = m - im * g.P * g.Q;
+        const int y = (int)fdiv((uint32_t)rem, p.d_w), x = rem - y * g.Q;
+        my_j = window_level_sum(p.csum + (size_t)im * g.H * g.W * p.nseg, p.nseg, g.R, g.S, p.d_s, g.H, g.W,
+                                y * g.sh - g.pt, x * g.sw - g.pl);
+      }
+      // the accumulator tile and the columns' constants (e1 = s_a alpha_c / k_w, e2 = s_a beta_c; weight centre 0)
+      named_bar_sync(1, kMmaWarps * 32);
+      wgmma_store_acc<BN>(acc, acc_s, acc_pitch(BN), 64 * wg, tid & 127);
+      for (int c = tid; c < BN; c += kMmaWarps * 32) {
+        const bool cok = n0 + c < p.Ng;
+        const int bi = p.aff.per_channel ? n0 + c : 0;
+        const float al = cok ? __ldg(p.aff.w_alpha + bi) : 0.f, be = cok ? __ldg(p.aff.w_beta + bi) : 0.f;
+        aff_tab[c] = al * p.aff.w_rk * a_s;
+        aff_tab[256 + c] = be * a_s;
+      }
+      if (BNO) bn_table(bn, aff_tab + 512, n0, BN, p.Ng, tid, kMmaWarps * 32);
+      named_bar_sync(1, kMmaWarps * 32);
+      epilogue_tile_a<2, BNO>(acc_s, warp, off, rowoff, out, residual, bias, p.relu, n0, BN, p.Ng, lane, nullptr, p.aff,
+                              my_j, jrow, bn, aff_tab);
+    }
+  }
+}
+
+int launch_u8(const TcGeom& g, const pf_tc_act& a, const pf_tc_wt& w, float* out, const float* bias, int relu,
+              const float* residual, const pf_tc_bn_out* bn, cudaStream_t st, const char* who) {
+  const int64_t M64 = (int64_t)g.N * g.P * g.Q;
+  PF_REQUIRE(M64 < (1ll << 31), "%s: too many rows", who);
+  U8P p;
+  memset(&p, 0, sizeof(p));
+  p.g = g;
+  p.M = (int)M64;
+  p.Ng = g.K;
+  p.Kdim = g.R * g.S * g.C;
+  p.nk = (p.Kdim + BKU - 1) / BKU;
+  p.relu = relu;
+  p.nseg = a.nseg;
+  p.d_hw = make_fastdiv((uint32_t)(g.P * g.Q));
+  p.d_w = make_fastdiv((uint32_t)g.Q);
+  p.d_c = make_fastdiv((uint32_t)g.C);
+  p.d_s = make_fastdiv((uint32_t)g.S);
+  p.aff.w_alpha = w.alpha;
+  p.aff.w_beta = w.beta;
+  p.aff.per_channel = w.per_channel;
+  p.aff.w_rk = 1.f / (float)((1 << w.bits) - 1);
+  p.aff.w_centre = 0.f;
+  p.hdr = a.hdr;
+  p.csum = a.csum;
+  // tile width: the widest the accumulators allow; the folded batch norm's epilogue does not fit the registers of this
+  // 512-thread kernel beside a 128-wide tile (as in launch_persist)
+  int BN = g.K >= 128 ? 128 : (g.K >= 64 ? 64 : (g.K >= 32 ? 32 : 16));
+  if (bn && BN > 64) BN = 64;
+  p.n_tiles = (g.K + BN - 1) / BN;
+  p.total_tiles = (int)((M64 + TM - 1) / TM) * p.n_tiles;
+  p.d_ntiles = make_fastdiv((uint32_t)p.n_tiles);
+  const int stage = (TM + BN) * BKU;
+  const int fixed = epi_fixed_bytes(BN) + (512 + 4 * kMaxBN) * 4;   // + e1 / e2 and the batch norm's constants
+  p.n_stages = std::min(kMaxStages, (kSmemLimit - fixed) / stage);
+  PF_REQUIRE(p.n_stages >= 2, "%s: shared-memory plan failed (BN %d)", who, BN);
+  const size_t smem = (size_t)p.n_stages * stage + fixed;
+  const int grid = std::min(p.total_tiles, PF_NUM_SMS);
+  record_plan(pf_tc_plan{0, 0, 0, 0, BN, 2, 1, 1, 0, 0, 0, p.n_stages, p.total_tiles, grid, 0, 0});
+  if (p.total_tiles == 0) return PF_OK;
+  pf_tc_bn_out bn_p{};
+  if (bn) bn_p = *bn;
+  cudaError_t err = cudaSuccess;
+  with_bn(BN, [&](auto bn_c) {
+    constexpr int B = decltype(bn_c)::value;
+    auto kern = conv_u8_persist_kernel<B, false>;
+    if constexpr (B <= 64)
+      if (bn) kern = conv_u8_persist_kernel<B, true>;
+    err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess)
+      kern<<<grid, kThreadsP, smem, st>>>((const uint8_t*)a.plane0, (const uint8_t*)w.plane0, out, bias, residual, p, bn_p);
+  });
+  PF_CUDA(err);
+  PF_CHECK_LAUNCH(who);
+  return PF_OK;
+}
+
 // multi-tensor split-K reduction: the partials of every wgrad of a step in ONE launch (kind-0 work items)
 __global__ void __launch_bounds__(256)
 tc_splitk_reduce_multi_kernel(const pf_tc_reduce_seg* __restrict__ segs, const pf_work* __restrict__ work) {
@@ -869,6 +1112,16 @@ int pf_conv2d_tc_prep_weights_multi(const pf_tc_prep_seg* segs_dev, const pf_wor
   return PF_OK;
 }
 
+static int check_bn_out(const pf_tc_bn_out* bn, const char* who) {
+  PF_REQUIRE(bn->mean && bn->var && bn->gamma && bn->beta && (bn->y || bn->hi), "%s: batch norm: null pointer", who);
+  PF_REQUIRE((bn->hi == nullptr) == (bn->lo == nullptr), "%s: batch norm: planes come in pairs", who);
+  PF_REQUIRE(bn->eps >= 0.f && bn->act >= 0 && bn->act <= 2, "%s: batch norm: eps < 0 or act not in 0..2", who);
+  PF_REQUIRE((((uintptr_t)bn->mean | (uintptr_t)bn->var | (uintptr_t)bn->gamma | (uintptr_t)bn->beta |
+               (uintptr_t)bn->y) & 15) == 0 && (((uintptr_t)bn->hi | (uintptr_t)bn->lo) & 7) == 0,
+             "%s: batch norm: alignment", who);
+  return PF_OK;
+}
+
 static int tc_fwd_impl(const pf_conv_desc* d, const float* x_dev, const void* x_hi, const void* x_lo, const void* w_hi_dev,
                        const void* w_lo_dev, const float* bias_dev, int relu, const float* residual_dev, float* y_dev,
                        void* stream, const char* who, const pf_tc_bn_out* bn = nullptr) {
@@ -881,12 +1134,8 @@ static int tc_fwd_impl(const pf_conv_desc* d, const float* x_dev, const void* x_
                (uintptr_t)w_lo_dev | (uintptr_t)residual_dev | (uintptr_t)bias_dev) & 15) == 0,
              "%s: 16-byte alignment required", who);
   if (bn) {
-    PF_REQUIRE(bn->mean && bn->var && bn->gamma && bn->beta && (bn->y || bn->hi), "%s: batch norm: null pointer", who);
-    PF_REQUIRE((bn->hi == nullptr) == (bn->lo == nullptr), "%s: batch norm: planes come in pairs", who);
-    PF_REQUIRE(bn->eps >= 0.f && bn->act >= 0 && bn->act <= 2, "%s: batch norm: eps < 0 or act not in 0..2", who);
-    PF_REQUIRE((((uintptr_t)bn->mean | (uintptr_t)bn->var | (uintptr_t)bn->gamma | (uintptr_t)bn->beta |
-                 (uintptr_t)bn->y) & 15) == 0 && (((uintptr_t)bn->hi | (uintptr_t)bn->lo) & 7) == 0,
-               "%s: batch norm: alignment", who);
+    rc = check_bn_out(bn, who);
+    if (rc) return rc;
   }
   if (x_hi && conv_tma_eligible(0, g)) {
     const pf_tc_act a{x_hi, x_lo, nullptr, nullptr, 0, 0};
@@ -1104,6 +1353,18 @@ int pf_conv2d_u8_supported(const pf_conv_desc* d) {
   return conv_tma_u8_eligible(g);
 }
 
+// the cp.async-fed u8 kernel: channel counts that are multiples of 16, and K = R*S*Cin small enough for the exact s32
+// sum (K * 255^2 < 2^31)
+static bool u8_narrow_eligible(const TcGeom& g) {
+  return g.C % 16 == 0 && g.K % 16 == 0 && (int64_t)g.R * g.S * g.C <= 32768;
+}
+
+int pf_conv2d_u8_narrow_supported(const pf_conv_desc* d) {
+  TcGeom g;
+  if (!d || tc_geom(d, &g, "pf_conv2d_u8_narrow_supported")) return 0;
+  return conv_tma_u8_eligible(g) || u8_narrow_eligible(g);
+}
+
 int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* w, const float* bias_dev, int relu,
                      const float* residual_dev, float* y_dev, const pf_tc_bn_out* bn, void* stream) {
   const char* who = "pf_conv2d_u8_fwd";
@@ -1113,12 +1374,21 @@ int pf_conv2d_u8_fwd(const pf_conv_desc* d, const pf_tc_act* x, const pf_tc_wt* 
   TcGeom g;
   int rc = tc_geom(d, &g, who);
   if (rc) return rc;
-  PF_REQUIRE(conv_tma_u8_eligible(g), "%s: needs Cin %% 64 == 0, Cout %% 64 == 0, strides <= 8 and filters <= 16", who);
+  const bool tma = conv_tma_u8_eligible(g);
+  PF_REQUIRE(tma || u8_narrow_eligible(g),
+             "%s: needs Cin %% 16 == 0, Cout %% 16 == 0 and R*S*Cin <= 32768 (or Cin, Cout %% 64 == 0, strides <= 8 and "
+             "filters <= 16)", who);
   PF_REQUIRE((((uintptr_t)x->plane0 | (uintptr_t)w->plane0 | (uintptr_t)y_dev | (uintptr_t)residual_dev |
                (uintptr_t)bias_dev | (uintptr_t)w->alpha | (uintptr_t)w->beta) & 15) == 0 &&
                  ((uintptr_t)x->hdr & 7) == 0,
              "%s: 16-byte alignment required (header: 8)", who);
-  return conv_tma_launch(0, g, *x, *w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who, bn, true);
+  if (bn) {
+    rc = check_bn_out(bn, who);
+    if (rc) return rc;
+  }
+  if (tma) return conv_tma_launch(0, g, *x, *w, y_dev, 0, bias_dev, relu, residual_dev, (cudaStream_t)stream, who, bn, true);
+  PF_REQUIRE(w->bits >= 1 && w->bits <= 8, "%s: weight levels need 1..8 bits", who);
+  return launch_u8(g, *x, *w, y_dev, bias_dev, relu, residual_dev, bn, (cudaStream_t)stream, who);
 }
 
 int pf_conv2d_tc_dgrad_ex(const pf_conv_desc* d, const pf_tc_act* dy, const pf_tc_wt* wd, int accumulate, float* dx_dev,

@@ -512,7 +512,8 @@ bool conv_tma_eligible(int pass, const TcGeom& g) {
   return g.C % 64 == 0 && g.K % 64 == 0 && g.sh <= 8 && g.sw <= 8;
 }
 
-// the u8 forward has no cp.async sibling: only the shape decides
+// the u8 forward of these shapes runs here, the other shapes pf_conv2d_u8_narrow_supported takes run the cp.async-fed
+// u8 kernel (pf_conv_tc.cu): only the shape decides, not the feed setting
 bool conv_tma_u8_eligible(const TcGeom& g) {
   return g.C % 64 == 0 && g.K % 64 == 0 && g.sh <= 8 && g.sw <= 8 && g.R <= 16 && g.S <= 16;
 }

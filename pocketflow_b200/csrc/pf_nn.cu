@@ -10,6 +10,7 @@
 // (uniform_quantization/utils.py:51-79), so the separate reduce_max/reduce_min passes of the
 // reference disappear.
 #include <cstdlib>
+#include <numeric>
 
 #include "pf_common.cuh"
 
@@ -460,6 +461,111 @@ bn_eval_levels_u8_kernel(const float* __restrict__ x, int64_t total, int C, int 
       const int64_t e = i << 2;
       csum[(e >> cshift) * nseg + (int)((e & (int64_t)(C - 1)) >> 7)] = part;
     }
+  }
+}
+
+// The same two passes for a C that is a multiple of 16 but not a power of two (MobileNet-v2's 96 .. 960 channels):
+// an item is one pixel's channel segment (128 channels, the last one partial, as csum counts them), owned by a group
+// of 8 lanes of 16 channels each (lanes past C idle); a lane reads 64 bytes, writes 16 bytes of levels (as two 8-byte stores), and the group's
+// level sum is a 3-step xor butterfly (integers below 2^24: exact).  The item index is the csum index.  Segment-
+// stationary grid: the number of groups is a multiple of nseg (host: seg_grid), so every lane keeps its 16 channels
+// and their batch-norm constants.  The levels are pf_quant_level of the same values as in bn_eval_levels_u8_kernel.
+template <bool RANGE>
+__global__ void __launch_bounds__(NT)
+bn_eval_levels_u8_seg_kernel(const float* __restrict__ x, int64_t items, int C, int nseg, const float* __restrict__ mean,
+                             const float* __restrict__ var, float eps, const float* __restrict__ gamma,
+                             const float* __restrict__ beta, int act, uint32_t* __restrict__ range_enc, int q_bits,
+                             uint8_t* __restrict__ levels, pf_tc_act_hdr* __restrict__ hdr, float* __restrict__ csum) {
+  const int lane = threadIdx.x & 31, sub = threadIdx.x & 7;
+  const int64_t first = ((int64_t)blockIdx.x * NT + threadIdx.x) >> 3;       // this lane's group
+  const int64_t stride = (int64_t)gridDim.x * (NT / 8);
+  const int c0 = (int)(first % nseg) * 128 + sub * 16;
+  const bool cok = c0 < C;
+  float mu[16], rs[16], ga[16], be[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = cok ? c0 + j : 0;
+    mu[j] = __ldg(mean + c);
+    rs[j] = __frsqrt_rn(__fadd_rn(__ldg(var + c), eps));
+    ga[j] = __ldg(gamma + c);
+    be[j] = __ldg(beta + c);
+  }
+  auto load_bn = [&](int64_t item, float (&y)[16]) {
+    const float* src = x + (item / nseg) * C + c0;
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      const float4 a = pf_ld_stream(src + 4 * v);
+      y[4 * v] = pf_bn_act(a.x, mu[4 * v], rs[4 * v], ga[4 * v], be[4 * v], act);
+      y[4 * v + 1] = pf_bn_act(a.y, mu[4 * v + 1], rs[4 * v + 1], ga[4 * v + 1], be[4 * v + 1], act);
+      y[4 * v + 2] = pf_bn_act(a.z, mu[4 * v + 2], rs[4 * v + 2], ga[4 * v + 2], be[4 * v + 2], act);
+      y[4 * v + 3] = pf_bn_act(a.w, mu[4 * v + 3], rs[4 * v + 3], ga[4 * v + 3], be[4 * v + 3], act);
+    }
+  };
+  if (RANGE) {
+    __shared__ float s_mn[NT / 32], s_mx[NT / 32];
+    float mn = INFINITY, mx = -INFINITY;
+    if (cok) {
+      for (int64_t i = first; i < items; i += stride) {
+        float y[16];
+        load_bn(i, y);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          mn = fminf(mn, y[j]);
+          mx = fmaxf(mx, y[j]);
+        }
+      }
+    }
+    mn = pf_warp_min(mn);
+    mx = pf_warp_max(mx);
+    if (lane == 0) {
+      s_mn[threadIdx.x >> 5] = mn;
+      s_mx[threadIdx.x >> 5] = mx;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      mn = lane < NT / 32 ? s_mn[lane] : INFINITY;
+      mx = lane < NT / 32 ? s_mx[lane] : -INFINITY;
+      mn = pf_warp_min(mn);
+      mx = pf_warp_max(mx);
+      if (lane == 0 && mn <= mx) {
+        atomicMin(range_enc, pf_enc(mn));
+        atomicMax(range_enc + 1, pf_enc(mx));
+      }
+    }
+    return;
+  }
+  const float qmn = pf_dec(__ldg(range_enc)), qmx = pf_dec(__ldg(range_enc + 1));
+  const float q_alpha = __fadd_rn(__fsub_rn(qmx, qmn), 1e-10f);
+  const float q_k = pf_uq_kf(q_bits), q_ra = __frcp_rn(q_alpha);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    hdr->scale = qmn == 0.f ? __fdiv_rn(q_alpha, q_k) : 1.f;
+    hdr->nplanes = qmn == 0.f ? 1 : 0;
+  }
+  const int64_t wbase = first - (lane >> 3);           // the warp's first group
+  for (int64_t i = first; wbase + (i - first) < items; i += stride) {   // warp-uniform trip count (group shuffles)
+    float part = 0.f;
+    if (i < items && cok) {
+      float y[16];
+      load_bn(i, y);
+      uint32_t w[4];
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const float l0 = pf_quant_level(y[4 * v], q_alpha, qmn, q_k, q_ra);
+        const float l1 = pf_quant_level(y[4 * v + 1], q_alpha, qmn, q_k, q_ra);
+        const float l2 = pf_quant_level(y[4 * v + 2], q_alpha, qmn, q_k, q_ra);
+        const float l3 = pf_quant_level(y[4 * v + 3], q_alpha, qmn, q_k, q_ra);
+        w[v] = (uint32_t)l0 | ((uint32_t)l1 << 8) | ((uint32_t)l2 << 16) | ((uint32_t)l3 << 24);
+        part += (l0 + l1) + (l2 + l3);
+      }
+      // two 8-byte stores: the entry point promises to work with an 8-byte-aligned levels buffer
+      uint2* dst = reinterpret_cast<uint2*>(levels + (i / nseg) * C + c0);
+      dst[0] = make_uint2(w[0], w[1]);
+      dst[1] = make_uint2(w[2], w[3]);
+    }
+    part += __shfl_xor_sync(0xffffffffu, part, 4);
+    part += __shfl_xor_sync(0xffffffffu, part, 2);
+    part += __shfl_xor_sync(0xffffffffu, part, 1);
+    if (i < items && sub == 0) csum[i] = part;
   }
 }
 
@@ -1070,7 +1176,7 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
                          uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
                          float* csum_dev, void* stream) {
   const char* who = "pf_bn_eval_levels_u8";
-  PF_REQUIRE(m > 0 && c >= 16 && (c & (c - 1)) == 0, "%s: C must be a power of two >= 16 (got %d)", who, c);
+  PF_REQUIRE(m > 0 && c >= 16 && c % 16 == 0, "%s: C must be a multiple of 16 (got %d)", who, c);
   PF_REQUIRE(act >= 0 && act <= 2, "%s: act must be 0 (none), 1 (relu) or 2 (relu6)", who);
   PF_REQUIRE(bits >= 1 && bits <= 8, "%s: u8 levels need 1..8 bits", who);
   PF_REQUIRE(eps >= 0.f, "%s: eps < 0", who);
@@ -1080,13 +1186,33 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
                (uintptr_t)beta_dev) & 15) == 0 && (((uintptr_t)levels_dev | (uintptr_t)hdr_dev) & 7) == 0,
              "%s: fp32 tensors must be 16-byte aligned, levels / header 8-byte aligned", who);
   const int64_t total = m * c;
-  int cshift = 0;
-  while ((1 << cshift) < c) ++cshift;
   const int nseg = (c + 127) / 128;
-  const unsigned grid = chan_grid(total >> 2, c);
-  PF_REQUIRE(((int64_t)grid * NT) % (c >> 2) == 0, "%s: C = %d too large for the channel-stationary grid", who, c);
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* lv = reinterpret_cast<uint8_t*>(levels_dev);
+  if (c & (c - 1)) {
+    // groups of 8 lanes per (pixel, segment) item; a multiple of nseg groups in the grid
+    const int64_t items = m * nseg;
+    int64_t grid = std::min((items * 8 + NT - 1) / NT, (int64_t)PF_NUM_SMS * bn_grid_cap());
+    const int64_t mult = nseg / std::gcd(nseg, NT / 8);
+    grid = std::max<int64_t>(1, (grid + mult - 1) / mult) * mult;
+    if (!have_range) {
+      const int rc = pf_minmax_reset(range_enc_dev, 1, stream);
+      if (rc) return rc;
+      bn_eval_levels_u8_seg_kernel<true><<<(unsigned)grid, NT, 0, st>>>(x_dev, items, c, nseg, moving_mean_dev,
+                                                                        moving_var_dev, eps, gamma_dev, beta_dev, act,
+                                                                        range_enc_dev, bits, lv, hdr_dev, csum_dev);
+      PF_CHECK_LAUNCH(who);
+    }
+    bn_eval_levels_u8_seg_kernel<false><<<(unsigned)grid, NT, 0, st>>>(x_dev, items, c, nseg, moving_mean_dev,
+                                                                       moving_var_dev, eps, gamma_dev, beta_dev, act,
+                                                                       range_enc_dev, bits, lv, hdr_dev, csum_dev);
+    PF_CHECK_LAUNCH(who);
+    return PF_OK;
+  }
+  int cshift = 0;
+  while ((1 << cshift) < c) ++cshift;
+  const unsigned grid = chan_grid(total >> 2, c);
+  PF_REQUIRE(((int64_t)grid * NT) % (c >> 2) == 0, "%s: C = %d too large for the channel-stationary grid", who, c);
   if (!have_range) {
     const int rc = pf_minmax_reset(range_enc_dev, 1, stream);
     if (rc) return rc;

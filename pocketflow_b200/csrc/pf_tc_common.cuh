@@ -106,7 +106,13 @@ __device__ __forceinline__ void wgmma_wait(float (&d)[H][R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[h][i])::"memory");
 }
-// the same for an s32 accumulator of H row blocks (u8 x u8 MMAs)
+// the same for an s32 accumulator (u8 x u8 MMAs), of one or of H row blocks
+template <int N, int R>
+__device__ __forceinline__ void wgmma_wait(int (&d)[R]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 template <int N, int H, int R>
 __device__ __forceinline__ void wgmma_wait(int (&d)[H][R]) {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
@@ -234,6 +240,33 @@ template <> struct Wgmma<256> {
 // is below 2^16, so a sum of K products stays below 2^31 for K < 33,000.
 template <int N>
 struct WgmmaU8;
+template <> struct WgmmaU8<16> {
+  __device__ __forceinline__ static void mma(int (&d)[8], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.u8 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+        : "l"(a), "l"(b), "r"(1)
+        : "memory");
+  }
+};
+template <> struct WgmmaU8<32> {
+  __device__ __forceinline__ static void mma(int (&d)[16], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, %16, %17, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(a), "l"(b), "r"(1)
+        : "memory");
+  }
+};
 template <> struct WgmmaU8<64> {
   __device__ __forceinline__ static void mma(int (&d)[32], uint64_t a, uint64_t b) {
     asm volatile(

@@ -23,6 +23,19 @@ conditions run on u8 levels too (pf_dwconv_u8_fwd, CUDA cores: exact window sums
 channel, then the same affine epilogue), fed by the same batch norm + ReLU level producer.  Their sidecar carries
 version 2, which loaders before this option refuse.
 
+With `cfg['int8_narrow']` (opt-in, like `int8_depthwise`) the shape conditions widen to channel counts that are
+multiples of 16: a convolution qualifies where `ops.conv2d_u8_narrow_supported` holds (pf_conv2d_u8_fwd picks its
+cp.async-fed kernel for the shapes the TMA-fed one does not take), a depthwise layer at any input C % 16 == 0, and the
+level producer writes any such C.  ResNet-20's 16- and 32-channel stages and MobileNet-v2's depthwise layers and
+projections then run on integers.  The sidecar records the option in its config and keeps its version (1, or 2 with
+depthwise integer layers): a loader that does not know the option selects fewer integer layers than the file holds
+levels for, and IntModel refuses that with its coverage ValueError instead of building a different model.
+
+select() decides from the graph alone.  The u8 convolution takes its residual and folded batch norm over from the
+executor's tensor-core lowering of the layer (_TcConv), which every selected shape has on the default conv path
+(Cin, Cout % 16 == 0); with another path (PF_CONV_PATH) IntModel's construction fails with a ValueError naming the
+layer, rather than the layer falling back to fake-quant.
+
     im = IntModel.from_checkpoint(graph, images, logits, state, cfg)   # the learner's checkpoint (unquantized weights)
     logits = im.forward(images_tensor)
     im.export(path)                                                    # integer checkpoint + sidecar
@@ -94,11 +107,13 @@ def _conv_desc(op):
 
 def select(graph, logits, cfg):
     """[(op name, None or the reason it keeps the fake-quant kernels)] for every Conv2D / MatMul / depthwise op in
-    graph order; None = it runs on a u8 kernel.  Depthwise ops are considered only with cfg['int8_depthwise']."""
+    graph order; None = it runs on a u8 kernel.  Depthwise ops are considered only with cfg['int8_depthwise'];
+    cfg['int8_narrow'] admits channel counts that are multiples of 16."""
     from . import ops
     mm, acts = quant_marks(graph, cfg)
     mm, acts = set(mm), set(acts)
     depthwise = bool(cfg.get('int8_depthwise', False))
+    narrow = bool(cfg.get('int8_narrow', False))
     out = []
     for op in compact.reachable_ops(graph, logits):
         if op.type not in ('Conv2D', 'MatMul', 'DepthwiseConv2dNative'):
@@ -122,13 +137,17 @@ def select(graph, logits, cfg):
             why = 'activation bits %d > 8' % cfg['activation_bits']
         else:
             c = x.shape[-1]
-            if dw and (c < 16 or c & (c - 1)):
-                why = 'input channels %d: the level producer needs a power of two >= 16' % c
+            if dw and (c < 16 or (c % 16 if narrow else c & (c - 1))):
+                why = 'input channels %d: the level producer needs %s' % (
+                    c, 'a multiple of 16' if narrow else 'a power of two >= 16')
             elif dw:
                 if not ops.dwconv_u8_supported(_conv_desc(op)):
                     (kh, kw), (sh, sw) = op.attrs['ksize'], op.attrs['strides']
                     why = 'depthwise %dx%d stride %dx%d over %d channels (the u8 depthwise kernel needs C %% 16 == 0, ' \
                           '<= 9 taps, strides 1 or 2)' % (kh, kw, sh, sw, c)
+            elif narrow:
+                if not ops.conv2d_u8_narrow_supported(_conv_desc(op)):
+                    why = 'shape %d -> %d channels (the u8 kernels need multiples of 16)' % (c, op.output.shape[-1])
             elif c < 16 or c & (c - 1):
                 why = 'input channels %d not a power of two' % c
             elif not ops.conv2d_u8_supported(_conv_desc(op)):
@@ -216,7 +235,9 @@ class _U8Conv:
         self.alpha = torch.from_numpy(np.ascontiguousarray(alpha, F32)).to(dev)
         self.beta = torch.from_numpy(np.ascontiguousarray(beta, F32)).to(dev)
         tc = ex.conv[op]
-        assert isinstance(tc, _TcConv), op.name
+        if not isinstance(tc, _TcConv):
+            raise ValueError('%s: its fake-quant lowering is %s, not a tensor-core convolution, so there is no residual '
+                             'or folded batch norm plan for the u8 kernel to take over' % (op.name, type(tc).__name__))
         self.res, self.bn_out = tc.res, tc.bn_out
 
     def prepare_weights(self):
@@ -347,8 +368,9 @@ class IntModel:
             raise ValueError('%s.int8.json: unsupported sidecar version %r (this loader reads %s)'
                              % (path, rec.get('version'), ', '.join(map(str, SIDECAR_VERSIONS))))
         cfg = {k: rec['config'][k] for k in CFG_KEYS}
-        if rec['config'].get('int8_depthwise'):
-            cfg['int8_depthwise'] = True
+        for opt in ('int8_depthwise', 'int8_narrow'):
+            if rec['config'].get(opt):
+                cfg[opt] = True
         d = np.load(path + '.npz')
         arrays = {k.replace('|', '/'): d[k] for k in d.files}
         byname = {op.name: op for op in compact.reachable_ops(graph, logits)}

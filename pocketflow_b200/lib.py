@@ -74,6 +74,7 @@ SIGNATURES = {
     'pf_conv2d_tc_wgrad_ex': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_conv2d_tc_last_plan': (c_i32, [c_vp]),
     'pf_conv2d_u8_supported': (c_i32, [c_vp]),
+    'pf_conv2d_u8_narrow_supported': (c_i32, [c_vp]),
     'pf_conv2d_u8_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_eval_levels_u8': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp,
                                      c_vp, c_vp]),

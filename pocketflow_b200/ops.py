@@ -1144,6 +1144,12 @@ def conv2d_u8_supported(d):
     return bool(_lib.load().pf_conv2d_u8_supported(ctypes.byref(d)))
 
 
+def conv2d_u8_narrow_supported(d):
+    """the shapes pf_conv2d_u8_fwd runs on either of its kernels: those of conv2d_u8_supported, and any Cin and Cout
+    that are multiples of 16 with R*S*Cin <= 32768 (the cp.async-fed kernel)"""
+    return bool(_lib.load().pf_conv2d_u8_narrow_supported(ctypes.byref(d)))
+
+
 def conv2d_u8_fwd(d, x_levels, hdr, csum, w_levels, alpha, beta, bits, y, bias=None, relu=False, residual=None,
                   bn_out=None):
     """y = the fake-quantized conv from u8 levels (pf_conv2d_u8_fwd): x_levels uint8 [N, H, W, Cin] with its header and

@@ -7,6 +7,9 @@ both on the inputs a forward of the seed-initialised model left in their buffers
 u8 kernel's lower bound: the larger of the FLOP bound (2 M N K at the u8 data-sheet rate, 1,979 dense TOPS) and the byte
 bound (u8 operands read once, fp32 output written once, at 3.35 TB/s).
 
+With --int8_narrow the integer model also runs the layers whose channel counts are multiples of 16 but not of 64 (the
+cp.async-fed u8 kernel); each line names the kernel that ran.
+
 The integer model is built with its depthwise layers on u8 levels too (cfg['int8_depthwise']): each is timed the same
 way against pf_dwconv_fwd on the fake-quant model's fp32 input, with the byte bound of each (u8: 1 B read per input
 element, 4 B written per output; fp32: 4 B and 4 B) and the u8 kernel's share of its own.
@@ -33,6 +36,7 @@ def parse(argv=None):
     p.add_argument('--mobilenet_version', type=int, default=None)
     p.add_argument('--batch_size_eval', type=int, default=128)
     p.add_argument('--launches', type=int, default=50, help='launches per timed layer')
+    p.add_argument('--int8_narrow', action='store_true', help='also the layers of the cp.async-fed u8 kernel')
     p.add_argument('--json', default=None)
     return p.parse_args(argv)
 
@@ -53,7 +57,7 @@ def main(argv=None):
     args = parse(argv)
     import torch
     from export_uq_int8 import gpu_name, load_state, setup
-    from pocketflow_b200 import compact, int8
+    from pocketflow_b200 import compact, int8, ops
     args.ckpt_dir = None
     for k, v in dict(uql_weight_bits=8, uql_activation_bits=8, uql_use_buckets=True, uql_bucket_type='channel',
                      uql_bucket_size=256, uql_quantize_all_layers=False).items():
@@ -83,15 +87,15 @@ def main(argv=None):
         t_u8 = _ms(lo.forward, args.launches, torch)
         t_fq = _ms(fq_conv[op.name].forward, args.launches, torch)
         bound = max(flop_s, byte_s) * 1e3
-        rows.append(dict(op=op.name, m=m, n=n, k=k, u8_ms=t_u8, fake_quant_ms=t_fq, bound_ms=bound,
+        kern = 'tma' if ops.conv2d_u8_supported(d) else 'cp.async'
+        rows.append(dict(op=op.name, kernel=kern, m=m, n=n, k=k, u8_ms=t_u8, fake_quant_ms=t_fq, bound_ms=bound,
                          bound_by='flops' if flop_s >= byte_s else 'bytes', u8_share_of_bound=bound / t_u8))
         for key, v in (('u8', t_u8), ('fq', t_fq), ('bound', bound)):
             tot[key] += v
-        print('%-48s M %7d N %5d K %5d | u8 %.4f ms  fake-quant %.4f ms | bound %.4f ms (%s) = %.0f %% of u8'
-              % (op.name, m, n, k, t_u8, t_fq, bound, rows[-1]['bound_by'], 100 * bound / t_u8))
+        print('%-48s %-8s M %7d N %5d K %5d | u8 %.4f ms  fake-quant %.4f ms | bound %.4f ms (%s) = %.0f %% of u8'
+              % (op.name, kern, m, n, k, t_u8, t_fq, bound, rows[-1]['bound_by'], 100 * bound / t_u8))
     print('all %d u8 layers: u8 %.3f ms, fake-quant %.3f ms, bound %.3f ms' % (len(rows), tot['u8'], tot['fq'],
                                                                               tot['bound']))
-    from pocketflow_b200 import ops
     dw_rows, dw_tot = [], dict(u8=0.0, fp32=0.0, bound=0.0, fp32_bound=0.0)
     for op, lo in im.ex.dwconv.items():
         d = lo.d

@@ -41,6 +41,9 @@ def parse(argv=None):
     p.add_argument('--uql_quantize_all_layers', action='store_true')
     p.add_argument('--int8_depthwise', action='store_true',
                    help='depthwise layers on u8 levels too (pf_dwconv_u8_fwd); also times the integer model without them')
+    p.add_argument('--int8_narrow', action='store_true',
+                   help='channel counts that are multiples of 16 too (the cp.async-fed u8 kernel, any C %% 16 level '
+                        'producer); also times the integer model without them')
     p.add_argument('--batch_size_eval', type=int, default=100)
     p.add_argument('--nb_repts_warmup', type=int, default=20, help='graph replays before timing')
     p.add_argument('--nb_repts', type=int, default=50, help='graph replays per timed window')
@@ -67,8 +70,9 @@ def setup(args):
         setattr(FLAGS, k, getattr(args, k))
     graph, images, logits = compact.build_eval_graph(net.ModelHelper(), args.batch_size_eval)
     cfg = int8.config_from_flags()
-    if getattr(args, 'int8_depthwise', False):
-        cfg['int8_depthwise'] = True
+    for opt in ('int8_depthwise', 'int8_narrow'):
+        if getattr(args, opt, False):
+            cfg[opt] = True
     return graph, images, logits, cfg
 
 
@@ -115,12 +119,14 @@ def main(argv=None):
     x = torch.randn(images.shape, generator=torch.Generator().manual_seed(0)).to(dev)
     fq.buf[images].copy_(x)
     im.ex.buf[images].copy_(x)
-    arms = {'fake_quant': fq, 'integer': im.ex}
-    if cfg.get('int8_depthwise'):             # the same integer model with its depthwise layers on the fake-quant path
-        nodw = {k: v for k, v in cfg.items() if k != 'int8_depthwise'}
-        im_nodw = int8.IntModel.from_checkpoint(graph, images, logits, state, nodw, dev)
-        im_nodw.ex.buf[images].copy_(x)
-        arms = {'fake_quant': fq, 'integer_no_depthwise': im_nodw.ex, 'integer': im.ex}
+    arms = {'fake_quant': fq}
+    for opt, arm in (('int8_narrow', 'integer_no_narrow'), ('int8_depthwise', 'integer_no_depthwise')):
+        if cfg.get(opt):                      # the same integer model without the option's layers
+            im_without = int8.IntModel.from_checkpoint(graph, images, logits, state,
+                                                       {k: v for k, v in cfg.items() if k != opt}, dev)
+            im_without.ex.buf[images].copy_(x)
+            arms[arm] = im_without.ex
+    arms['integer'] = im.ex
     graphs = {arm: _capture(lambda ex=ex: ex.forward(training=False), torch) for arm, ex in arms.items()}
     for gr in graphs.values():
         gr.replay()
