@@ -34,6 +34,9 @@ class _ConvLowering:
 
     def __init__(self, ex, op):
         self.ex, self.op, self.d, self.x = ex, op, ex.desc[op], op.inputs[0]
+        # the residual Add and the folded inference BN (_BnFolded) of the epilogue: tensor-core lowerings only
+        self.res = ex.fused_add[op][1] if op in ex.fused_add else None
+        self.bn_out = ex.batch_norm[ex.bn_fold[op]].bn_out if op in ex.bn_fold else None
 
     def _epilogue(self):
         """(bias, fused relu, output buffer) of the forward kernel"""
@@ -65,8 +68,6 @@ class _TcConv(_ConvLowering):
         super().__init__(ex, op)
         self.tw, self.xp, self.w_lv = ex.tc[op], ex.planes_of(self.x), ex.w_lv.get(op)
         self.x_lv = ex.act_lv.get(ex._root(self.x).op) if self.xp is not None else None
-        self.res = ex.fused_add[op][1] if op in ex.fused_add else None
-        self.bn_out = ex.batch_norm[ex.bn_fold[op]].bn_out if op in ex.bn_fold else None    # folded BN (_BnFolded)
         self.tc_wgrad = op in ex.tc_wgrad
         if self.tc_wgrad:
             self.xw = ops.Planes(self.x.numel, ex.device, ex.x_scratch.buf) if self.xp is None else self.xp
@@ -182,6 +183,66 @@ class _StemConv(_ConvLowering):
             ops.add(im['dwpad'][:dw.numel()], None, dw.reshape(-1))
 
 
+def _u8_operands(lo, layout):
+    """an integer layer's operands (Executor.int_layers): the _U8Bn of its input's producer, and its weight levels in
+    `layout`, scales and bits"""
+    ex = lo.ex
+    levels, alpha, beta, lo.bits = ex.int_layers[lo.op]
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(ex.device)
+    lo.bn = ex.batch_norm[ex._root(lo.x).op]
+    lo.wl, lo.alpha, lo.beta = up(layout(levels)), up(np.asarray(alpha, F32)), up(np.asarray(beta, F32))
+
+
+class _U8Conv(_ConvLowering):
+    """Integer layer: the u8 tensor-core conv (pf_conv2d_u8_fwd) from the levels of its input's producer and its own
+    weight levels [Cout, R*S*Cin], with a tensor-core lowering's residual and folded BN; no split-bf16 weight copy."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op)
+        _u8_operands(self, lambda lv: lv.reshape(-1, lv.shape[-1]).T)
+
+    def forward(self):
+        ex, (bias, relu, y) = self.ex, self._epilogue()
+        res = ex.T(self.res) if self.res is not None else None
+        with ex.timed('conv_fwd'):
+            ops.conv2d_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.bn.csum, self.wl, self.alpha, self.beta,
+                              self.bits, y, bias, relu, res, self.bn_out)
+
+
+class _DwConv:
+    """How one DepthwiseConv2dNative runs, fixed at plan time; this class: the exact-fp32 CUDA-core kernels."""
+
+    def __init__(self, ex, op):
+        self.ex, self.op, self.d, self.x = ex, op, ex.desc[op], op.inputs[0]
+
+    def forward(self):
+        ex = self.ex
+        with ex.timed('dwconv'):
+            ops.dwconv_fwd(self.d, ex.T(self.x), ex.kernel_of(self.op), ex.buf[self.op.output])
+
+    def backward(self, gy):
+        ex = self.ex
+        with ex.timed('dwconv'):
+            ops.dwconv_wgrad(self.d, ex.T(self.x), gy, ex.wgrad_ws, ex.store.view(self.op.vars['kernel'], ex.G))
+            if self.x.op.type != 'Placeholder':
+                gx, acc = ex.grad_target(self.x)
+                ops.dwconv_dgrad(self.d, gy, ex.kernel_of(self.op), acc, gx)
+
+
+class _U8DwConv(_DwConv):
+    """Integer depthwise layer: pf_dwconv_u8_fwd from the levels of its input's producer and its own weight levels
+    [R*S, C]."""
+
+    def __init__(self, ex, op):
+        super().__init__(ex, op)
+        _u8_operands(self, lambda lv: lv.reshape(-1, lv.shape[-2]))
+
+    def forward(self):
+        with self.ex.timed('dwconv'):
+            ops.dwconv_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.wl, self.alpha, self.beta, self.bits,
+                              self.ex.buf[self.op.output])
+
+
 class _BnLowering:
     """How one FusedBatchNorm runs, fixed at plan time; this class: the apply, with the quantizer of its fused ReLU in
     the same pass (integer levels where it writes them).  `writes`: the op whose fp32 output / planes it writes."""
@@ -282,6 +343,26 @@ class _BnFolded(_BnLowering):
 
     def forward(self, training):
         """applied by the producing conv's epilogue"""
+
+
+class _U8Bn:
+    """Inference BN + quantized ReLU that feeds integer layers: writes the u8 levels, header and channel sums they read
+    (pf_bn_eval_levels_u8), after its fake-quant lowering `base` when other readers need the fp32 tensor or planes."""
+
+    def __init__(self, ex, op, base):
+        self.ex, self.op, self.base, self.others = ex, op, base, ex.u8_others[op]
+        c = op.output.shape[-1]
+        self.levels = torch.empty(op.output.numel, dtype=torch.uint8, device=ex.device)
+        self.hdr = torch.zeros(2, dtype=torch.int32, device=ex.device)
+        self.csum = torch.empty(op.output.numel // c * ((c + 127) // 128), dtype=torch.float32, device=ex.device)
+
+    def forward(self, training):
+        ex, base = self.ex, self.base
+        if self.others:
+            base.forward(training)
+        with ex.timed('act_quant'):
+            ops.bn_eval_levels_u8(ex.T(self.op.inputs[0]), *base.moving, base.act, ex.act_quant['bits'][base.aq],
+                                  base.slot, self.levels, self.hdr, self.csum, have_range=self.others)
 
 
 class ParamStore:
@@ -394,8 +475,13 @@ class Executor:
     def __init__(self, graph, images, logits, device, store=None, train=True, loss=None, labels=None,
                  optimizer=None, weight_quant=None, act_quant=None, maskable=None, teacher=None,
                  seed=1, exact_ste=True, grad_scale=1.0, scope=None, conv_path=None, fuse_add=True,
-                 update_moving_stats=True, frozen=None):
+                 update_moving_stats=True, frozen=None, int_layers=None):
         self.g, self.device, self.train = graph, device, train
+        # int_layers (inference only, int8.IntModel): {Conv2D / depthwise op: (weight levels uint8 HWIO, alpha, beta,
+        # bits)} of the layers that run on the u8 kernels, from the u8 levels their batch norm + ReLU producer writes
+        if int_layers and train:
+            raise ValueError('integer layers run only in an inference executor (train=False)')
+        self.int_layers = dict(int_layers or {})
         # fuse_add=False: every Conv2D output is materialised on its own (the channel-pruning learner regresses conv
         # outputs of a pruned model onto those of the full model, learners/channel_pruning_gpu/learner.py:339-354);
         # update_moving_stats=False: training-mode BN without the moving-average update ops (the FULL model of that
@@ -565,7 +651,8 @@ class Executor:
                 self.aq_out[op] = E(t.shape)
         # ---- per-op scratch
         self.bn = {}
-        self.tc = {}
+        self.tc_conv = set()       # convs with a tensor-core lowering (_TcConv, or _U8Conv for an integer layer)
+        self.tc = {}               # their split-bf16 weight copies (not an integer layer's)
         self.tc_wgrad = set()
         self.im2col = {}
         self.pool_argmax = {}
@@ -636,7 +723,12 @@ class Executor:
                             max_ws = max(max_ws, ops.conv2d_tc_wgrad_planes_workspace_floats(d1))
                         max_ws = max(max_ws, ops.conv2d_wgrad_workspace_floats(d1))
                 if self.conv_path == 'tc' and ops.conv2d_tc_supported(d):
-                    self.tc[op] = ops.TcWeights(d, dev, need_dgrad=self.train and x.op.type != 'Placeholder')
+                    self.tc_conv.add(op)
+                    if op not in self.int_layers:
+                        self.tc[op] = ops.TcWeights(d, dev, need_dgrad=self.train and x.op.type != 'Placeholder')
+                elif op in self.int_layers:
+                    raise ValueError('%s: an integer layer needs a tensor-core lowering (conv path %r) for its '
+                                     'residual and folded batch norm' % (op.name, self.conv_path))
                 if self.train:
                     if op in self.tc and ops.conv2d_tc_wgrad_supported(d):
                         self.tc_wgrad.add(op)
@@ -668,8 +760,8 @@ class Executor:
                 continue
             for i, x_t in enumerate(op.inputs):
                 src, other = x_t.op, op.inputs[1 - i]
-                if src.type == 'Conv2D' and src in self.tc and x_t not in self.alias and src not in self.fused_act \
-                        and 'bias' not in src.vars and len(self._consumers(x_t)) == 1 \
+                if src.type == 'Conv2D' and src in self.tc_conv and x_t not in self.alias \
+                        and src not in self.fused_act and 'bias' not in src.vars and len(self._consumers(x_t)) == 1 \
                         and self.g.ops.index(other.op) < self.g.ops.index(src):
                     self.fused_add[src] = (op, other)
                     self.add_fused.add(op)
@@ -803,14 +895,18 @@ class Executor:
             self.beta1_power = F32(self.optimizer.get('beta1', 0.9))
             self.beta2_power = F32(self.optimizer.get('beta2', 0.999))
         self.bn_fold = self._plan_bn_fold()
-        # ---- how each FusedBatchNorm and each Conv2D / MatMul runs forward, backward and in layer_wgrad
-        self.batch_norm = {op: (_BnAdd if op in self.bn_add else _BnFolded if op in self.bn_fold.values() else
-                                _BnGather if op in self.bn_gather else _BnLowering)(self, op)
-                           for op in self.ops if op.type == 'FusedBatchNorm'}
-        self.conv = {op: (_StemConv if op in self.im2col else _TcConv if op in self.tc else _ConvLowering)(self, op)
+        # ---- how each FusedBatchNorm, Conv2D / MatMul and depthwise conv runs forward, backward and in layer_wgrad
+        self.batch_norm = {}
+        for op in self.ops:
+            if op.type == 'FusedBatchNorm':
+                lo = (_BnAdd if op in self.bn_add else _BnFolded if op in self.bn_fold.values() else
+                      _BnGather if op in self.bn_gather else _BnLowering)(self, op)
+                self.batch_norm[op] = _U8Bn(self, op, lo) if op in self.u8_others else lo
+        self.conv = {op: (_U8Conv if op in self.int_layers else _StemConv if op in self.im2col else
+                          _TcConv if op in self.tc else _ConvLowering)(self, op)
                      for op in self.ops if op.type in ('Conv2D', 'MatMul')}
-        # depthwise convolutions run pf_dwconv_fwd unless a lowering is registered here (int8.IntModel's u8 layers)
-        self.dwconv = {}
+        self.depthwise = {op: (_U8DwConv if op in self.int_layers else _DwConv)(self, op)
+                          for op in self.ops if op.type == 'DepthwiseConv2dNative'}
 
     def _plan_bn_add(self):
         """Linear bottleneck: a BatchNorm without activation whose only consumer is a residual Add (MobileNet-v2's
@@ -834,7 +930,9 @@ class Executor:
     def _plan_operand_planes(self):
         """Split-bf16 operand planes (tensor-core path): the BN apply / activation quantizer / gather that produces a
         conv input writes it directly in the operand format of the tensor-core kernels (x = hi + lo, two bf16 planes);
-        the fp32 copy is only written when some other consumer needs it.  Returns {producer: the convs reading them}."""
+        the fp32 copy is only written when some other consumer needs it.  An integer layer reads its producer's u8
+        levels (_U8Bn): it is neither a planes nor an fp32 reader, and `u8_others` says whether such a producer also
+        writes its planes or fp32 output for other readers.  Returns {producer: the convs reading its planes}."""
         bn_adds = {a for a, _ in self.bn_add.values()}
         self.xplanes, self.bn_need_f32, readers = {}, {}, {}
         for op in self.ops:
@@ -844,15 +942,19 @@ class Executor:
                         and r.numel % 8 == 0:
                     if r.op not in self.xplanes:
                         self.xplanes[r.op] = ops.Planes(r.numel, self.device)
-                        self.bn_need_f32[r.op] = False
                     readers.setdefault(r.op, []).append(op)
-        for bn_op in self.xplanes:
+        u8_src = dict.fromkeys(self._root(op.inputs[0]).op for op in self.ops if op in self.int_layers)
+        self.u8_others = {}
+        for bn_op in dict.fromkeys(list(self.xplanes) + list(u8_src)):
             ts = [bn_op.output] + [c.output for c in self._consumers(bn_op.output) if c in self.fused_into]
-            for t in ts:
-                for c in self._consumers(t):        # a reader that is not the fused activation nor a planes conv
-                    if self.fused_into.get(c) is not bn_op and \
-                            not (c in self.tc and c not in self.im2col and (not self.train or c in self.tc_wgrad)):
-                        self.bn_need_f32[bn_op] = True
+            # a reader that is not the fused activation, an integer layer nor a planes conv
+            f32 = any(self.fused_into.get(c) is not bn_op and c not in self.int_layers and
+                      not (c in self.tc and c not in self.im2col and (not self.train or c in self.tc_wgrad))
+                      for t in ts for c in self._consumers(t))
+            if bn_op in self.xplanes:
+                self.bn_need_f32[bn_op] = f32
+            if bn_op in u8_src:
+                self.u8_others[bn_op] = f32 or bn_op in self.xplanes
         return readers
 
     def _plan_bn_gather(self):
@@ -959,7 +1061,7 @@ class Executor:
             if r is None or r.shape[-1] != x.shape[-1]:
                 continue
             conv = r.op if r.op.type == 'Conv2D' else add_conv.get(r.op)
-            if conv is None or conv not in self.tc or conv in self.im2col or conv in fold \
+            if conv is None or conv not in self.tc_conv or conv in self.im2col or conv in fold \
                     or self._aq_of_bn(op) is not None:
                 continue
             fold[conv] = op
@@ -1090,11 +1192,7 @@ class Executor:
             if ty in ('Conv2D', 'MatMul'):
                 self.conv[op].forward()
             elif ty == 'DepthwiseConv2dNative':
-                if op in self.dwconv:
-                    self.dwconv[op].forward()
-                    continue
-                with self.timed('dwconv'):
-                    ops.dwconv_fwd(self.desc[op], self.T(op.inputs[0]), self.kernel_of(op), self.buf[op.output])
+                self.depthwise[op].forward()
             elif ty == 'FusedBatchNorm':
                 self.batch_norm[op].forward(training)
             elif ty == 'GatherChannels':
@@ -1245,13 +1343,7 @@ class Executor:
                     with self.timed('conv_dgrad'):
                         lo.dgrad(gy, gx, acc)
             elif ty == 'DepthwiseConv2dNative':
-                d = self.desc[op]
-                x_t = op.inputs[0]
-                with self.timed('dwconv'):
-                    ops.dwconv_wgrad(d, self.T(x_t), gy, self.wgrad_ws, st.view(op.vars['kernel'], self.G))
-                    if x_t.op.type != 'Placeholder':
-                        gx, acc = self.grad_target(x_t)
-                        ops.dwconv_dgrad(d, gy, self.kernel_of(op), acc, gx)
+                self.depthwise[op].backward(gy)
             elif ty == 'FusedBatchNorm':
                 self.batch_norm[op].backward(gy)
             elif ty == 'GatherChannels':

@@ -31,10 +31,12 @@ projections then run on integers.  The sidecar records the option in its config 
 depthwise integer layers): a loader that does not know the option selects fewer integer layers than the file holds
 levels for, and IntModel refuses that with its coverage ValueError instead of building a different model.
 
-select() decides from the graph alone.  The u8 convolution takes its residual and folded batch norm over from the
-executor's tensor-core lowering of the layer (_TcConv), which every selected shape has on the default conv path
-(Cin, Cout % 16 == 0); with another path (PF_CONV_PATH) IntModel's construction fails with a ValueError naming the
-layer, rather than the layer falling back to fake-quant.
+select() decides from the graph alone.  IntModel hands the selected layers and their weight levels to the executor
+(`int_layers`), whose plan lowers them (engine._U8Conv, _U8DwConv) and the batch norms feeding them (_U8Bn) beside
+every other layer.  A u8 convolution takes the residual and folded batch norm a tensor-core lowering of the layer would
+take, and owns no split-bf16 weight copy.  Every selected shape has that lowering on the default conv path (Cin, Cout
+% 16 == 0); with another path (PF_CONV_PATH) the executor's plan fails with a ValueError naming the layer, rather than
+the layer falling back to fake-quant.
 
     im = IntModel.from_checkpoint(graph, images, logits, state, cfg)   # the learner's checkpoint (unquantized weights)
     logits = im.forward(images_tensor)
@@ -196,87 +198,9 @@ def fake_quant_executor(graph, images, logits, state, cfg, device):
     return ex
 
 
-class _U8Bn:
-    """The batch norm + quantized ReLU feeding u8 convolutions: writes the u8 levels, header and channel sums (and,
-    first, what its fake-quant lowering writes when other readers need the fp32 tensor or split-bf16 planes)."""
-
-    def __init__(self, ex, op, base, others):
-        import torch
-        self.ex, self.op, self.base, self.others = ex, op, base, others
-        st = ex.store
-        c = op.output.shape[-1]
-        self.m, self.c = op.output.numel // c, c
-        self.args = (st.view(op.vars['moving_mean']), st.view(op.vars['moving_variance']), op.attrs['epsilon'],
-                     st.view(op.vars['gamma']), st.view(op.vars['beta']), ex.fused_act.get(op, 0))
-        self.bits = ex.act_quant['bits'][base.aq]
-        self.levels = torch.empty(op.output.numel, dtype=torch.uint8, device=ex.device)
-        self.hdr = torch.zeros(2, dtype=torch.int32, device=ex.device)
-        self.csum = torch.empty(self.m * ((c + 127) // 128), dtype=torch.float32, device=ex.device)
-
-    def forward(self, training):
-        from . import ops
-        if self.others:
-            self.base.forward(training)
-        with self.ex.timed('act_quant'):
-            ops.bn_eval_levels_u8(self.ex.T(self.op.inputs[0]), self.m, self.c, *self.args, self.bits, self.base.slot,
-                                  self.levels, self.hdr, self.csum, have_range=self.others)
-
-
-class _U8Conv:
-    """A convolution on the u8 kernel, from the levels of its input's producer and its own weight levels."""
-
-    def __init__(self, ex, op, bn, levels, alpha, beta, bits):
-        from .engine import _TcConv
-        import torch
-        self.ex, self.op, self.bn, self.bits = ex, op, bn, bits
-        self.d = ex.desc[op]
-        dev = ex.device
-        self.wl = torch.from_numpy(np.ascontiguousarray(levels.reshape(-1, levels.shape[-1]).T)).to(dev)
-        self.alpha = torch.from_numpy(np.ascontiguousarray(alpha, F32)).to(dev)
-        self.beta = torch.from_numpy(np.ascontiguousarray(beta, F32)).to(dev)
-        tc = ex.conv[op]
-        if not isinstance(tc, _TcConv):
-            raise ValueError('%s: its fake-quant lowering is %s, not a tensor-core convolution, so there is no residual '
-                             'or folded batch norm plan for the u8 kernel to take over' % (op.name, type(tc).__name__))
-        self.res, self.bn_out = tc.res, tc.bn_out
-
-    def prepare_weights(self):
-        """the levels are uploaded once"""
-
-    def forward(self):
-        from . import ops
-        ex, op = self.ex, self.op
-        bias = ex.store.view(op.vars['bias']) if 'bias' in op.vars else None
-        res = ex.T(self.res) if self.res is not None else None
-        with ex.timed('conv_fwd'):
-            ops.conv2d_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.bn.csum, self.wl, self.alpha, self.beta,
-                              self.bits, ex.buf[op.output], bias, op in ex.fused_act, res, self.bn_out)
-
-
-class _U8DwConv:
-    """A depthwise convolution on pf_dwconv_u8_fwd, from the levels of its input's producer and its own weight levels
-    (registered in the executor's `dwconv` table, which its forward consults before pf_dwconv_fwd)."""
-
-    def __init__(self, ex, op, bn, levels, alpha, beta, bits):
-        import torch
-        self.ex, self.op, self.bn, self.bits = ex, op, bn, bits
-        self.d = ex.desc[op]
-        dev = ex.device
-        self.wl = torch.from_numpy(np.ascontiguousarray(levels.reshape(-1, levels.shape[-2]))).to(dev)   # [R*S, C]
-        self.alpha = torch.from_numpy(np.ascontiguousarray(alpha, F32)).to(dev)
-        self.beta = torch.from_numpy(np.ascontiguousarray(beta, F32)).to(dev)
-
-    def forward(self):
-        from . import ops
-        ex = self.ex
-        with ex.timed('dwconv'):
-            ops.dwconv_u8_fwd(self.d, self.bn.levels, self.bn.hdr, self.wl, self.alpha, self.beta, self.bits,
-                              ex.buf[self.op.output])
-
-
 class IntModel:
-    """A uniformly quantized model whose eligible convolutions run on the u8 tensor cores (engine.Executor in inference
-    mode, with those convolutions and the batch norms feeding them lowered to the u8 kernels)."""
+    """A uniformly quantized model whose eligible convolutions run on the u8 kernels: an inference engine.Executor
+    given them as its `int_layers`, whose plan lowers them and the batch norms feeding them to the u8 kernels."""
 
     def __init__(self, graph, images, logits, cfg, state, wlevels, device=None):
         """state: {variable name: fp32 array} of every variable but the integer layers' kernels; wlevels: {conv op
@@ -292,34 +216,15 @@ class IntModel:
         self.state = dict(state)
         bits = cfg['weight_bits']
         byname = {op.name: op for op in compact.reachable_ops(graph, logits)}
-        full = dict(state)
+        full, int_layers = dict(state), {}
         for name, (lv, al, be) in wlevels.items():                 # the executor's copy: the fake-quantized kernel
             full[byname[name].vars['kernel'].name] = dequantize(lv, al, be, bits)
+            int_layers[byname[name]] = (lv, al, be, bits)
         self.device = device or torch.device('cuda', torch.cuda.current_device())
         wq, aq = _specs(graph, cfg, exclude=set(ints))
-        self.ex = ex = Executor(graph, images, logits, self.device, train=False, weight_quant=wq, act_quant=aq)
-        _load(ex, full)
-        u8_readers = {}
-        for name in ints:
-            op = byname[name]
-            u8_readers.setdefault(ex._root(op.inputs[0]).op, []).append(op)
-        for bn, readers in u8_readers.items():
-            if bn in ex.xplanes:     # it writes operand planes: other planes readers, or fp32 readers the plan found
-                fp_readers = [c for c in ex.ops if c in ex.tc and c not in readers
-                              and ex.planes_of(c.inputs[0]) is not None and ex._root(c.inputs[0]).op is bn]
-                others = ex.bn_need_f32[bn] or bool(fp_readers)
-            else:                    # fp32 only (it feeds depthwise layers): does anything but the u8 layers read it?
-                ts = [bn.output] + [c.output for c in ex._consumers(bn.output) if ex.fused_into.get(c) is bn]
-                others = any(c not in readers and ex.fused_into.get(c) is not bn for t in ts for c in ex._consumers(t))
-            ex.batch_norm[bn] = _U8Bn(ex, bn, ex.batch_norm[bn], others)
-        for name in ints:
-            op = byname[name]
-            lv, al, be = wlevels[name]
-            bn = ex.batch_norm[ex._root(op.inputs[0]).op]
-            if op.type == 'DepthwiseConv2dNative':
-                ex.dwconv[op] = _U8DwConv(ex, op, bn, lv, al, be, bits)
-            else:
-                ex.conv[op] = _U8Conv(ex, op, bn, lv, al, be, bits)
+        self.ex = Executor(graph, images, logits, self.device, train=False, weight_quant=wq, act_quant=aq,
+                           int_layers=int_layers)
+        _load(self.ex, full)
 
     @classmethod
     def from_checkpoint(cls, graph, images, logits, state, cfg, device=None):

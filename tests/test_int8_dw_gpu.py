@@ -177,17 +177,20 @@ def _learner_state(flags):
 
 @pytest.mark.parametrize('flags', [dict(), dict(uql_use_buckets=True, uql_bucket_type='channel')],
                          ids=['per_layer', 'channel_buckets'])
-def test_int_model_dw_against_oracle(flags, tmp_path):
+def test_int_model_planned_dw_against_oracle(flags, tmp_path):
+    """the executor's plan lowers all 13 depthwise layers to pf_dwconv_u8_fwd; distance to the float64 oracle, top-1
+    agreement with fake-quant and a bit-identical export / load"""
     from oracle.step_oracle import StepOracle
     from pocketflow_b200 import compact, int8
+    from pocketflow_b200.engine import _U8DwConv
     state = _learner_state(flags)
     g, images, logits, cfg = _model(32, flags)
     dev = torch.device('cuda', 0)
     im = int8.IntModel.from_checkpoint(g, images, logits, state, cfg, dev)
     dws = [op for op in im.ex.ops if op.type == 'DepthwiseConv2dNative']
-    assert len(dws) == 13 and set(im.ex.dwconv) == set(dws)
+    assert len(dws) == 13 and all(isinstance(im.ex.depthwise[op], _U8DwConv) for op in dws)
     for op in dws:                       # the producers feeding only u8 layers no longer write the fp32 tensor
-        assert im.ex.dwconv[op].bn.others is False, op.name
+        assert im.ex.depthwise[op].bn.others is False, op.name
     full = compact.map_state(g, compact.reachable_ops(g, logits), state)
     fq = int8.fake_quant_executor(g, images, logits, full, cfg, dev)
     x = torch.randn(images.shape, generator=torch.Generator().manual_seed(1)).to(dev)
@@ -214,5 +217,5 @@ def test_int_model_dw_against_oracle(flags, tmp_path):
         rec = json.load(f)
     assert rec['version'] == int8.SIDECAR_VERSION == 2 and rec['config']['int8_depthwise'] is True
     im2 = int8.IntModel.load(g, images, logits, str(tmp_path / 'int8'), dev)
-    assert {op.name for op in im2.ex.dwconv} == {op.name for op in dws}
+    assert {op.name for op, lo in im2.ex.depthwise.items() if isinstance(lo, _U8DwConv)} == {op.name for op in dws}
     assert torch.equal(im2.forward(x), li)

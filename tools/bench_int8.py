@@ -78,7 +78,7 @@ def main(argv=None):
     fq_conv = {op.name: lo for op, lo in fq.conv.items()}
     rows, tot = [], dict(u8=0.0, fq=0.0, bound=0.0)
     for op, lo in im.ex.conv.items():
-        if not isinstance(lo, int8._U8Conv):
+        if op not in im.ex.int_layers:
             continue
         d = lo.d
         m, k, n = d.n * d.p * d.q, d.r * d.s * d.c, d.k
@@ -97,7 +97,9 @@ def main(argv=None):
     print('all %d u8 layers: u8 %.3f ms, fake-quant %.3f ms, bound %.3f ms' % (len(rows), tot['u8'], tot['fq'],
                                                                               tot['bound']))
     dw_rows, dw_tot = [], dict(u8=0.0, fp32=0.0, bound=0.0, fp32_bound=0.0)
-    for op, lo in im.ex.dwconv.items():
+    for op, lo in im.ex.depthwise.items():
+        if op not in im.ex.int_layers:
+            continue
         d = lo.d
         nin, nout = d.n * d.h * d.w * d.c, d.n * d.p * d.q * d.c
         bound = (nin + d.r * d.s * d.c + 4 * nout) / HBM_BYTES_PER_S * 1e3
