@@ -200,6 +200,7 @@ def conv64(x, w, d):
     pb, pr = (p - 1) * sh + r - h - pt, (q - 1) * sw + s - wd - pl      # negative: rows / columns no window reaches
     xp = F.pad(x.permute(0, 3, 1, 2), (pl, pr, pt, pb))
     cols = F.unfold(xp, (r, s), stride=(sh, sw))                          # [n, c*r*s, p*q], channel-major
+    k = w.shape[-1]                                                       # w may have fewer output channels than d
     wm = w.permute(3, 2, 0, 1).reshape(k, c * r * s)
     return (wm @ cols).view(n, k, p, q).permute(0, 2, 3, 1)
 
@@ -2367,3 +2368,115 @@ def expected_contributions(ex, t, memo):
         s.add('loss')
     memo[t] = s
     return s
+
+
+# ---------------------------------------------------------------------------------------------- integer models
+# The four integer inference models (int8.IntModel): network module, its flags, the int8 options.  The weight buckets
+# are per channel on the ResNets and per layer on the MobileNets, so both forms of the weight scales run.
+INT8_MODELS = {
+    'resnet20_narrow': ('resnet_at_cifar10', dict(resnet_size=20, uql_use_buckets=True, uql_bucket_type='channel'),
+                        dict(int8_narrow=True)),
+    'resnet50': ('resnet_at_ilsvrc12', dict(resnet_size=50, uql_use_buckets=True, uql_bucket_type='channel'), {}),
+    'mobilenet_v1_depthwise': ('mobilenet_at_ilsvrc12', {}, dict(int8_depthwise=True)),
+    'mobilenet_v2_depthwise_narrow': ('mobilenet_at_ilsvrc12', dict(mobilenet_version=2, nb_classes=1001),
+                                      dict(int8_depthwise=True, int8_narrow=True)),
+}
+
+# Every integer layer of those models, in graph order of first appearance: (kind, H, W, Cin, Cout, R, S, stride,
+# pad top, pad left, P, Q, kernel, layers of that shape).  kind 'conv' runs pf_conv2d_u8_fwd on its TMA-fed kernel
+# ('tma', where pf_conv2d_u8_supported holds) or its cp.async-fed one ('cp.async'); kind 'dw' runs pf_dwconv_u8_fwd
+# on its row-blocked kernel ('rows': 3 x 3, equal strides, P >= 2) or its one-pixel kernel ('pixel').  The shapes do
+# not depend on the batch.  tests/test_int8_edges_cpu.py checks these lists against int8.select on the graphs, and
+# the kernel tests parametrize over them.
+INT8_LAYERS = {
+    'resnet20_narrow': [
+        ('conv', 32, 32, 16, 16, 1, 1, 1, 0, 0, 32, 32, 'cp.async', 1),
+        ('conv', 32, 32, 16, 16, 3, 3, 1, 1, 1, 32, 32, 'cp.async', 6),
+        ('conv', 32, 32, 16, 32, 1, 1, 2, 0, 0, 16, 16, 'cp.async', 1),
+        ('conv', 32, 32, 16, 32, 3, 3, 2, 1, 1, 16, 16, 'cp.async', 1),
+        ('conv', 16, 16, 32, 32, 3, 3, 1, 1, 1, 16, 16, 'cp.async', 5),
+        ('conv', 16, 16, 32, 64, 1, 1, 2, 0, 0, 8, 8, 'cp.async', 1),
+        ('conv', 16, 16, 32, 64, 3, 3, 2, 1, 1, 8, 8, 'cp.async', 1),
+        ('conv', 8, 8, 64, 64, 3, 3, 1, 1, 1, 8, 8, 'tma', 5),
+    ],
+    'resnet50': [
+        ('conv', 56, 56, 64, 256, 1, 1, 1, 0, 0, 56, 56, 'tma', 4),
+        ('conv', 56, 56, 64, 64, 1, 1, 1, 0, 0, 56, 56, 'tma', 1),
+        ('conv', 56, 56, 64, 64, 3, 3, 1, 1, 1, 56, 56, 'tma', 3),
+        ('conv', 56, 56, 256, 64, 1, 1, 1, 0, 0, 56, 56, 'tma', 2),
+        ('conv', 56, 56, 256, 512, 1, 1, 2, 0, 0, 28, 28, 'tma', 1),
+        ('conv', 56, 56, 256, 128, 1, 1, 1, 0, 0, 56, 56, 'tma', 1),
+        ('conv', 56, 56, 128, 128, 3, 3, 2, 1, 1, 28, 28, 'tma', 1),
+        ('conv', 28, 28, 128, 512, 1, 1, 1, 0, 0, 28, 28, 'tma', 4),
+        ('conv', 28, 28, 512, 128, 1, 1, 1, 0, 0, 28, 28, 'tma', 3),
+        ('conv', 28, 28, 128, 128, 3, 3, 1, 1, 1, 28, 28, 'tma', 3),
+        ('conv', 28, 28, 512, 1024, 1, 1, 2, 0, 0, 14, 14, 'tma', 1),
+        ('conv', 28, 28, 512, 256, 1, 1, 1, 0, 0, 28, 28, 'tma', 1),
+        ('conv', 28, 28, 256, 256, 3, 3, 2, 1, 1, 14, 14, 'tma', 1),
+        ('conv', 14, 14, 256, 1024, 1, 1, 1, 0, 0, 14, 14, 'tma', 6),
+        ('conv', 14, 14, 1024, 256, 1, 1, 1, 0, 0, 14, 14, 'tma', 5),
+        ('conv', 14, 14, 256, 256, 3, 3, 1, 1, 1, 14, 14, 'tma', 5),
+        ('conv', 14, 14, 1024, 2048, 1, 1, 2, 0, 0, 7, 7, 'tma', 1),
+        ('conv', 14, 14, 1024, 512, 1, 1, 1, 0, 0, 14, 14, 'tma', 1),
+        ('conv', 14, 14, 512, 512, 3, 3, 2, 1, 1, 7, 7, 'tma', 1),
+        ('conv', 7, 7, 512, 2048, 1, 1, 1, 0, 0, 7, 7, 'tma', 3),
+        ('conv', 7, 7, 2048, 512, 1, 1, 1, 0, 0, 7, 7, 'tma', 2),
+        ('conv', 7, 7, 512, 512, 3, 3, 1, 1, 1, 7, 7, 'tma', 2),
+    ],
+    'mobilenet_v1_depthwise': [
+        ('dw', 112, 112, 32, 32, 3, 3, 1, 1, 1, 112, 112, 'rows', 1),
+        ('dw', 112, 112, 64, 64, 3, 3, 2, 0, 0, 56, 56, 'rows', 1),
+        ('conv', 56, 56, 64, 128, 1, 1, 1, 0, 0, 56, 56, 'tma', 1),
+        ('dw', 56, 56, 128, 128, 3, 3, 1, 1, 1, 56, 56, 'rows', 1),
+        ('conv', 56, 56, 128, 128, 1, 1, 1, 0, 0, 56, 56, 'tma', 1),
+        ('dw', 56, 56, 128, 128, 3, 3, 2, 0, 0, 28, 28, 'rows', 1),
+        ('conv', 28, 28, 128, 256, 1, 1, 1, 0, 0, 28, 28, 'tma', 1),
+        ('dw', 28, 28, 256, 256, 3, 3, 1, 1, 1, 28, 28, 'rows', 1),
+        ('conv', 28, 28, 256, 256, 1, 1, 1, 0, 0, 28, 28, 'tma', 1),
+        ('dw', 28, 28, 256, 256, 3, 3, 2, 0, 0, 14, 14, 'rows', 1),
+        ('conv', 14, 14, 256, 512, 1, 1, 1, 0, 0, 14, 14, 'tma', 1),
+        ('dw', 14, 14, 512, 512, 3, 3, 1, 1, 1, 14, 14, 'rows', 5),
+        ('conv', 14, 14, 512, 512, 1, 1, 1, 0, 0, 14, 14, 'tma', 5),
+        ('dw', 14, 14, 512, 512, 3, 3, 2, 0, 0, 7, 7, 'rows', 1),
+        ('conv', 7, 7, 512, 1024, 1, 1, 1, 0, 0, 7, 7, 'tma', 1),
+        ('dw', 7, 7, 1024, 1024, 3, 3, 1, 1, 1, 7, 7, 'rows', 1),
+        ('conv', 7, 7, 1024, 1024, 1, 1, 1, 0, 0, 7, 7, 'tma', 1),
+    ],
+    'mobilenet_v2_depthwise_narrow': [
+        ('dw', 112, 112, 32, 32, 3, 3, 1, 1, 1, 112, 112, 'rows', 1),
+        ('conv', 112, 112, 32, 16, 1, 1, 1, 0, 0, 112, 112, 'cp.async', 1),
+        ('dw', 112, 112, 96, 96, 3, 3, 2, 0, 0, 56, 56, 'rows', 1),
+        ('dw', 56, 56, 144, 144, 3, 3, 1, 1, 1, 56, 56, 'rows', 1),
+        ('dw', 56, 56, 144, 144, 3, 3, 2, 0, 0, 28, 28, 'rows', 1),
+        ('conv', 28, 28, 144, 32, 1, 1, 1, 0, 0, 28, 28, 'cp.async', 1),
+        ('dw', 28, 28, 192, 192, 3, 3, 1, 1, 1, 28, 28, 'rows', 2),
+        ('conv', 28, 28, 192, 32, 1, 1, 1, 0, 0, 28, 28, 'cp.async', 2),
+        ('dw', 28, 28, 192, 192, 3, 3, 2, 0, 0, 14, 14, 'rows', 1),
+        ('conv', 14, 14, 192, 64, 1, 1, 1, 0, 0, 14, 14, 'tma', 1),
+        ('dw', 14, 14, 384, 384, 3, 3, 1, 1, 1, 14, 14, 'rows', 4),
+        ('conv', 14, 14, 384, 64, 1, 1, 1, 0, 0, 14, 14, 'tma', 3),
+        ('conv', 14, 14, 384, 96, 1, 1, 1, 0, 0, 14, 14, 'cp.async', 1),
+        ('dw', 14, 14, 576, 576, 3, 3, 1, 1, 1, 14, 14, 'rows', 2),
+        ('conv', 14, 14, 576, 96, 1, 1, 1, 0, 0, 14, 14, 'cp.async', 2),
+        ('dw', 14, 14, 576, 576, 3, 3, 2, 0, 0, 7, 7, 'rows', 1),
+        ('conv', 7, 7, 576, 160, 1, 1, 1, 0, 0, 7, 7, 'cp.async', 1),
+        ('dw', 7, 7, 960, 960, 3, 3, 1, 1, 1, 7, 7, 'rows', 3),
+        ('conv', 7, 7, 960, 160, 1, 1, 1, 0, 0, 7, 7, 'cp.async', 2),
+        ('conv', 7, 7, 960, 320, 1, 1, 1, 0, 0, 7, 7, 'tma', 1),
+    ],
+}
+
+
+def int8_graph(key, batch, weight_bits=8, activation_bits=8):
+    """(graph, images, logits, int8 config) of INT8_MODELS[key]'s inference graph at `batch`, with FLAGS set as the
+    uniform learner of that model would have them"""
+    from pocketflow_b200 import int8
+    net, flags, opts = INT8_MODELS[key]
+    mod = importlib.import_module('pocketflow_b200.nets.' + net)
+    importlib.import_module('pocketflow_b200.learners.uniform_quantization.learner')
+    FLAGS.reset()
+    for k, v in flags.items():
+        setattr(FLAGS, k, v)
+    FLAGS.uql_weight_bits, FLAGS.uql_activation_bits = weight_bits, activation_bits
+    g, images, logits = C.build_eval_graph(mod.ModelHelper(), batch)
+    return g, images, logits, dict(int8.config_from_flags(), **opts)
