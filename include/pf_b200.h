@@ -116,6 +116,10 @@ int pf_uq_act_quant(const float* x_dev, float* y_dev, int64_t n, const uint32_t*
 /* same, (also) writing y as split-bf16 planes for the tensor-core conv that consumes it (y_dev may be NULL) */
 int pf_uq_act_quant_planes(const float* x_dev, float* y_dev, void* y_hi_dev, void* y_lo_dev, int64_t n,
                            const uint32_t* minmax_enc_dev, int bits, void* stream);
+/* static range (a calibrated model): y = Q(clamp(x, lo, hi)) with range_enc_dev[0..1] = the encoded lo / hi, written
+ * once by the caller; one pass, no range pass.  Bit-identical to pf_uq_act_quant when lo / hi is x's own range. */
+int pf_uq_act_quant_static(const float* x_dev, float* y_dev, int64_t n, const uint32_t* range_enc_dev, int bits,
+                           void* stream);
 
 int pf_fill_u32(uint32_t* p_dev, int64_t n, uint32_t value, void* stream);
 /* (min,max) ordered-uint pairs <- (0xFFFFFFFF, 0): one launch resets every activation range slot. */
@@ -476,6 +480,14 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
                          float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
                          uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
                          float* csum_dev, void* stream);
+/* the same producer with a static (calibrated) range in range_enc_dev[0..1] (ordered-uint lo / hi, read only): y is
+ * clamped to [lo, hi] and quantized with lo / hi in place of the batch's min / max, in ONE pass with no atomics (4 B
+ * read + 1 B written per element).  Levels, csum and header equal pf_bn_eval_levels_u8's whenever lo / hi is the
+ * batch's range of y.  Same shapes, bits and alignments as pf_bn_eval_levels_u8. */
+int pf_bn_eval_levels_u8_static(const float* x_dev, int64_t m, int c, const float* moving_mean_dev,
+                                const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev,
+                                int act, int bits, const uint32_t* range_enc_dev, void* levels_dev,
+                                pf_tc_act_hdr* hdr_dev, float* csum_dev, void* stream);
 /* host-side decisions of the most recent tensor-core conv launch (fwd / dgrad / wgrad, either feed), recorded by the
  * launcher from the values it launches with, so that tests can tell which kernel variant a call exercised.  One
  * process-wide record, not synchronised: read it from the thread that launched.  Returns PF_ERR_INVALID_ARG when
@@ -576,6 +588,13 @@ int pf_bn_eval_prepare(const float* moving_var_dev, int c, float eps, float* rst
 int pf_bn_apply_eval(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
                      float eps, const float* gamma_dev, const float* beta_dev, int act, float* y_dev, void* y_hi_dev,
                      void* y_lo_dev, uint32_t* minmax_enc_dev, void* stream);
+/* inference-mode BN + act + fake-quant with a static (calibrated) range in one pass: y = Q(clamp(act(bn(x)), lo, hi))
+ * with range_enc_dev[0..1] = the encoded lo / hi; fp32 and/or split-bf16 planes.  Bit-identical to pf_bn_apply_eval
+ * followed by pf_uq_act_quant(_planes) when lo / hi is the batch's range of act(bn(x)). */
+int pf_bn_apply_eval_quant_static(const float* x_dev, int64_t m, int c, const float* moving_mean_dev,
+                                  const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev,
+                                  int act, const uint32_t* range_enc_dev, int bits, float* y_dev, void* y_hi_dev,
+                                  void* y_lo_dev, void* stream);
 /* y = Q(act(bn(x))) in one pass with a known range (pf_bn_train_stats_range): fp32 and/or split-bf16 planes */
 int pf_bn_apply_quant(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
                       const float* gamma_dev, const float* beta_dev, int act, const uint32_t* range_enc_dev, int bits,

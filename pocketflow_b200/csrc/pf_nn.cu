@@ -189,7 +189,9 @@ bn_eval_prepare_kernel(const float* __restrict__ mov_var, int C, float eps, floa
 // RES: y = bn(x) + res — a linear-bottleneck BN (no activation) feeding a residual Add (MobileNet-v2,
 // conv_blocks.py:289-313) in one pass; the add is one more correctly rounded step after the BN chain, so the result is
 // bit-identical to BN apply followed by pf_add.  8 B/element read (x, res) instead of 4 + 8 + 8 for the three passes.
-template <bool RES>
+// CLAMP (static range, pf_bn_apply_eval_quant_static): act(bn(x)) is clamped to [min, max] of q_range before the
+// fake-quant, so values outside a calibrated range take its end levels; inside it the result is the unclamped one.
+template <bool RES, bool CLAMP = false>
 __global__ void __launch_bounds__(NT)
 bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* __restrict__ mean,
                 const float* __restrict__ rstd, const float* __restrict__ gamma,
@@ -200,9 +202,10 @@ bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* 
   // same two roundings as bn_eval_prepare_kernel, one launch less per layer)
   __shared__ float s_mn[NT / 32], s_mx[NT / 32];
   // fused activation fake-quant (range known beforehand: pf_bn_train_stats_range)
-  float q_alpha = 1.f, q_beta = 0.f, q_k = 1.f, q_ra = 1.f, q_rk = 1.f;
+  float q_alpha = 1.f, q_beta = 0.f, q_k = 1.f, q_ra = 1.f, q_rk = 1.f, q_hi = 0.f;
   if (q_range) {
     const float qmn = pf_dec(__ldg(q_range)), qmx = pf_dec(__ldg(q_range + 1));
+    q_hi = qmx;
     q_alpha = __fadd_rn(__fsub_rn(qmx, qmn), 1e-10f);
     q_beta = qmn;
     q_k = pf_uq_kf(q_bits);
@@ -225,6 +228,10 @@ bn_apply_kernel(const float* __restrict__ x, int64_t total, int C, const float* 
       v.x = __fadd_rn(v.x, r.x); v.y = __fadd_rn(v.y, r.y); v.z = __fadd_rn(v.z, r.z); v.w = __fadd_rn(v.w, r.w);
     }
     if (q_range) {
+      if (CLAMP) {
+        v.x = pf_clamp(v.x, q_beta, q_hi); v.y = pf_clamp(v.y, q_beta, q_hi);
+        v.z = pf_clamp(v.z, q_beta, q_hi); v.w = pf_clamp(v.w, q_beta, q_hi);
+      }
       v.x = pf_fake_quant(v.x, q_alpha, q_beta, q_k, q_ra, q_rk);
       v.y = pf_fake_quant(v.y, q_alpha, q_beta, q_k, q_ra, q_rk);
       v.z = pf_fake_quant(v.z, q_alpha, q_beta, q_k, q_ra, q_rk);
@@ -387,7 +394,10 @@ bn_apply_levels_kernel(const float* __restrict__ x, int64_t total, int C, int cs
 // pf_bn_apply_eval accumulates it), then the levels.  A range that does not start at 0 (an activation offset the u8
 // convolution has no term for) is recorded as header {1, 0}.  Channel-stationary grid (host: chan_grid), C a power of
 // two >= 16.  HBM traffic: 4 B read per element and pass, 1 B written.
-template <bool RANGE>
+// CLAMP (pf_bn_eval_levels_u8_static): range_enc holds a calibrated range and only the level pass runs; y is clamped
+// to it first (a value above max gets level k), so with the batch's own range the levels and sums are these.  4 B read
+// and 1 B written per element, no atomics.
+template <bool RANGE, bool CLAMP = false>
 __global__ void __launch_bounds__(NT)
 bn_eval_levels_u8_kernel(const float* __restrict__ x, int64_t total, int C, int cshift, const float* __restrict__ mean,
                          const float* __restrict__ var, float eps, const float* __restrict__ gamma,
@@ -449,7 +459,11 @@ bn_eval_levels_u8_kernel(const float* __restrict__ x, int64_t total, int C, int 
     const bool valid = i < nvec;
     float part = 0.f;
     if (valid) {
-      const float4 y = bn4(pf_ld_stream(x + (i << 2)));
+      float4 y = bn4(pf_ld_stream(x + (i << 2)));
+      if (CLAMP) {
+        y.x = pf_clamp(y.x, qmn, qmx); y.y = pf_clamp(y.y, qmn, qmx);
+        y.z = pf_clamp(y.z, qmn, qmx); y.w = pf_clamp(y.w, qmn, qmx);
+      }
       const float lx = pf_quant_level(y.x, q_alpha, qmn, q_k, q_ra), ly = pf_quant_level(y.y, q_alpha, qmn, q_k, q_ra);
       const float lz = pf_quant_level(y.z, q_alpha, qmn, q_k, q_ra), lw = pf_quant_level(y.w, q_alpha, qmn, q_k, q_ra);
       *reinterpret_cast<uint32_t*>(levels + (i << 2)) =
@@ -469,8 +483,9 @@ bn_eval_levels_u8_kernel(const float* __restrict__ x, int64_t total, int C, int 
 // of 8 lanes of 16 channels each (lanes past C idle); a lane reads 64 bytes, writes 16 bytes of levels (as two 8-byte stores), and the group's
 // level sum is a 3-step xor butterfly (integers below 2^24: exact).  The item index is the csum index.  Segment-
 // stationary grid: the number of groups is a multiple of nseg (host: seg_grid), so every lane keeps its 16 channels
-// and their batch-norm constants.  The levels are pf_quant_level of the same values as in bn_eval_levels_u8_kernel.
-template <bool RANGE>
+// and their batch-norm constants.  The levels are pf_quant_level of the same values as in bn_eval_levels_u8_kernel
+// (CLAMP as there).
+template <bool RANGE, bool CLAMP = false>
 __global__ void __launch_bounds__(NT)
 bn_eval_levels_u8_seg_kernel(const float* __restrict__ x, int64_t items, int C, int nseg, const float* __restrict__ mean,
                              const float* __restrict__ var, float eps, const float* __restrict__ gamma,
@@ -547,6 +562,10 @@ bn_eval_levels_u8_seg_kernel(const float* __restrict__ x, int64_t items, int C, 
     if (i < items && cok) {
       float y[16];
       load_bn(i, y);
+      if (CLAMP) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) y[j] = pf_clamp(y[j], qmn, qmx);
+      }
       uint32_t w[4];
 #pragma unroll
       for (int v = 0; v < 4; ++v) {
@@ -1096,7 +1115,7 @@ int pf_bn_eval_prepare(const float* moving_var_dev, int c, float eps, float* rst
 static int bn_apply_impl(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
                          const float* gamma_dev, const float* beta_dev, int act, float* y_dev, void* y_hi_dev,
                          void* y_lo_dev, uint32_t* minmax_enc_dev, const uint32_t* q_range_dev, int q_bits, void* stream,
-                         float var_eps = -1.f, const float* res_dev = nullptr) {
+                         float var_eps = -1.f, const float* res_dev = nullptr, bool clamp = false) {
   PF_REQUIRE(m > 0 && c > 0 && (c & 3) == 0, "pf_bn_apply: bad shape (C must be a multiple of 4)");
   PF_REQUIRE(act >= 0 && act <= 2, "pf_bn_apply: act must be 0 (none), 1 (relu) or 2 (relu6)");
   PF_REQUIRE(x_dev && mean_dev && rstd_dev && gamma_dev && beta_dev, "pf_bn_apply: null pointer");
@@ -1105,7 +1124,11 @@ static int bn_apply_impl(const float* x_dev, int64_t m, int c, const float* mean
   PF_REQUIRE((((uintptr_t)y_hi_dev | (uintptr_t)y_lo_dev) & 7) == 0, "pf_bn_apply: planes must be 8-byte aligned");
   const int64_t total = m * c;
   const unsigned grid = chan_grid(total >> 2, c);
-  if (res_dev)
+  if (clamp)
+    bn_apply_kernel<false, true><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, total, c, mean_dev, rstd_dev, gamma_dev, beta_dev,
+                                                                        act, y_dev, nullptr, y_hi_dev, y_lo_dev, q_range_dev,
+                                                                        q_bits, var_eps, nullptr);
+  else if (res_dev)
     bn_apply_kernel<true><<<grid, NT, 0, (cudaStream_t)stream>>>(x_dev, total, c, mean_dev, rstd_dev, gamma_dev, beta_dev, act,
                                                                  y_dev, minmax_enc_dev, y_hi_dev, y_lo_dev, q_range_dev, q_bits,
                                                                  var_eps, res_dev);
@@ -1130,6 +1153,17 @@ int pf_bn_apply_eval(const float* x_dev, int64_t m, int c, const float* moving_m
   PF_REQUIRE(eps >= 0.f, "pf_bn_apply_eval: eps < 0");
   return bn_apply_impl(x_dev, m, c, moving_mean_dev, moving_var_dev, gamma_dev, beta_dev, act, y_dev, y_hi_dev, y_lo_dev,
                        minmax_enc_dev, nullptr, 0, stream, eps);
+}
+
+int pf_bn_apply_eval_quant_static(const float* x_dev, int64_t m, int c, const float* moving_mean_dev,
+                                  const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev,
+                                  int act, const uint32_t* range_enc_dev, int bits, float* y_dev, void* y_hi_dev,
+                                  void* y_lo_dev, void* stream) {
+  PF_REQUIRE(eps >= 0.f, "pf_bn_apply_eval_quant_static: eps < 0");
+  PF_REQUIRE(range_enc_dev != nullptr, "pf_bn_apply_eval_quant_static: null range");
+  PF_REQUIRE(bits >= 1 && bits <= 32, "pf_bn_apply_eval_quant_static: bits must be in [1, 32]");
+  return bn_apply_impl(x_dev, m, c, moving_mean_dev, moving_var_dev, gamma_dev, beta_dev, act, y_dev, y_hi_dev, y_lo_dev,
+                       nullptr, range_enc_dev, bits, stream, eps, nullptr, true);
 }
 
 int pf_bn_apply_quant(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,
@@ -1171,11 +1205,12 @@ int pf_bn_apply_quant_levels(const float* x_dev, int64_t m, int c, const float* 
   return PF_OK;
 }
 
-int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
-                         float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
-                         uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
-                         float* csum_dev, void* stream) {
-  const char* who = "pf_bn_eval_levels_u8";
+// have_range: 0 = reset range_enc and run the range pass first, 1 = range_enc holds this batch's range, 2 = it holds
+// a calibrated range (the clamping level pass only)
+static int bn_eval_levels_u8_impl(const char* who, const float* x_dev, int64_t m, int c, const float* moving_mean_dev,
+                                  const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev,
+                                  int act, int bits, uint32_t* range_enc_dev, int have_range, void* levels_dev,
+                                  pf_tc_act_hdr* hdr_dev, float* csum_dev, void* stream) {
   PF_REQUIRE(m > 0 && c >= 16 && c % 16 == 0, "%s: C must be a multiple of 16 (got %d)", who, c);
   PF_REQUIRE(act >= 0 && act <= 2, "%s: act must be 0 (none), 1 (relu) or 2 (relu6)", who);
   PF_REQUIRE(bits >= 1 && bits <= 8, "%s: u8 levels need 1..8 bits", who);
@@ -1195,6 +1230,13 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
     int64_t grid = std::min((items * 8 + NT - 1) / NT, (int64_t)PF_NUM_SMS * bn_grid_cap());
     const int64_t mult = nseg / std::gcd(nseg, NT / 8);
     grid = std::max<int64_t>(1, (grid + mult - 1) / mult) * mult;
+    if (have_range == 2) {
+      bn_eval_levels_u8_seg_kernel<false, true><<<(unsigned)grid, NT, 0, st>>>(x_dev, items, c, nseg, moving_mean_dev,
+                                                                               moving_var_dev, eps, gamma_dev, beta_dev, act,
+                                                                               range_enc_dev, bits, lv, hdr_dev, csum_dev);
+      PF_CHECK_LAUNCH(who);
+      return PF_OK;
+    }
     if (!have_range) {
       const int rc = pf_minmax_reset(range_enc_dev, 1, stream);
       if (rc) return rc;
@@ -1213,6 +1255,13 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
   while ((1 << cshift) < c) ++cshift;
   const unsigned grid = chan_grid(total >> 2, c);
   PF_REQUIRE(((int64_t)grid * NT) % (c >> 2) == 0, "%s: C = %d too large for the channel-stationary grid", who, c);
+  if (have_range == 2) {
+    bn_eval_levels_u8_kernel<false, true><<<grid, NT, 0, st>>>(x_dev, total, c, cshift, moving_mean_dev, moving_var_dev,
+                                                               eps, gamma_dev, beta_dev, act, range_enc_dev, bits, lv,
+                                                               hdr_dev, csum_dev, nseg);
+    PF_CHECK_LAUNCH(who);
+    return PF_OK;
+  }
   if (!have_range) {
     const int rc = pf_minmax_reset(range_enc_dev, 1, stream);
     if (rc) return rc;
@@ -1226,6 +1275,25 @@ int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* movi
                                                        nseg);
   PF_CHECK_LAUNCH(who);
   return PF_OK;
+}
+
+int pf_bn_eval_levels_u8(const float* x_dev, int64_t m, int c, const float* moving_mean_dev, const float* moving_var_dev,
+                         float eps, const float* gamma_dev, const float* beta_dev, int act, int bits,
+                         uint32_t* range_enc_dev, int have_range, void* levels_dev, pf_tc_act_hdr* hdr_dev,
+                         float* csum_dev, void* stream) {
+  return bn_eval_levels_u8_impl("pf_bn_eval_levels_u8", x_dev, m, c, moving_mean_dev, moving_var_dev, eps, gamma_dev,
+                                beta_dev, act, bits, range_enc_dev, have_range ? 1 : 0, levels_dev, hdr_dev, csum_dev,
+                                stream);
+}
+
+int pf_bn_eval_levels_u8_static(const float* x_dev, int64_t m, int c, const float* moving_mean_dev,
+                                const float* moving_var_dev, float eps, const float* gamma_dev, const float* beta_dev,
+                                int act, int bits, const uint32_t* range_enc_dev, void* levels_dev,
+                                pf_tc_act_hdr* hdr_dev, float* csum_dev, void* stream) {
+  // the kernels read range_enc only in the level pass (have_range 2 launches no other)
+  return bn_eval_levels_u8_impl("pf_bn_eval_levels_u8_static", x_dev, m, c, moving_mean_dev, moving_var_dev, eps,
+                                gamma_dev, beta_dev, act, bits, const_cast<uint32_t*>(range_enc_dev), 2, levels_dev,
+                                hdr_dev, csum_dev, stream);
 }
 
 int pf_bn_apply_add(const float* x_dev, int64_t m, int c, const float* mean_dev, const float* rstd_dev,

@@ -245,10 +245,13 @@ uq_act_minmax_kernel(const float* __restrict__ x, int64_t n, uint32_t* __restric
   block_minmax_to_slot(mn, mx, minmax_enc, minmax_enc + 1);
 }
 
+// CLAMP (pf_uq_act_quant_static): minmax_enc holds a calibrated range and x is clamped to it before the quantizer.
+template <bool CLAMP = false>
 __global__ void __launch_bounds__(kThreads)
 uq_act_quant_kernel(const float* x, float* y, int64_t n, const uint32_t* __restrict__ minmax_enc,
                     int bits, void* __restrict__ y_hi, void* __restrict__ y_lo) {
   const float mn = pf_dec(__ldg(minmax_enc)), mx = pf_dec(__ldg(minmax_enc + 1));
+  auto in = [&](float v) { return CLAMP ? pf_clamp(v, mn, mx) : v; };
   const float alpha = __fadd_rn(__fsub_rn(mx, mn), 1e-10f);
   const float k = pf_uq_kf(bits);
   const float ra = __frcp_rn(alpha), rk = __frcp_rn(k);
@@ -261,26 +264,26 @@ uq_act_quant_kernel(const float* x, float* y, int64_t n, const uint32_t* __restr
     for (int u = 0; u < kActUnroll; ++u) v[u] = pf_ld4(x + ((i + u * stride) << 2));
 #pragma unroll
     for (int u = 0; u < kActUnroll; ++u) {
-      v[u].x = pf_fake_quant(v[u].x, alpha, mn, k, ra, rk);
-      v[u].y = pf_fake_quant(v[u].y, alpha, mn, k, ra, rk);
-      v[u].z = pf_fake_quant(v[u].z, alpha, mn, k, ra, rk);
-      v[u].w = pf_fake_quant(v[u].w, alpha, mn, k, ra, rk);
+      v[u].x = pf_fake_quant(in(v[u].x), alpha, mn, k, ra, rk);
+      v[u].y = pf_fake_quant(in(v[u].y), alpha, mn, k, ra, rk);
+      v[u].z = pf_fake_quant(in(v[u].z), alpha, mn, k, ra, rk);
+      v[u].w = pf_fake_quant(in(v[u].w), alpha, mn, k, ra, rk);
       if (y) pf_st_stream(y + ((i + u * stride) << 2), v[u]);
       if (y_hi) pf_st_planes4(y_hi, y_lo, (i + u * stride) << 2, v[u]);
     }
   }
   for (; i < nvec; i += stride) {
     float4 v = pf_ld4(x + (i << 2));
-    v.x = pf_fake_quant(v.x, alpha, mn, k, ra, rk);
-    v.y = pf_fake_quant(v.y, alpha, mn, k, ra, rk);
-    v.z = pf_fake_quant(v.z, alpha, mn, k, ra, rk);
-    v.w = pf_fake_quant(v.w, alpha, mn, k, ra, rk);
+    v.x = pf_fake_quant(in(v.x), alpha, mn, k, ra, rk);
+    v.y = pf_fake_quant(in(v.y), alpha, mn, k, ra, rk);
+    v.z = pf_fake_quant(in(v.z), alpha, mn, k, ra, rk);
+    v.w = pf_fake_quant(in(v.w), alpha, mn, k, ra, rk);
     if (y) pf_st_stream(y + (i << 2), v);
     if (y_hi) pf_st_planes4(y_hi, y_lo, i << 2, v);
   }
   if (y && blockIdx.x == 0 && threadIdx.x < (n & 3)) {
     const int64_t j = (nvec << 2) + threadIdx.x;
-    y[j] = pf_fake_quant(x[j], alpha, mn, k, ra, rk);
+    y[j] = pf_fake_quant(in(x[j]), alpha, mn, k, ra, rk);
   }
 }
 
@@ -362,9 +365,22 @@ int pf_uq_act_quant_planes(const float* x_dev, float* y_dev, void* y_hi_dev, voi
   PF_REQUIRE(y_hi_dev == nullptr || (n & 3) == 0, "pf_uq_act_quant: plane output needs n %% 4 == 0");
   PF_REQUIRE((((uintptr_t)x_dev | (uintptr_t)y_dev) & 15) == 0 && (((uintptr_t)y_hi_dev | (uintptr_t)y_lo_dev) & 7) == 0,
              "pf_uq_act_quant: x and y must be 16-byte aligned (planes: 8)");
-  uq_act_quant_kernel<<<act_grid(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, y_dev, n, minmax_enc_dev, bits,
+  uq_act_quant_kernel<><<<act_grid(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, y_dev, n, minmax_enc_dev, bits,
                                                                          y_hi_dev, y_lo_dev);
   PF_CHECK_LAUNCH("pf_uq_act_quant");
+  return PF_OK;
+}
+
+int pf_uq_act_quant_static(const float* x_dev, float* y_dev, int64_t n, const uint32_t* range_enc_dev, int bits,
+                           void* stream) {
+  PF_REQUIRE(n >= 0, "pf_uq_act_quant_static: n < 0");
+  PF_REQUIRE(bits >= 1 && bits <= 32, "pf_uq_act_quant_static: bits must be in [1, 32]");
+  if (n == 0) return PF_OK;
+  PF_REQUIRE(x_dev && y_dev && range_enc_dev, "pf_uq_act_quant_static: null pointer");
+  PF_REQUIRE((((uintptr_t)x_dev | (uintptr_t)y_dev) & 15) == 0, "pf_uq_act_quant_static: x and y must be 16-byte aligned");
+  uq_act_quant_kernel<true><<<act_grid(n), kThreads, 0, (cudaStream_t)stream>>>(x_dev, y_dev, n, range_enc_dev, bits,
+                                                                               nullptr, nullptr);
+  PF_CHECK_LAUNCH("pf_uq_act_quant_static");
   return PF_OK;
 }
 

@@ -276,18 +276,24 @@ class _BnLowering:
         """the one per-pass choice: batch statistics in training passes of a training-mode BN, else moving statistics"""
         ex, x = self.ex, self.ex.T(self.x)
         batch_stats = self.op.attrs['training'] and training
+        if batch_stats and ex.aq_static and self.slot is not None:
+            # bn_train_stats_range would fold this batch's range into the static range slot, which nothing resets
+            raise RuntimeError('%s: a batch-statistics pass in an executor with static activation ranges' % self.op.name)
         if batch_stats:
             with ex.timed('bn_stats'):
                 (ops.bn_train_stats if self.slot is None else ops.bn_train_stats_range)(x, *self.stats, ex.bn_ws)
         with ex.timed('bn_apply'):
             self._apply(x, batch_stats)
-        if self.slot is not None and not batch_stats:     # the BN apply wrote fp32 (+ range), the quantizer the planes
+        if self.slot is not None and not batch_stats and not ex.aq_static:
+            # the BN apply wrote fp32 (+ range), the quantizer the planes
             with ex.timed('act_quant'):
                 ops.act_quant(self.y, self.y_out, self.slot, ex.act_quant['bits'][self.aq], self.pl)
 
     def _apply(self, x, batch_stats):
         bits = self.ex.act_quant['bits'][self.aq] if self.slot is not None else None
-        if not batch_stats:
+        if not batch_stats and self.slot is not None and self.ex.aq_static:    # calibrated range: one clamping pass
+            ops.bn_apply_eval_quant_static(x, *self.moving, self.act, self.slot, bits, self.y_out, self.pl)
+        elif not batch_stats:
             ops.bn_apply_eval(x, *self.moving, self.act, *self.eval_out)
         elif self.slot is None:
             ops.bn_apply(x, *self.batch, self.act, self.y_out, None, self.pl)
@@ -347,7 +353,8 @@ class _BnFolded(_BnLowering):
 
 class _U8Bn:
     """Inference BN + quantized ReLU that feeds integer layers: writes the u8 levels, header and channel sums they read
-    (pf_bn_eval_levels_u8), after its fake-quant lowering `base` when other readers need the fp32 tensor or planes."""
+    (pf_bn_eval_levels_u8; pf_bn_eval_levels_u8_static in one pass with a calibrated range), after its fake-quant
+    lowering `base` when other readers need the fp32 tensor or planes."""
 
     def __init__(self, ex, op, base):
         self.ex, self.op, self.base, self.others = ex, op, base, ex.u8_others[op]
@@ -360,9 +367,14 @@ class _U8Bn:
         ex, base = self.ex, self.base
         if self.others:
             base.forward(training)
+        x, bits = ex.T(self.op.inputs[0]), ex.act_quant['bits'][base.aq]
         with ex.timed('act_quant'):
-            ops.bn_eval_levels_u8(ex.T(self.op.inputs[0]), *base.moving, base.act, ex.act_quant['bits'][base.aq],
-                                  base.slot, self.levels, self.hdr, self.csum, have_range=self.others)
+            if ex.aq_static:
+                ops.bn_eval_levels_u8_static(x, *base.moving, base.act, bits, base.slot, self.levels, self.hdr,
+                                             self.csum)
+            else:
+                ops.bn_eval_levels_u8(x, *base.moving, base.act, bits, base.slot, self.levels, self.hdr, self.csum,
+                                      have_range=self.others)
 
 
 class ParamStore:
@@ -587,6 +599,15 @@ class Executor:
         self.aq_ops = list(self.act_quant['ops']) if self.act_quant else []
         self.aq_index = {op: i for i, op in enumerate(self.aq_ops)}
         self.aq_slots = torch.zeros(max(len(self.aq_ops), 1), 2, dtype=torch.int32, device=dev)
+        # act_quant['ranges'] (inference only, int8.calibrate): a static (lo, hi) per quantized activation, in the same
+        # slots, written once here; every quantizer then clamps to it in one pass and no range is computed per batch
+        self.aq_static = bool(self.act_quant and self.act_quant.get('ranges') is not None)
+        if self.aq_static:
+            if self.train:
+                raise ValueError('static activation ranges are for inference executors only (train=False)')
+            if len(self.act_quant['ranges']) != len(self.aq_ops):
+                raise ValueError('one activation range per quantized activation expected (%d)' % len(self.aq_ops))
+            self.aq_slots = ops.range_slots(self.act_quant['ranges'], dev)
         self.aq_out = {}           # relu op -> out-of-place quantized buffer (producer is not BN)
         # quantized weights live in a flat buffer with the same offsets as the parameters
         self.QW = torch.zeros(st.n_train, dtype=torch.float32, device=dev) if self.wq_ops else None
@@ -1169,7 +1190,7 @@ class Executor:
     def forward(self, training=None, upto=None):
         """upto: stop after this op has run (its output buffer is the result wanted)."""
         training = self.train if training is None else training
-        if self.aq_ops:
+        if self.aq_ops and not self.aq_static:
             ops.minmax_reset(self.aq_slots)
         if self.wq is not None:
             with self.timed('weight_quant'):
@@ -1204,8 +1225,11 @@ class Executor:
                 if op in self.aq_out:                      # a quantized ReLU whose producer is not a BN
                     y, i = self.buf[self.fused_into[op].output], self.aq_index[op]
                     with self.timed('act_quant'):
-                        ops.act_minmax(y, self.aq_slots[i])
-                        ops.act_quant(y, self.aq_out[op], self.aq_slots[i], self.act_quant['bits'][i])
+                        if self.aq_static:
+                            ops.act_quant_static(y, self.aq_out[op], self.aq_slots[i], self.act_quant['bits'][i])
+                        else:
+                            ops.act_minmax(y, self.aq_slots[i])
+                            ops.act_quant(y, self.aq_out[op], self.aq_slots[i], self.act_quant['bits'][i])
             elif ty == 'MaxPool':
                 with self.timed('pool'):
                     ops.maxpool_fwd(self.desc[op], self.T(op.inputs[0]), self.buf[op.output], self.pool_argmax.get(op))

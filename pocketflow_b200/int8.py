@@ -31,7 +31,16 @@ projections then run on integers.  The sidecar records the option in its config 
 depthwise integer layers): a loader that does not know the option selects fewer integer layers than the file holds
 levels for, and IntModel refuses that with its coverage ValueError instead of building a different model.
 
-select() decides from the graph alone.  IntModel hands the selected layers and their weight levels to the executor
+Calibrated activation ranges (opt-in): `calibrate` runs the fake-quantized model over a few batches and returns a
+static (lo, hi) per quantized activation, the float64 mean of the per-batch min / max ('mean', the default: the learner
+trained with per-batch ranges) or their extremes ('max').  With `act_ranges`, every quantized activation of the model is
+clamped to its range and quantized with lo / hi in place of the batch's min / max, in one pass: the u8 level producer
+(pf_bn_eval_levels_u8_static) and the fake-quant BN + act (pf_bn_apply_eval_quant_static) and activation quantizers
+(pf_uq_act_quant_static) compute no range, so an image's logits no longer depend on the rest of its batch.  A consumer
+whose calibrated input range does not start at 0 keeps fake-quant (the u8 convolution has no term for an activation
+offset).  The sidecar of a calibrated model carries the ranges under version 3; one without them is written as before.
+
+select() decides from the graph (and the ranges) alone.  IntModel hands the selected layers and their weight levels to the executor
 (`int_layers`), whose plan lowers them (engine._U8Conv, _U8DwConv) and the batch norms feeding them (_U8Bn) beside
 every other layer.  A u8 convolution takes the residual and folded batch norm a tensor-core lowering of the layer would
 take, and owns no split-bf16 weight copy.  Every selected shape has that lowering on the default conv path (Cin, Cout
@@ -40,6 +49,8 @@ the layer falling back to fake-quant.
 
     im = IntModel.from_checkpoint(graph, images, logits, state, cfg)   # the learner's checkpoint (unquantized weights)
     logits = im.forward(images_tensor)
+    r = calibrate(graph, images, logits, state, cfg, batches)          # optional: static activation ranges
+    im = IntModel.from_checkpoint(graph, images, logits, state, cfg, act_ranges=r)
     im.export(path)                                                    # integer checkpoint + sidecar
     im2 = IntModel.load(graph, images, logits, path)
 `graph` / `images` / `logits` are the network's inference graph (compact.build_eval_graph); `cfg` the quantizer settings
@@ -54,7 +65,9 @@ from . import compact
 
 F32 = np.float32
 SIDECAR_VERSION = 2          # written when depthwise layers run as integers; version 1 otherwise
-SIDECAR_VERSIONS = (1, 2)    # what load() reads
+SIDECAR_VERSION_RANGES = 3   # written when the model has calibrated activation ranges
+SIDECAR_VERSIONS = (1, 2, 3)  # what load() reads
+STATS = ('mean', 'max')      # calibrate()'s statistics
 CFG_KEYS = ('weight_bits', 'activation_bits', 'quantize_all_layers', 'use_buckets', 'bucket_type', 'bucket_size')
 
 
@@ -107,13 +120,70 @@ def _conv_desc(op):
     return ops.conv_desc(n, h, w, c, k, kh, kw, p, q, sh, sw, pt, pl)
 
 
-def select(graph, logits, cfg):
+def range_stats(per_batch, stat='mean'):
+    """{name: (lo, hi)} in fp32 from per-batch ranges [{name: (lo, hi)}, ...]: 'mean' = the float64 mean of the
+    per-batch min and max (with one batch, that batch's range bit for bit), 'max' = the extremes over the batches."""
+    if stat not in STATS:
+        raise ValueError('calibration statistic %r (one of %s)' % (stat, ', '.join(STATS)))
+    if not per_batch:
+        raise ValueError('calibration needs at least one batch')
+    out = {}
+    for name in per_batch[0]:
+        r = np.array([b[name] for b in per_batch], np.float64)
+        lo, hi = (r.mean(axis=0) if stat == 'mean' else (r[:, 0].min(), r[:, 1].max()))
+        out[name] = (F32(lo), F32(hi))
+    return out
+
+
+def executor_ranges(ex, batches, stat='mean'):
+    """range_stats of the per-batch ranges an inference executor's activation quantizers write into their slots, over
+    `batches` (an iterable of image tensors of its input's shape, each read once, in turn)"""
+    from . import ops
+    if ex.aq_static:
+        raise ValueError('the executor already quantizes with static ranges: it computes none per batch')
+    per_batch = []
+    for x in batches:
+        ex.buf[ex.images].copy_(x)
+        ex.forward(training=False)
+        r = ops.decode_ordered(ex.aq_slots.cpu().numpy().view(np.uint32)).reshape(-1, 2)
+        per_batch.append({op.name: (r[i, 0], r[i, 1]) for i, op in enumerate(ex.aq_ops)})
+    return range_stats(per_batch, stat)
+
+
+def calibrate(graph, images, logits, state, cfg, batches, stat='mean', device=None):
+    """Static activation ranges {Relu / Relu6 op name: (lo, hi) fp32} of every activation quant_marks returns: the
+    fake-quantized model (fake_quant_executor, the learner's checkpoint `state`) run over `batches`, its per-batch
+    ranges combined by `stat` (range_stats)."""
+    import torch
+    device = device or torch.device('cuda', torch.cuda.current_device())
+    full = compact.map_state(graph, compact.reachable_ops(graph, logits), state)
+    return executor_ranges(fake_quant_executor(graph, images, logits, full, cfg, device), batches, stat)
+
+
+def _ranges(graph, cfg, act_ranges):
+    """act_ranges normalised to {name: (F32 lo, F32 hi)}, checked to cover every quantized activation"""
+    if act_ranges is None:
+        return None
+    names = [op.name for op in quant_marks(graph, cfg)[1]]
+    missing = [n for n in names if n not in act_ranges]
+    if missing:
+        raise ValueError('no calibrated range for the quantized activations %s' % missing)
+    out = {n: (F32(act_ranges[n][0]), F32(act_ranges[n][1])) for n in names}
+    bad = [n for n, (lo, hi) in out.items() if not lo <= hi]
+    if bad:
+        raise ValueError('calibrated ranges with lo > hi (or NaN): %s' % bad)
+    return out
+
+
+def select(graph, logits, cfg, act_ranges=None):
     """[(op name, None or the reason it keeps the fake-quant kernels)] for every Conv2D / MatMul / depthwise op in
     graph order; None = it runs on a u8 kernel.  Depthwise ops are considered only with cfg['int8_depthwise'];
-    cfg['int8_narrow'] admits channel counts that are multiples of 16."""
+    cfg['int8_narrow'] admits channel counts that are multiples of 16; with calibrated `act_ranges` ({activation name:
+    (lo, hi)}) a layer whose input range does not start at 0 keeps fake-quant."""
     from . import ops
     mm, acts = quant_marks(graph, cfg)
     mm, acts = set(mm), set(acts)
+    act_ranges = _ranges(graph, cfg, act_ranges)
     depthwise = bool(cfg.get('int8_depthwise', False))
     narrow = bool(cfg.get('int8_narrow', False))
     out = []
@@ -137,6 +207,8 @@ def select(graph, logits, cfg):
             why = 'input is not a quantized batch norm + ReLU output'
         elif cfg['activation_bits'] > 8:
             why = 'activation bits %d > 8' % cfg['activation_bits']
+        elif act_ranges is not None and act_ranges[x.op.name][0] != 0:
+            why = 'calibrated activation range does not start at 0'
         else:
             c = x.shape[-1]
             if dw and (c < 16 or (c % 16 if narrow else c & (c - 1))):
@@ -170,13 +242,16 @@ def report_lines(sel):
     return lines
 
 
-def _specs(graph, cfg, exclude=()):
-    """the Executor's weight_quant / act_quant specs of the fake-quant model, less the weight quantizers of `exclude`"""
+def _specs(graph, cfg, exclude=(), act_ranges=None):
+    """the Executor's weight_quant / act_quant specs of the fake-quant model, less the weight quantizers of `exclude`;
+    with act_ranges ({name: (lo, hi)}, _ranges) the activation quantizers take them as static ranges"""
     mm, acts = quant_marks(graph, cfg)
     mm = [op for op in mm if op.name not in exclude]
     wq = dict(kind='uniform', ops=mm, bits=[cfg['weight_bits']] * len(mm), use_buckets=cfg['use_buckets'],
               bucket_type=cfg['bucket_type'], bucket_size=cfg['bucket_size']) if mm else None
     aq = dict(ops=acts, bits=[cfg['activation_bits']] * len(acts)) if acts else None
+    if aq and act_ranges is not None:
+        aq['ranges'] = [act_ranges[op.name] for op in acts]
     return wq, aq
 
 
@@ -189,10 +264,11 @@ def _load(ex, state):
     ex.prepare_static_weights()
 
 
-def fake_quant_executor(graph, images, logits, state, cfg, device):
-    """The fake-quantized model as the learner evaluates it, on `graph` in inference mode (engine.Executor)."""
+def fake_quant_executor(graph, images, logits, state, cfg, device, act_ranges=None):
+    """The fake-quantized model as the learner evaluates it, on `graph` in inference mode (engine.Executor); with
+    act_ranges (calibrate) its activations are quantized with those static ranges instead of each batch's."""
     from .engine import Executor
-    wq, aq = _specs(graph, cfg)
+    wq, aq = _specs(graph, cfg, act_ranges=_ranges(graph, cfg, act_ranges))
     ex = Executor(graph, images, logits, device, train=False, weight_quant=wq, act_quant=aq)
     _load(ex, state)
     return ex
@@ -202,13 +278,19 @@ class IntModel:
     """A uniformly quantized model whose eligible convolutions run on the u8 kernels: an inference engine.Executor
     given them as its `int_layers`, whose plan lowers them and the batch norms feeding them to the u8 kernels."""
 
-    def __init__(self, graph, images, logits, cfg, state, wlevels, device=None):
+    # None, or the static {activation name: (lo, hi)} it quantizes with (calibrate); a class default as well, so that
+    # export() answers for subclasses that fill the model's fields without this __init__
+    act_ranges = None
+
+    def __init__(self, graph, images, logits, cfg, state, wlevels, device=None, act_ranges=None):
         """state: {variable name: fp32 array} of every variable but the integer layers' kernels; wlevels: {conv op
-        name: (levels uint8 HWIO, alpha, beta)} of the integer layers"""
+        name: (levels uint8 HWIO, alpha, beta)} of the integer layers; act_ranges: None (each batch's ranges) or the
+        static {activation name: (lo, hi)} of every quantized activation (calibrate)"""
         import torch
         from .engine import Executor
         self.graph, self.images, self.logits, self.cfg = graph, images, logits, dict(cfg)
-        self.sel = select(graph, logits, cfg)
+        self.act_ranges = _ranges(graph, cfg, act_ranges)
+        self.sel = select(graph, logits, cfg, self.act_ranges)
         ints = [name for name, why in self.sel if why is None]
         if sorted(ints) != sorted(wlevels):
             raise ValueError('the weight levels do not cover the integer layers: %s' % sorted(set(ints) ^ set(wlevels)))
@@ -221,23 +303,30 @@ class IntModel:
             full[byname[name].vars['kernel'].name] = dequantize(lv, al, be, bits)
             int_layers[byname[name]] = (lv, al, be, bits)
         self.device = device or torch.device('cuda', torch.cuda.current_device())
-        wq, aq = _specs(graph, cfg, exclude=set(ints))
+        wq, aq = _specs(graph, cfg, exclude=set(ints), act_ranges=self.act_ranges)
         self.ex = Executor(graph, images, logits, self.device, train=False, weight_quant=wq, act_quant=aq,
                            int_layers=int_layers)
         _load(self.ex, full)
 
     @classmethod
-    def from_checkpoint(cls, graph, images, logits, state, cfg, device=None):
-        """From the uniform learner's checkpoint (unquantized weights under any one scope, compact.map_state)."""
+    def from_checkpoint(cls, graph, images, logits, state, cfg, device=None, act_ranges=None):
+        """From the uniform learner's checkpoint (unquantized weights under any one scope, compact.map_state), with
+        calibrated activation ranges or without."""
         full = compact.map_state(graph, compact.reachable_ops(graph, logits), state)
         per_channel = cfg['use_buckets'] and cfg['bucket_type'] == 'channel'
         byname = {op.name: op for op in compact.reachable_ops(graph, logits)}
         wlevels = {}
-        for name, why in select(graph, logits, cfg):
+        for name, why in select(graph, logits, cfg, act_ranges):
             if why is None:
                 kname = byname[name].vars['kernel'].name
                 wlevels[name] = weight_levels(full.pop(kname), cfg['weight_bits'], per_channel)
-        return cls(graph, images, logits, cfg, full, wlevels, device)
+        return cls(graph, images, logits, cfg, full, wlevels, device, act_ranges)
+
+    def calibrate(self, batches, stat='mean'):
+        """Static activation ranges {name: (lo, hi)} measured on this (per-batch) integer model's own activations over
+        `batches`, combined by `stat` (range_stats): with the batch that is then evaluated, a model built with them
+        computes what this one computes."""
+        return executor_ranges(self.ex, batches, stat)
 
     def forward(self, images=None):
         """Logits (device tensor, the executor's own buffer) of `images` (or of what the input buffer holds)."""
@@ -260,8 +349,12 @@ class IntModel:
         fn = path + '.npz'
         np.savez(fn, **arrays)
         version = SIDECAR_VERSION if any(byname[n].type == 'DepthwiseConv2dNative' for n in self.wlevels) else 1
+        rec = dict(version=version, config=self.cfg, layers=[[n, w] for n, w in self.sel])
+        if self.act_ranges is not None:      # fp32 -> JSON double -> fp32 is exact
+            rec.update(version=SIDECAR_VERSION_RANGES,
+                       act_ranges={n: [float(lo), float(hi)] for n, (lo, hi) in self.act_ranges.items()})
         with open(path + '.int8.json', 'w') as f:
-            json.dump(dict(version=version, config=self.cfg, layers=[[n, w] for n, w in self.sel]), f)
+            json.dump(rec, f)
         return fn
 
     @classmethod
@@ -272,6 +365,9 @@ class IntModel:
         if rec.get('version') not in SIDECAR_VERSIONS:
             raise ValueError('%s.int8.json: unsupported sidecar version %r (this loader reads %s)'
                              % (path, rec.get('version'), ', '.join(map(str, SIDECAR_VERSIONS))))
+        if (rec['version'] == SIDECAR_VERSION_RANGES) != ('act_ranges' in rec):
+            raise ValueError('%s.int8.json: unsupported sidecar version %r with%s act_ranges (version %d carries them)'
+                             % (path, rec['version'], '' if 'act_ranges' in rec else 'out', SIDECAR_VERSION_RANGES))
         cfg = {k: rec['config'][k] for k in CFG_KEYS}
         for opt in ('int8_depthwise', 'int8_narrow'):
             if rec['config'].get(opt):
@@ -284,4 +380,5 @@ class IntModel:
             if why is None:
                 k = byname[name].vars['kernel'].name[:-2]
                 wlevels[name] = (arrays.pop(k + '/levels'), arrays.pop(k + '/alpha'), arrays.pop(k + '/beta'))
-        return cls(graph, images, logits, cfg, arrays, wlevels, device)
+        kw = dict(act_ranges=rec['act_ranges']) if 'act_ranges' in rec else {}
+        return cls(graph, images, logits, cfg, arrays, wlevels, device, **kw)

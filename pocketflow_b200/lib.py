@@ -28,6 +28,7 @@ SIGNATURES = {
     'pf_uq_act_minmax': (c_i32, [c_vp, c_i64, c_vp, c_vp]),
     'pf_uq_act_quant': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_vp]),
     'pf_uq_act_quant_planes': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp]),
+    'pf_uq_act_quant_static': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_vp]),
     'pf_ws_mask_build': (c_i32, [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_select_desc': (c_i32, [c_vp, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_momentum_step': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_f32, c_f32, c_f32, c_vp]),
@@ -78,6 +79,8 @@ SIGNATURES = {
     'pf_conv2d_u8_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_eval_levels_u8': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp,
                                      c_vp, c_vp]),
+    'pf_bn_eval_levels_u8_static': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp,
+                                            c_vp, c_vp, c_vp]),
     'pf_tc_probe': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32] + [ctypes.c_uint32] * 6 + [c_vp]),
     'pf_dwconv_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     'pf_dwconv_dgrad': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),
@@ -94,6 +97,8 @@ SIGNATURES = {
     'pf_bn_train_stats_range': (c_i32, [c_vp, c_i64, c_i32, c_f32, c_f32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32,
                                         c_vp, c_vp, c_vp]),
     'pf_bn_apply_eval': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'pf_bn_apply_eval_quant_static': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_f32, c_vp, c_vp, c_i32, c_vp, c_i32, c_vp,
+                                              c_vp, c_vp, c_vp]),
     'pf_bn_apply_quant': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_bn_apply_quant_levels': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp,
                                          c_vp, c_vp]),

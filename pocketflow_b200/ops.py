@@ -136,6 +136,12 @@ def decode_ordered(u):
     return bits.view(np.float32)
 
 
+def encode_ordered(f):
+    """the ordered-uint encoding (pf_enc) of fp32 values, as uint32: the inverse of decode_ordered"""
+    u = np.asarray(f, np.float32).view(np.uint32)
+    return np.where(u & np.uint32(0x80000000), ~u, u | np.uint32(0x80000000)).astype(np.uint32)
+
+
 # ----------------------------------------------------------------------------- device plumbing
 def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
@@ -306,6 +312,19 @@ def act_quant(x, y, minmax, bits, planes=None):
     else:
         _lib.check(_lib.load().pf_uq_act_quant_planes(_p(x), _p(y), _p(planes.hi), _p(planes.lo), x.numel(), _p(minmax),
                                                       int(bits), _stream()), 'pf_uq_act_quant_planes')
+
+
+def act_quant_static(x, y, rng, bits):
+    """y = Q(clamp(x, lo, hi)) with a static range rng (int32[2], ordered-uint lo / hi: range_slots) in one pass"""
+    _check_f32(x, y)
+    _lib.check(_lib.load().pf_uq_act_quant_static(_p(x), _p(y), x.numel(), _p(rng), int(bits), _stream()),
+               'pf_uq_act_quant_static')
+
+
+def range_slots(ranges, device):
+    """int32 [n, 2]: the fp32 ranges [(lo, hi), ...] in the range slots' ordered-uint encoding (encode_ordered)"""
+    enc = encode_ordered(np.asarray(ranges, np.float32).reshape(-1, 2))
+    return torch.from_numpy(enc.view(np.int32)).to(device)
 
 
 def act_fake_quant(x, bits, out=None, minmax=None):
@@ -714,6 +733,15 @@ def bn_apply_eval(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, y, minmax=N
                                             _p(y), _p(planes.hi if planes is not None else None),
                                             _p(planes.lo if planes is not None else None), _p(minmax), _stream()),
                'pf_bn_apply_eval')
+
+
+def bn_apply_eval_quant_static(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, rng, bits, y=None, planes=None):
+    """Q(clamp(act(bn(x)), lo, hi)) with the moving statistics and a static range rng (range_slots) in one launch, to
+    fp32 and/or operand planes"""
+    _lib.check(_lib.load().pf_bn_apply_eval_quant_static(
+        _p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma), _p(beta), int(act), _p(rng), int(bits), _p(y),
+        _p(planes.hi if planes is not None else None), _p(planes.lo if planes is not None else None), _stream()),
+        'pf_bn_apply_eval_quant_static')
 
 
 def bn_apply_quant(x, m, c, mean, rstd, gamma, beta, act, rng, bits, y=None, planes=None):
@@ -1176,6 +1204,17 @@ def bn_eval_levels_u8(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, bits, r
     _lib.check(_lib.load().pf_bn_eval_levels_u8(_p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma), _p(beta),
                                                 int(act), int(bits), _p(rng), int(bool(have_range)), _p(levels), _p(hdr),
                                                 _p(csum), _stream()), 'pf_bn_eval_levels_u8')
+
+
+def bn_eval_levels_u8_static(x, m, c, mov_mean, mov_var, eps, gamma, beta, act, bits, rng, levels, hdr, csum):
+    """bn_eval_levels_u8 with a static range rng (range_slots; read only): y clamped to it, one pass, no range pass
+    (pf_bn_eval_levels_u8_static)"""
+    if levels.dtype != torch.uint8:
+        raise ValueError('bn_eval_levels_u8_static: levels must be uint8')
+    _check_f32(x, mov_mean, mov_var, gamma, beta, csum)
+    _lib.check(_lib.load().pf_bn_eval_levels_u8_static(_p(x), m, c, _p(mov_mean), _p(mov_var), float(eps), _p(gamma),
+                                                       _p(beta), int(act), int(bits), _p(rng), _p(levels), _p(hdr),
+                                                       _p(csum), _stream()), 'pf_bn_eval_levels_u8_static')
 
 
 def conv2d_tc_last_plan():

@@ -11,6 +11,12 @@ inference forward of both models is timed as CUDA-graph replays at --batch_size_
         --uql_weight_bits 8 --uql_activation_bits 8 --uql_use_buckets --batch_size_eval 128 --out ./rn50_int8/model
 
 Without --ckpt_dir the model keeps its seed initialisation (for speed measurements only).
+
+With --int8_calibrate N the fake-quantized model is run over N fresh batches of the net's training set (--data_dir_local:
+real data, with the training augmentation, so that the ranges are not fitted to the evaluation images; otherwise the
+learners' synthetic batches) and the exported model carries static activation ranges (int8.calibrate,
+--int8_calib_stat mean | max): its logits no longer depend on the rest of the batch.  The tool prints every range and
+also times the integer model with per-batch ranges ('integer') against the calibrated one ('integer_calibrated').
 """
 import argparse
 import importlib
@@ -44,6 +50,14 @@ def parse(argv=None):
     p.add_argument('--int8_narrow', action='store_true',
                    help='channel counts that are multiples of 16 too (the cp.async-fed u8 kernel, any C %% 16 level '
                         'producer); also times the integer model without them')
+    p.add_argument('--int8_calibrate', type=int, default=0, metavar='N',
+                   help='calibrate static activation ranges on N batches and export the calibrated model')
+    p.add_argument('--int8_calib_stat', default='mean', choices=('mean', 'max'),
+                   help='mean: the mean of the per-batch min / max; max: their extremes')
+    p.add_argument('--batch_size_calib', type=int, default=None, help='calibration batch size (default: batch_size_eval)')
+    p.add_argument('--data_dir_local', default=None,
+                   help='the net\'s dataset on disk; calibration reads its training split with the training augmentation '
+                        '(default: synthetic batches)')
     p.add_argument('--batch_size_eval', type=int, default=100)
     p.add_argument('--nb_repts_warmup', type=int, default=20, help='graph replays before timing')
     p.add_argument('--nb_repts', type=int, default=50, help='graph replays per timed window')
@@ -89,6 +103,31 @@ def load_state(args, graph, logits):
     return {v.name: v.initializer(rng, v.shape) for op in compact.reachable_ops(graph, logits) for v in op.vars.values()}
 
 
+def calibration_batches(helper, n, bs):
+    """n image batches [bs, ...] of the net's training set, each drawn when it is consumed, from the dataset's own source
+    (the generator behind its iterator): the iterator hands out rotating pinned buffers, rewritten after POOL_SIZE draws
+    (real data) or cycled (synthetic), so its batches must not be held; these are n distinct batches."""
+    import torch
+    it = helper.DATASET(is_train=True).build()
+    for _ in range(n):
+        yield torch.from_numpy(np.ascontiguousarray(it.generator(bs)[0]))
+
+
+def calibration_ranges(args, cfg, state):
+    """int8.calibrate over --int8_calibrate batches of the net's training set at --batch_size_calib"""
+    from pocketflow_b200 import compact, int8
+    from pocketflow_b200.flags import FLAGS
+    net = importlib.import_module('pocketflow_b200.nets.' + args.net)
+    bs = args.batch_size_calib or args.batch_size_eval
+    FLAGS.batch_size = bs
+    if args.data_dir_local:
+        FLAGS.data_dir_local = args.data_dir_local
+    helper = net.ModelHelper()
+    graph, images, logits = compact.build_eval_graph(helper, bs)
+    return int8.calibrate(graph, images, logits, state, cfg, calibration_batches(helper, args.int8_calibrate, bs),
+                          args.int8_calib_stat)
+
+
 def gpu_name(torch):
     try:
         return subprocess.check_output(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm',
@@ -111,7 +150,17 @@ def main(argv=None):
     dev = torch.device('cuda', 0)
     torch.cuda.set_device(dev)
     im = int8.IntModel.from_checkpoint(graph, images, logits, state, cfg, dev)
-    print('integer model written to ' + im.export(args.out) + ' (+ %s.int8.json)' % args.out)
+    ranges, imc = None, None
+    if args.int8_calibrate:
+        ranges = calibration_ranges(args, cfg, state)
+        print('calibrated activation ranges (%s of %d batches):' % (args.int8_calib_stat, args.int8_calibrate))
+        for name, (lo, hi) in ranges.items():
+            print('  %s: [%.9g, %.9g]' % (name, lo, hi))
+        imc = int8.IntModel.from_checkpoint(graph, images, logits, state, cfg, dev, act_ranges=ranges)
+        for line in int8.report_lines(imc.sel):
+            print('calibrated ' + line)
+    out = imc or im
+    print('integer model written to ' + out.export(args.out) + ' (+ %s.int8.json)' % args.out)
     if args.no_time:
         return 0
     fq = int8.fake_quant_executor(graph, images, logits, compact.map_state(graph, compact.reachable_ops(graph, logits),
@@ -127,6 +176,9 @@ def main(argv=None):
             im_without.ex.buf[images].copy_(x)
             arms[arm] = im_without.ex
     arms['integer'] = im.ex
+    if imc is not None:
+        imc.ex.buf[images].copy_(x)
+        arms['integer_calibrated'] = imc.ex
     graphs = {arm: _capture(lambda ex=ex: ex.forward(training=False), torch) for arm, ex in arms.items()}
     for gr in graphs.values():
         gr.replay()
@@ -144,7 +196,7 @@ def main(argv=None):
     bs = args.batch_size_eval
     res = dict(net=args.net, resnet_size=args.resnet_size, batch=bs, config=cfg,
                int_layers=sum(1 for _, w in im.sel if w is None), layers=len(im.sel), logits_max_rel_diff=diff,
-               top1_agreement=agree)
+               top1_agreement=agree, calibrated=bool(imc))
     for arm, v in ms.items():
         ips = sorted(bs / (t / 1e3) for t in v)
         res[arm] = dict(ms_per_batch=sorted(v), images_per_s_min=ips[0], images_per_s_median=float(np.median(ips)),
