@@ -769,6 +769,25 @@ int pf_cpr_ista(const float* g_dev, const float* b_dev, const float* m0_dev, int
                 float* m_dev, float* ws_dev, int32_t* nnz_dev, void* stream);
 int pf_cpr_mask_channels(float* a_dev, int64_t rows, int rs, int cin, int inner, const float* m_dev, void* stream);
 
+/* f5b Channel selection of the LASSO channel-pruning learner (pf_cpr.cu, /root/reference/learners/channel_pruning).
+ *   pf_cp_sample     rows_dev int32 [n_rows, 8] = (n, oh, ow, dst, rh, rw, 0, 0) (16-byte aligned; dst < 0: skip):
+ *                    X[dst] = the R x S x C input patch at (n, oh, ow) as pf_cpr_sample gathers it, and in float64
+ *                    Y[dst, k] = (y - bias)[n, oh, ow, k] + (res_full - res_cur)[n, rh, rw, k] (res_* [N, res_h,
+ *                    res_w, K], both NULL: no residual term).
+ *   pf_cp_gram       G_aug [(cin+1)^2 (+1 scratch)] = [P | y]^T [P | y] over the n_idx sampled rows idx_dev, where
+ *                    P[(j, o), c] = sum_t X[idx[j], t, c] W[t, c, o] and y[(j, o)] = Y[idx[j], o]; float64, formed
+ *                    chunk_rows rows at a time in ws_dev ((cin+1) * chunk_rows * cout doubles).
+ *   pf_cp_normal_eq  G_aug [(ncols+cout)^2 (+1 scratch)] = [X_k | Y]^T [X_k | Y] over all n_rows rows, X_k = the columns
+ *                    cols_dev of X [n_rows, K]; ws_dev holds (ncols + cout) * chunk_rows doubles.
+ */
+int pf_cp_sample(const pf_conv_desc* d, const float* x_dev, const void* x_hi_dev, const void* x_lo_dev,
+                 const float* y_dev, const float* bias_dev, const float* res_full_dev, const float* res_cur_dev,
+                 int res_h, int res_w, const int32_t* rows_dev, int n_rows, float* X_dev, double* Y_dev, void* stream);
+int pf_cp_gram(const float* X_dev, const double* Y_dev, const int32_t* idx_dev, int n_idx, const float* w_dev, int rs,
+               int cin, int cout, double* ws_dev, int64_t chunk_rows, double* g_dev, void* stream);
+int pf_cp_normal_eq(const float* X_dev, const double* Y_dev, int64_t n_rows, int64_t K, int cout, const int32_t* cols_dev,
+                    int ncols, double* ws_dev, int64_t chunk_rows, double* g_dev, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * a10 The collective of the data-parallel step (pf_comm.cu).  Replaces mgw.DistributedOptimizer's per-variable
  *     Horovod all-reduces and mgw.broadcast_global_variables (utils/multi_gpu_wrapper.py:82-98; call sites

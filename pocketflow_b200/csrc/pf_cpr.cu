@@ -19,6 +19,16 @@
 //                         are the same bits run after run whatever the grid size
 //   pf_cpr_mask_channels  a[.., t, c, k] *= [|m[c]| > 0]  (the kept-channel patch matrix and the final W * bnry)
 // Every reduction has a fixed order: results are deterministic.
+//
+// The LASSO channel-pruning learner (/root/reference/learners/channel_pruning/channel_pruner.py) has its own entry
+// points here, on the same Gram machinery:
+//   pf_cp_sample      the patches of the current model's conv input and the full model's conv outputs at positions
+//                     shared by a whole batch (:263-341, :391-412); Y in float64, plus the residual branch difference
+//                     full - current of the block's Add output, gathered at the Add's own positions (:579-586)
+//   pf_cp_gram        the design matrix product[(s, o), c] = sum_hw X[s, hw, c] W2[hw, c, o] over the sampled rows
+//                     (:468-476) and G_aug = [P | y]^T [P | y] in float64, unnormalised
+//   pf_cp_normal_eq   [X_k | Y]^T [X_k | Y] in float64 over every row: the normal equations of the refit of the kept
+//                     input channels (:569-573)
 #include <cooperative_groups.h>
 #include <cuda_bf16.h>
 
@@ -28,6 +38,35 @@ namespace cg = cooperative_groups;
 
 namespace {
 
+// ------------------------------------------------------------------------------------------------ shared pieces
+// the R x S x C input patch at output position (n, oh, ow) into xr (zero outside the image), one block per row
+__device__ __forceinline__ void gather_patch(const pf_conv_desc& d, const float* __restrict__ x,
+                                             const __nv_bfloat16* __restrict__ xhi,
+                                             const __nv_bfloat16* __restrict__ xlo, int n, int oh, int ow,
+                                             float* __restrict__ xr) {
+  const int K = d.r * d.s * d.c;
+  for (int e = threadIdx.x; e < K; e += blockDim.x) {
+    const int t = e / d.c, c = e - t * d.c;
+    const int r = t / d.s, s = t - r * d.s;
+    const int ih = oh * d.stride_h - d.pad_t + r, iw = ow * d.stride_w - d.pad_l + s;
+    float v = 0.f;
+    if (ih >= 0 && ih < d.h && iw >= 0 && iw < d.w) {
+      const size_t i = (((size_t)n * d.h + ih) * d.w + iw) * d.c + c;
+      v = x ? x[i] : __fadd_rn(__bfloat162float(xhi[i]), __bfloat162float(xlo[i]));
+    }
+    xr[e] = v;
+  }
+}
+
+// sum_t X[src, t, c] W[t, c, o] in float64, in t order
+__device__ __forceinline__ double patch_times_kernel(const float* __restrict__ X, const float* __restrict__ w,
+                                                     int64_t src, int64_t K, int rs, int cin, int cout, int c, int o) {
+  double acc = 0.0;
+  const float* xr = X + src * K + c;
+  for (int t = 0; t < rs; ++t) acc = fma((double)xr[(int64_t)t * cin], (double)w[((int64_t)t * cin + c) * cout + o], acc);
+  return acc;
+}
+
 // ------------------------------------------------------------------------------------------------ sampler
 __global__ void __launch_bounds__(256)
 cpr_sample_kernel(pf_conv_desc d, const float* __restrict__ x, const __nv_bfloat16* __restrict__ xhi,
@@ -36,18 +75,7 @@ cpr_sample_kernel(pf_conv_desc d, const float* __restrict__ x, const __nv_bfloat
   const int4 row = reinterpret_cast<const int4*>(rows)[blockIdx.x];    // (n, oh, ow, dst)
   if (row.w < 0) return;
   const int K = d.r * d.s * d.c;
-  float* xr = X + (size_t)row.w * K;
-  for (int e = threadIdx.x; e < K; e += blockDim.x) {
-    const int t = e / d.c, c = e - t * d.c;
-    const int r = t / d.s, s = t - r * d.s;
-    const int ih = row.y * d.stride_h - d.pad_t + r, iw = row.z * d.stride_w - d.pad_l + s;
-    float v = 0.f;
-    if (ih >= 0 && ih < d.h && iw >= 0 && iw < d.w) {
-      const size_t i = (((size_t)row.x * d.h + ih) * d.w + iw) * d.c + c;
-      v = x ? x[i] : __fadd_rn(__bfloat162float(xhi[i]), __bfloat162float(xlo[i]));
-    }
-    xr[e] = v;
-  }
+  gather_patch(d, x, xhi, xlo, row.x, row.y, row.z, X + (size_t)row.w * K);
   const float* yr = y + (((size_t)row.x * d.p + row.y) * d.q + row.z) * d.k;
   for (int k = threadIdx.x; k < d.k; k += blockDim.x)
     Y[(size_t)row.w * d.k + k] = bias ? __fsub_rn(yr[k], bias[k]) : yr[k];
@@ -70,9 +98,7 @@ cpr_feature_kernel(const float* __restrict__ X, const float* __restrict__ Y, con
     if (c == cin) {
       acc = (double)Y[src * cout + o];
     } else {
-      acc = 0.0;
-      const float* xr = X + src * K + c;
-      for (int t = 0; t < rs; ++t) acc = fma((double)xr[(int64_t)t * cin], (double)w[((int64_t)t * cin + c) * cout + o], acc);
+      acc = patch_times_kernel(X, w, src, K, rs, cin, cout, c, o);
     }
     Ft[(int64_t)c * mcap + m] = acc;
   }
@@ -203,6 +229,60 @@ cpr_mask_channels_kernel(float* __restrict__ a, int64_t total, int cin, int inne
   }
 }
 
+// ------------------------------------------------------------------------------------------------ LASSO learner
+// rows: int32 [n, 8] = (n, oh, ow, dst, rh, rw, -, -): the conv's output position and the Add's (when res_full is set)
+__global__ void __launch_bounds__(256)
+cp_sample_kernel(pf_conv_desc d, const float* __restrict__ x, const __nv_bfloat16* __restrict__ xhi,
+                 const __nv_bfloat16* __restrict__ xlo, const float* __restrict__ y, const float* __restrict__ bias,
+                 const float* __restrict__ res_full, const float* __restrict__ res_cur, int res_h, int res_w,
+                 const int32_t* __restrict__ rows, float* __restrict__ X, double* __restrict__ Y) {
+  const int4 row = reinterpret_cast<const int4*>(rows)[2 * blockIdx.x];
+  const int4 rrow = reinterpret_cast<const int4*>(rows)[2 * blockIdx.x + 1];
+  if (row.w < 0) return;
+  const int K = d.r * d.s * d.c;
+  gather_patch(d, x, xhi, xlo, row.x, row.y, row.z, X + (size_t)row.w * K);
+  const float* yr = y + (((size_t)row.x * d.p + row.y) * d.q + row.z) * d.k;
+  const size_t ri = (((size_t)row.x * res_h + rrow.x) * res_w + rrow.y) * d.k;
+  for (int k = threadIdx.x; k < d.k; k += blockDim.x) {
+    double v = (double)(bias ? __fsub_rn(yr[k], bias[k]) : yr[k]);
+    if (res_full) v = v + ((double)res_full[ri + k] - (double)res_cur[ri + k]);
+    Y[(size_t)row.w * d.k + k] = v;
+  }
+}
+
+// Ft[c][m] (ld = mcap), m = j*cout + o over the chunk's sampled rows j: c < cin the design matrix, c == cin y
+__global__ void __launch_bounds__(256)
+cp_product_kernel(const float* __restrict__ X, const double* __restrict__ Y, const int32_t* __restrict__ idx, int j0,
+                  int nj, const float* __restrict__ w, int rs, int cin, int cout, double* __restrict__ Ft, int64_t mcap) {
+  const int64_t m_n = (int64_t)nj * cout, total = m_n * (cin + 1);
+  const int64_t K = (int64_t)rs * cin;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i / m_n);
+    const int64_t m = i - (int64_t)c * m_n;
+    const int j = (int)(m / cout), o = (int)(m - (int64_t)j * cout);
+    const int64_t src = idx[j0 + j];
+    double acc;
+    if (c == cin) {
+      acc = Y[src * cout + o];
+    } else {
+      acc = patch_times_kernel(X, w, src, K, rs, cin, cout, c, o);
+    }
+    Ft[(int64_t)c * mcap + m] = acc;
+  }
+}
+
+// Ft[c][m] (ld = mcap) over the chunk's rows m: c < ncols column cols[c] of X, then the cout columns of Y
+__global__ void __launch_bounds__(256)
+cp_columns_kernel(const float* __restrict__ X, const double* __restrict__ Y, const int32_t* __restrict__ cols, int ncols,
+                  int64_t K, int cout, int64_t r0, int64_t nr, double* __restrict__ Ft, int64_t mcap) {
+  const int64_t total = nr * (ncols + cout);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i / nr);
+    const int64_t m = i - (int64_t)c * nr, row = r0 + m;
+    Ft[(int64_t)c * mcap + m] = c < ncols ? (double)X[row * K + cols[c]] : Y[row * cout + (c - ncols)];
+  }
+}
+
 inline unsigned grid_for(int64_t n, int per_sm) {
   int64_t g = (n + 255) / 256;
   const int64_t cap = (int64_t)PF_NUM_SMS * per_sm;
@@ -297,6 +377,75 @@ int pf_cpr_mask_channels(float* a_dev, int64_t rows, int rs, int cin, int inner,
   const int64_t total = rows * rs * cin * (int64_t)inner;
   cpr_mask_channels_kernel<<<grid_for(total, 8), 256, 0, (cudaStream_t)stream>>>(a_dev, total, cin, inner, m_dev);
   PF_CHECK_LAUNCH("pf_cpr_mask_channels");
+  return PF_OK;
+}
+
+
+int pf_cp_sample(const pf_conv_desc* d, const float* x_dev, const void* x_hi_dev, const void* x_lo_dev,
+                 const float* y_dev, const float* bias_dev, const float* res_full_dev, const float* res_cur_dev,
+                 int res_h, int res_w, const int32_t* rows_dev, int n_rows, float* X_dev, double* Y_dev, void* stream) {
+  PF_REQUIRE(d != nullptr && n_rows >= 0, "pf_cp_sample: bad arguments");
+  PF_REQUIRE(d->n > 0 && d->h > 0 && d->w > 0 && d->c > 0 && d->k > 0 && d->r > 0 && d->s > 0 && d->p > 0 &&
+                 d->q > 0 && d->stride_h > 0 && d->stride_w > 0 && d->pad_t >= 0 && d->pad_l >= 0,
+             "pf_cp_sample: non-positive dimension in conv descriptor");
+  PF_REQUIRE(x_dev || (x_hi_dev && x_lo_dev), "pf_cp_sample: no input (fp32 tensor or hi/lo planes)");
+  PF_REQUIRE(y_dev && X_dev && Y_dev, "pf_cp_sample: null pointer");
+  PF_REQUIRE(!res_full_dev == !res_cur_dev, "pf_cp_sample: the residual needs both the full and the current tensor");
+  PF_REQUIRE(!res_full_dev || (res_h > 0 && res_w > 0), "pf_cp_sample: bad residual shape");
+  if (n_rows == 0) return PF_OK;
+  PF_REQUIRE(rows_dev && ((uintptr_t)rows_dev & 15) == 0, "pf_cp_sample: rows must be 16-byte aligned int32 [n, 8]");
+  cp_sample_kernel<<<n_rows, 256, 0, (cudaStream_t)stream>>>(*d, x_dev, (const __nv_bfloat16*)x_hi_dev,
+                                                              (const __nv_bfloat16*)x_lo_dev, y_dev, bias_dev,
+                                                              res_full_dev, res_cur_dev, res_h, res_w, rows_dev, X_dev,
+                                                              Y_dev);
+  PF_CHECK_LAUNCH("pf_cp_sample");
+  return PF_OK;
+}
+
+int pf_cp_gram(const float* X_dev, const double* Y_dev, const int32_t* idx_dev, int n_idx, const float* w_dev, int rs,
+               int cin, int cout, double* ws_dev, int64_t chunk_rows, double* g_dev, void* stream) {
+  PF_REQUIRE(n_idx >= 1 && rs >= 1 && cin >= 1 && cout >= 1 && chunk_rows >= 1, "pf_cp_gram: bad shape");
+  PF_REQUIRE(X_dev && Y_dev && idx_dev && w_dev && ws_dev && g_dev, "pf_cp_gram: null pointer");
+  PF_REQUIRE(cin < 65536 && (int64_t)rs * cin < (1ll << 31), "pf_cp_gram: kernel too large");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int n = cin + 1;
+  PF_CUDA(cudaMemsetAsync(g_dev, 0, sizeof(double) * ((size_t)n * n + 1), st));
+  const int64_t mcap = chunk_rows * cout;
+  const dim3 tiles((n + GT - 1) / GT, (n + GT - 1) / GT);
+  for (int j0 = 0; j0 < n_idx; j0 += (int)chunk_rows) {
+    const int nj = (int)((n_idx - j0) < chunk_rows ? (n_idx - j0) : chunk_rows);
+    const int64_t m_n = (int64_t)nj * cout;
+    cp_product_kernel<<<grid_for(m_n * n, 16), 256, 0, st>>>(X_dev, Y_dev, idx_dev, j0, nj, w_dev, rs, cin, cout, ws_dev,
+                                                             mcap);
+    PF_CHECK_LAUNCH("pf_cp_gram/product");
+    cpr_syrk_kernel<<<tiles, 256, 0, st>>>(ws_dev, mcap, m_n, n, g_dev);
+    PF_CHECK_LAUNCH("pf_cp_gram/syrk");
+  }
+  cpr_norm_kernel<<<1, 1024, 0, st>>>(g_dev, n, cin, g_dev + (size_t)n * n);     // (mirrors; the norm is not used)
+  PF_CHECK_LAUNCH("pf_cp_gram/mirror");
+  return PF_OK;
+}
+
+int pf_cp_normal_eq(const float* X_dev, const double* Y_dev, int64_t n_rows, int64_t K, int cout, const int32_t* cols_dev,
+                    int ncols, double* ws_dev, int64_t chunk_rows, double* g_dev, void* stream) {
+  PF_REQUIRE(n_rows >= 1 && K >= 1 && cout >= 1 && ncols >= 1 && ncols <= K && chunk_rows >= 1,
+             "pf_cp_normal_eq: bad shape");
+  PF_REQUIRE(X_dev && Y_dev && cols_dev && ws_dev && g_dev, "pf_cp_normal_eq: null pointer");
+  PF_REQUIRE((int64_t)ncols + cout < 65536, "pf_cp_normal_eq: too many columns");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int n = ncols + cout;
+  PF_CUDA(cudaMemsetAsync(g_dev, 0, sizeof(double) * ((size_t)n * n + 1), st));
+  const dim3 tiles((n + GT - 1) / GT, (n + GT - 1) / GT);
+  for (int64_t r0 = 0; r0 < n_rows; r0 += chunk_rows) {
+    const int64_t nr = (n_rows - r0) < chunk_rows ? (n_rows - r0) : chunk_rows;
+    cp_columns_kernel<<<grid_for(nr * n, 16), 256, 0, st>>>(X_dev, Y_dev, cols_dev, ncols, K, cout, r0, nr, ws_dev,
+                                                             chunk_rows);
+    PF_CHECK_LAUNCH("pf_cp_normal_eq/columns");
+    cpr_syrk_kernel<<<tiles, 256, 0, st>>>(ws_dev, chunk_rows, nr, n, g_dev);
+    PF_CHECK_LAUNCH("pf_cp_normal_eq/syrk");
+  }
+  cpr_norm_kernel<<<1, 1024, 0, st>>>(g_dev, n, n, g_dev + (size_t)n * n);        // (mirrors; the norm is not used)
+  PF_CHECK_LAUNCH("pf_cp_normal_eq/mirror");
   return PF_OK;
 }
 

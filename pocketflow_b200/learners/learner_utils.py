@@ -26,7 +26,10 @@ def create_learner(sm_writer, model_helper):
     elif FLAGS.learner == 'non-uniform':
         from .nonuniform_quantization.learner import NonUniformQuantLearner
         learner = NonUniformQuantLearner(sm_writer, model_helper)
-    elif FLAGS.learner in ('channel', 'dis-chn-pruned', 'uniform-tf'):
+    elif FLAGS.learner == 'channel':
+        from .channel_pruning.learner import ChannelPrunedLearner
+        learner = ChannelPrunedLearner(sm_writer, model_helper)
+    elif FLAGS.learner in ('dis-chn-pruned', 'uniform-tf'):
         raise ValueError('learner %s is outside the hot-path scope of this build (SURVEY.md §8)' % FLAGS.learner)
     else:
         raise ValueError('unrecognized learner\'s name: ' + FLAGS.learner)

@@ -143,6 +143,9 @@ SIGNATURES = {
     'pf_cpr_gram': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
     'pf_cpr_ista': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_f32, c_f32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_cpr_mask_channels': (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp]),
+    'pf_cp_sample': (c_i32, [c_vp] * 8 + [c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
+    'pf_cp_gram': (c_i32, [c_vp, c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_vp]),
+    'pf_cp_normal_eq': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_i32, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp]),
 }
 
 

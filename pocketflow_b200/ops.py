@@ -1446,6 +1446,72 @@ def cpr_mask_channels(a, m, rs, cin, inner):
                'pf_cpr_mask_channels')
 
 
+
+# ----------------------------------------------------------------------------- f5b LASSO channel selection (pf_cpr.cu)
+def _check_f64(*ts):
+    for t in ts:
+        if t is not None and (t.dtype != torch.float64 or not t.is_cuda or not t.is_contiguous()):
+            raise ValueError('expected a contiguous float64 CUDA tensor')
+
+
+def cp_sample(d, x, y, rows, X, Y, planes=None, bias=None, res_full=None, res_cur=None):
+    """Gather input patches into rows of X [*, R*S*Cin] (fp32) and conv outputs into rows of Y [*, Cout] (float64)
+    (channel_pruner.py:263-341, :391-412).  rows: int32 CUDA tensor [n, 8] = (n, oh, ow, dst row (< 0 skips it), rh,
+    rw, 0, 0).  The input is `x` (fp32 NHWC) or, when x is None, hi + lo of `planes`; `bias` is subtracted from the
+    output; res_full / res_cur [N, H', W', Cout]: Y += res_full - res_cur at (n, rh, rw), in float64 (:579-586)."""
+    _check_f32(x, y, X, bias, res_full, res_cur)
+    _check_f64(Y)
+    if rows.dtype != torch.int32 or not rows.is_cuda or not rows.is_contiguous() or rows.dim() != 2 or rows.shape[1] != 8:
+        raise ValueError('cp_sample: rows must be a contiguous int32 CUDA tensor [n, 8]')
+    rh, rw = (res_full.shape[1], res_full.shape[2]) if res_full is not None else (0, 0)
+    if res_full is not None and (res_cur is None or res_cur.shape != res_full.shape or res_full.shape[0] != d.n
+                                 or res_full.shape[3] != d.k):
+        raise ValueError('cp_sample: the residual tensors must both be [N, H, W, Cout]')
+    _lib.check(_lib.load().pf_cp_sample(ctypes.byref(d), _p(x), _p(planes.hi) if planes is not None else None,
+                                        _p(planes.lo) if planes is not None else None, _p(y), _p(bias), _p(res_full),
+                                        _p(res_cur), rh, rw, _p(rows), rows.shape[0], _p(X), _p(Y), _stream()),
+               'pf_cp_sample')
+
+
+def cp_gram(X, Y, idx, w, g, ws=None, chunk_rows=None, budget_bytes=1 << 30):
+    """G_aug = [P | y]^T [P | y] in float64 over the rows idx of X / Y, P[(j, o), c] = sum_t X[idx j, t, c] W[t, c, o]
+    (channel_pruner.py:468-476).  g: float64 [(Cin+1)^2 + 1]: G = g[:Cin, :Cin], P^T y = g[:Cin, Cin]."""
+    rs, cin, cout = _rs_cin_cout(w)
+    _check_f32(X, w)
+    _check_f64(Y, g)
+    if idx.dtype != torch.int32 or g.numel() < (cin + 1) ** 2 + 1:
+        raise ValueError('cp_gram: idx must be int32 and g float64 [(Cin+1)^2 + 1]')
+    if chunk_rows is None:
+        chunk_rows = cpr_gram_chunk_rows(cin, cout, idx.numel(), budget_bytes)
+    need = (cin + 1) * int(chunk_rows) * cout
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.float64, device=X.device)
+    _lib.check(_lib.load().pf_cp_gram(_p(X), _p(Y), _p(idx), idx.numel(), _p(w), rs, cin, cout, _p(ws), int(chunk_rows),
+                                      _p(g), _stream()), 'pf_cp_gram')
+    return ws
+
+
+def cp_normal_eq(X, Y, cols, g, ws=None, chunk_rows=None, budget_bytes=1 << 30):
+    """[X_k | Y]^T [X_k | Y] in float64 over every row, X_k = the columns `cols` (int32) of X [N, K] (fp32), Y [N, Cout]
+    (float64): A = g[:k, :k], B = g[:k, k:] are the normal equations of the refit (channel_pruner.py:569-573)."""
+    _check_f32(X)
+    _check_f64(Y, g)
+    nrows, K = X.shape
+    cout = Y.shape[1]
+    ncols = cols.numel()
+    n = ncols + cout
+    if cols.dtype != torch.int32 or Y.shape[0] != nrows or g.numel() < n * n + 1:
+        raise ValueError('cp_normal_eq: cols must be int32, Y [N, Cout] and g float64 [(k + Cout)^2 + 1]')
+    if chunk_rows is None:
+        chunk_rows = int(max(1, min(nrows, budget_bytes // (8 * n))))
+    need = n * int(chunk_rows)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.float64, device=X.device)
+    _lib.check(_lib.load().pf_cp_normal_eq(_p(X), _p(Y), int(nrows), int(K), int(cout), _p(cols), int(ncols), _p(ws),
+                                           int(chunk_rows), _p(g), _stream()), 'pf_cp_normal_eq')
+    return ws
+
+
 class CprLstsq:
     """The least-squares refit of one layer (channel_pruning_rmt/learner.py:470-523, :814-842): min_W ||X W - Y||^2 /
     (2N) + wd ||W||^2 / 2 by `iters` Adam steps from the current kernel.  X W is a 1x1 conv over N "pixels" of
