@@ -64,6 +64,13 @@ def load_checkpoint(fn):
     return {k + ':0': v for k, v in tf_bundle.load(fn).items()}
 
 
+def calc_prune_ratio(tensors):
+    """Overall pruning ratio 1 - nnz/size (weight_sparsification/learner.py:51-65)."""
+    nnz = sum(int(torch.count_nonzero(t).item()) for t in tensors)
+    tot = sum(t.numel() for t in tensors)
+    return np.float32(np.float32(1.0) - np.float32(nnz) / np.float32(tot))
+
+
 class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
     """A learner takes a ModelHelper (data pipeline + model definition) and performs training or
     evaluation with its specific algorithm (abstract_learner.py:41-54)."""
@@ -100,7 +107,6 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         self.ckpt_file = 'models_%s_at_%s.tar.gz' % (self.model_name, self.dataset_name)
         self.graph_train = None
         self._iterator_eval = None
-        self.compact = None             # compact.CompactTrainer of a channel-pruning learner (--enbl_compact_ft)
 
     @abstractmethod
     def train(self):
@@ -157,6 +163,16 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
             return int(nb_iters)
         bs = self.iterator_train.batch_size if FLAGS.data_dir_local else FLAGS.batch_size_eval
         return int(np.ceil(float(FLAGS.nb_smpls_eval) / bs))
+
+    def eval_losses(self, nb_iters=None):
+        """fetch_losses() of each of eval_nb_iters(nb_iters) evaluation batches, run through sess_train's forward pass"""
+        ex = self.sess_train
+        out = []
+        for _ in range(self.eval_nb_iters(nb_iters)):
+            self.feed(ex, self.eval_iterator())
+            ex.forward_eval_loss()
+            out.append(ex.fetch_losses())
+        return out
 
     @classmethod
     def is_primary_worker(cls, scope='global'):
@@ -248,27 +264,6 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         iterator.copy_enqueued()
         ops.preprocess_images(dev[0], dev[1], dev_images)
         return nbytes + desc.numel() + labels.numel() * 4
-
-    # ------------------------------------------------------------------ fine-tuning at the pruned width
-    def start_compact_ft(self):
-        """--enbl_compact_ft, once the channels of `sess_train`'s masked model are chosen: the fine-tune steps run on a
-        compact executor planned from that state (compact.CompactTrainer); `sess_train` keeps evaluating and saving."""
-        if not FLAGS.enbl_compact_ft:
-            return
-        from ..compact import CompactTrainer
-        self.compact = CompactTrainer(self.sess_train)
-        if self.is_primary_worker('global'):
-            print('\n'.join(self.compact.report()))
-
-    @property
-    def sess_step(self):
-        """the executor whose run_step is one fine-tune step"""
-        return self.sess_train if self.compact is None else self.compact.ex
-
-    def sync_from_compact(self):
-        """before `sess_train` is saved or evaluated: expand the compact state into it"""
-        if self.compact is not None:
-            self.compact.push()
 
     def grad_allreduce(self):
         """The one collective of the data-parallel step (replaces DistributedOptimizer,

@@ -44,20 +44,15 @@ saves and fine-tunes at every group boundary) and cp_finetune / cp_retrain (whic
 --enbl_compact_ft is refused for this learner.  Flagged deviations: a conv with a fused activation (LeNet) has no
 materialised output to regress onto and is refused; a depthwise producer that is not itself W1-prunable (the
 reference would loop forever) has its own channels zeroed instead."""
-import os
 from timeit import default_timer as timer
 
 import numpy as np
 import torch
 
-from ... import graph as G
 from ... import ops
-from ...engine import Executor, ParamStore
 from ...flags import FLAGS, DEFINE_string, DEFINE_float, DEFINE_boolean, DEFINE_integer
-from ...utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
-from ..abstract_learner import AbstractLearner, latest_checkpoint, save_checkpoint
-from ..channel_pruning_gpu.learner import calc_prune_ratio
-from ..distillation_helper import DistillationHelper
+from ..abstract_learner import save_checkpoint
+from ..channel_pruning_base import ChannelPrunedBase
 from . import lars
 
 # learner.py:38-80
@@ -205,47 +200,19 @@ def sample_rows(pos, pos_add, bs, base):
     return rows
 
 
-class ChannelPrunedLearner(AbstractLearner):  # pylint: disable=too-many-instance-attributes
+class ChannelPrunedLearner(ChannelPrunedBase):  # pylint: disable=too-many-instance-attributes
+    SAVE_PATH_FLAG = 'save_path'
+
     def __init__(self, sm_writer, model_helper, seed=1):
         super(ChannelPrunedLearner, self).__init__(sm_writer, model_helper)
-        self.model_scope_full = 'model'
-        self.model_scope_prnd = 'pruned_model'
-        self.model_scope = self.model_scope_prnd
         self.seed = seed                                                   # of the host RandomState
-        if FLAGS.enbl_dst:
-            self.helper_dst = DistillationHelper(sm_writer, model_helper, self.mpi_comm)
-        self.__build()
+        self.sampled_prnd = sampled_tensors(self.conv_ops_prnd)
+        self.sampled_full = sampled_tensors(self.conv_ops_full)
 
     # ------------------------------------------------------------------ training
     def train(self, nb_iters=None):
-        if self.is_primary_worker('global'):
-            time_prev = timer()
-            self.choose_channels()
-            print('time (channel selection): %.2f (s)' % (timer() - time_prev))
-        self.auto_barrier()
-        ex = self.sess_train
-        self.restore_model(FLAGS.cp_channel_pruned_path)
-        self.init_masks()
-        if FLAGS.enbl_multi_gpu:
-            mgw.broadcast_global_variables([ex.store.P, ex.store.O])
-        time_prev = timer()
-        total = self.nb_iters_train if nb_iters is None else nb_iters
-        for idx_iter in range(total):
-            self.train_step()
-            if (idx_iter + 1) % FLAGS.summ_step == 0 and self.is_primary_worker('global'):
-                r = ex.fetch_losses()
-                speed = FLAGS.batch_size * FLAGS.summ_step / (timer() - time_prev) * (mgw.size() if FLAGS.enbl_multi_gpu else 1)
-                print('iter #%d: lr = %.4e | loss = %.4e | pr_krn = %.4e | speed = %.2f pics / sec'
-                      % (idx_iter + 1, self.lrn_rate(idx_iter), r['loss'], self.pr_maskable(), speed))
-                time_prev = timer()
-            if (idx_iter + 1) % FLAGS.save_step == 0:
-                if self.is_primary_worker('global'):
-                    self.__save_model()
-                    self.evaluate()
-                self.auto_barrier()
-        if self.is_primary_worker('global'):
-            self.__save_model()
-            self.evaluate()
+        self.select_on_primary(FLAGS.cp_channel_pruned_path)
+        self.fine_tune(nb_iters, save_first=False)
 
     def init_masks(self):
         """mask = kept input channels x kept output channels of every conv kernel (learner.py:406-419), read from the
@@ -262,105 +229,19 @@ class ChannelPrunedLearner(AbstractLearner):  # pylint: disable=too-many-instanc
         ex.reset_optimizer_state()
         ex.step_count = 0
 
-    def __save_model(self):
-        ex = self.sess_train
-        print('model saved to ' + save_checkpoint(FLAGS.save_path, ex.store.state_dict(), ex.step_count))
-
-    def train_step(self):
-        ex = self.sess_train
-        self.h2d_bytes = self.feed(ex, self.iterator_train)
-        ex.run_step(self.lrn_rate(ex.step_count), self.grad_allreduce())
-
-    def evaluate(self, nb_iters=None):
-        self.restore_for_eval(FLAGS.save_path)
-        ex = self.sess_train
-        out = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            out.append(ex.fetch_losses()['loss'])
-        return float(np.mean(out)), float(self.pr_maskable())
-
-    def pr_maskable(self):
-        return calc_prune_ratio([self.sess_train.store.view(v) for v in self.maskable_vars])
-
-    # ------------------------------------------------------------------ graph
-    def __build(self):
-        self.graph_train = G.Graph()
-        with self.graph_train.as_default():
-            with G.variable_scope(self.data_scope):
-                self.iterator_train = self.build_dataset_train()
-                images, labels = self.iterator_train.get_next()
-            self.images, self.labels = images, labels
-            logits_dst = self.helper_dst.calc_logits(None, images) if FLAGS.enbl_dst else None
-            with G.variable_scope(self.model_scope_full):
-                logits_full = self.forward_train(images)
-            with G.variable_scope(self.model_scope_prnd):
-                logits = self.forward_train(images)
-                loss, metrics = self.calc_loss(labels, logits, self.trainable_vars)
-                if FLAGS.enbl_dst:
-                    loss += self.helper_dst.calc_loss(logits, logits_dst)
-                self.lrn_rate, self.nb_iters_train = self.setup_lrn_rate(None)
-        conv_of = lambda scope: [op for op in self.graph_train.ops
-                                 if op.name.endswith('/Conv2D') and op.name.startswith(scope + '/')]
-        self.conv_ops_full, self.conv_ops_prnd = conv_of(self.model_scope_full), conv_of(self.model_scope_prnd)
-        assert len(self.conv_ops_full) == len(self.conv_ops_prnd)
-        self.maskable_vars = [op.vars['kernel'] for op in self.conv_ops_prnd]
-        self.nb_layers = len(self.conv_ops_prnd)
+    def layer_ratios(self):
+        """each layer's preserve ratio; list groups are refused first, before any executor is built"""
         refuse_list_groups(self.nb_layers, FLAGS.cp_prune_option, FLAGS.cp_list_group, FLAGS.cp_finetune,
                            FLAGS.cp_retrain)
-        self.prune_ratios = preserve_ratios(self.nb_layers, FLAGS.cp_prune_option, FLAGS.cp_uniform_preserve_ratio,
-                                            FLAGS.cp_prune_list_file)
-        world = mgw.size() if FLAGS.enbl_multi_gpu else 1
-        teacher = None
-        if FLAGS.enbl_dst:
-            teacher = Executor(self.graph_train, images, logits_dst, self.device, train=False, seed=2)
-            self.helper_dst.restore(teacher.store)
-        self.sess_train = Executor(self.graph_train, images, logits, self.device, train=True, loss=loss, labels=labels,
-                                   optimizer=dict(kind='momentum', momentum=FLAGS.momentum),
-                                   maskable=self.maskable_vars, teacher=teacher, seed=1, grad_scale=1.0 / world)
-        if teacher is not None:
-            teacher.buf[images] = self.sess_train.buf[images]
-            self.sess_train.share_im2col_from(teacher)
-        self.logits_full, self.logits_prnd = logits_full, logits
-        self.store_full = ParamStore([v for v in self.graph_train.variables.values()
-                                      if v.name.startswith(self.model_scope_full + '/')], self.device, seed=1)
-        self.sampled_prnd = sampled_tensors(self.conv_ops_prnd)
-        self.sampled_full = sampled_tensors(self.conv_ops_full)
-
-    def init_from_full(self):
-        """restore the full model from the pre-trained checkpoint and copy it into the model to be pruned"""
-        ex = self.sess_train
-        ckpt_dir = os.path.dirname(FLAGS.save_path)
-        if os.path.isdir(ckpt_dir) and latest_checkpoint(ckpt_dir) is not None:
-            self.restore_model(FLAGS.save_path, store=self.store_full)
-        elif FLAGS.data_dir_local:
-            raise ValueError('channel pruning of a real model needs its pre-trained checkpoint in ' + ckpt_dir)
-        else:
-            print('no pre-trained checkpoint in %s: the full model keeps its seed initialisation (synthetic run)' % ckpt_dir)
-        full = self.store_full.state_dict()
-        renamed = {self.model_scope_prnd + k[len(self.model_scope_full):]: v for k, v in full.items()}
-        ex.store.load_state_dict(renamed, strict=True)
+        return preserve_ratios(self.nb_layers, FLAGS.cp_prune_option, FLAGS.cp_uniform_preserve_ratio,
+                               FLAGS.cp_prune_list_file)
 
     # ------------------------------------------------------------------ channel selection
-    def selection_executors(self):
-        """the full and the pruned model for sampling: forward only, training-mode BN without moving-average updates,
-        every conv and Add output materialised; one image buffer feeds both"""
-        ex_p = Executor(self.graph_train, self.images, self.logits_prnd, self.device, store=self.sess_train.store,
-                        train=False, fuse_add=False, update_moving_stats=False)
-        ex_f = Executor(self.graph_train, self.images, self.logits_full, self.device, store=self.store_full,
-                        train=False, fuse_add=False, update_moving_stats=False)
-        ex_f.buf[self.images] = ex_p.buf[self.images]
-        return ex_f, ex_p
-
-    def cache_batches(self):
-        """cp_nb_batches training mini-batches, drawn once (:310-314), kept on the device"""
-        ex = self.sess_train
-        cached = []
-        for _ in range(FLAGS.cp_nb_batches):
-            self.feed(ex, self.iterator_train)
-            cached.append(ex.buf[self.images].clone())
-        return cached
+    def cache_batches(self, nb_batches=None):
+        """cp_nb_batches training mini-batches by default, drawn once (:310-314)"""
+        if nb_batches is None:
+            nb_batches = FLAGS.cp_nb_batches
+        return super(ChannelPrunedLearner, self).cache_batches(nb_batches)
 
     def choose_channels(self, cached=None):
         """compress() over every layer (learner.py:513-529), then save to cp_channel_pruned_path"""
@@ -389,9 +270,7 @@ class ChannelPrunedLearner(AbstractLearner):  # pylint: disable=too-many-instanc
         """X [N, R*S*Cin] (fp32) and Y [N, Cout] (float64) of one layer on the device, N = batches x batch x points"""
         op_f, op_p = self.conv_ops_full[idx_layer], self.conv_ops_prnd[idx_layer]
         for ex_, op in ((ex_f, op_f), (ex_p, op_p)):
-            if op in ex_.fused_act:
-                raise ValueError('%s: a conv with a fused activation has no materialised output to regress onto'
-                                 % op.name)
+            self.check_regressable(ex_, op)
         add_f, add_p = add_after(op_f), add_after(op_p)
         t_conv = self.sampled_prnd.index(op_p)
         t_add = self.sampled_prnd.index(add_p) if add_p is not None else None

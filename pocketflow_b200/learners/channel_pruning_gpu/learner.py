@@ -26,15 +26,10 @@ from timeit import default_timer as timer
 import numpy as np
 import torch
 
-import os
-
-from ... import graph as G
 from ... import ops
-from ...engine import Executor, ParamStore
 from ...flags import FLAGS, DEFINE_string, DEFINE_float, DEFINE_boolean, DEFINE_integer
 from ...utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
-from ..abstract_learner import AbstractLearner, latest_checkpoint, save_checkpoint
-from ..distillation_helper import DistillationHelper
+from ..channel_pruning_base import ChannelPrunedBase
 
 DEFINE_string('cpg_save_path', './models_cpg/model.ckpt', 'CPG: model\'s save path')
 DEFINE_string('cpg_save_path_eval', './models_cpg_eval/model.ckpt', 'CPG: model\'s save path for evaluation')
@@ -49,72 +44,28 @@ DEFINE_float('cpg_lrn_rate_adam', 1e-2, 'CPG: Adam\'s initial learning rate')
 DEFINE_integer('cpg_nb_iters_layer', 1000, 'CPG: # of iterations for layer-wise FT')
 
 
-def calc_prune_ratio(tensors):
-    nnz = sum(int(torch.count_nonzero(t).item()) for t in tensors)
-    tot = sum(t.numel() for t in tensors)
-    return np.float32(np.float32(1.0) - np.float32(nnz) / np.float32(tot))
+class ChannelPrunedGpuLearner(ChannelPrunedBase):  # pylint: disable=too-many-instance-attributes
+    # the selection regresses on the step executor's own conv outputs, so no residual Add is fused into them
+    FUSE_ADD = False
+    SAVE_PATH_FLAG = 'cpg_save_path'
 
-
-class ChannelPrunedGpuLearner(AbstractLearner):  # pylint: disable=too-many-instance-attributes
     def __init__(self, sm_writer, model_helper):
         super(ChannelPrunedGpuLearner, self).__init__(sm_writer, model_helper)
-        # scopes of the full & channel-pruned models (:126-128); `vars` / `trainable_vars` are the pruned model's
-        self.model_scope_full = 'model'
-        self.model_scope_prnd = 'pruned_model'
-        self.model_scope = self.model_scope_prnd
-        if FLAGS.enbl_dst:
-            self.helper_dst = DistillationHelper(sm_writer, model_helper, self.mpi_comm)
         self.channels_chosen = False
-        self.__build()
+        # the full model's executor, built lazily: it is only needed while channels are being chosen
+        self.sess_full = None
 
     # ------------------------------------------------------------------ training
     def train(self, nb_iters=None):
-        ex = self.sess_train
         self.init_from_full()
         # choose channels and evaluate the model before re-training (:152-157)
         self.choose_channels()
-        self.start_compact_ft()
-        ex = self.sess_step
-        if self.is_primary_worker('global'):
-            self.__save_model()
-            self.evaluate()
-        self.auto_barrier()
-        time_prev = timer()
-        total = self.nb_iters_train if nb_iters is None else nb_iters
-        for idx_iter in range(total):
-            self.train_step()
-            if (idx_iter + 1) % FLAGS.summ_step == 0 and self.is_primary_worker('global'):
-                r = ex.fetch_losses()
-                speed = FLAGS.batch_size * FLAGS.summ_step / (timer() - time_prev) * (mgw.size() if FLAGS.enbl_multi_gpu else 1)
-                print('iter #%d: lr = %.4e | loss = %.4e | pr_msk = %.4e | speed = %.2f pics / sec'
-                      % (idx_iter + 1, self.lrn_rate(idx_iter), r['loss'], self.pr_maskable(), speed))
-                time_prev = timer()
-            # save the model at certain steps (learner.py:171-175).  The reference barriers after EVERY iteration; the
-            # gradient all-reduce already keeps the ranks in step, so only the iterations where the primary worker
-            # does extra work need one (a per-step NCCL barrier would drain the device queue every step).
-            if (idx_iter + 1) % FLAGS.save_step == 0:
-                if self.is_primary_worker('global'):
-                    self.__save_model()
-                    self.evaluate()
-                self.auto_barrier()
-        if self.is_primary_worker('global'):
-            self.__save_model()
-            self.evaluate()
+        self.fine_tune(nb_iters, label='pr_msk')
 
     def init_from_full(self):
-        """Restore the full model from the pre-trained checkpoint, copy it into the pruned model, masks = 1, fresh
-        optimizers, broadcast (:141-149, :283-289)."""
+        """restore_full(), then masks = 1, fresh optimizers, broadcast (:141-149, :283-289)"""
+        self.restore_full()
         ex = self.sess_train
-        ckpt_dir = os.path.dirname(FLAGS.save_path)
-        if os.path.isdir(ckpt_dir) and latest_checkpoint(ckpt_dir) is not None:
-            self.restore_model(FLAGS.save_path, store=self.store_full)
-        elif FLAGS.data_dir_local:
-            raise ValueError('channel pruning of a real model needs its pre-trained checkpoint in ' + ckpt_dir)
-        else:
-            print('no pre-trained checkpoint in %s: the full model keeps its seed initialisation (synthetic run)' % ckpt_dir)
-        full = self.store_full.state_dict()
-        renamed = {self.model_scope_prnd + k[len(self.model_scope_full):]: v for k, v in full.items()}
-        ex.store.load_state_dict(renamed, strict=True)
         ex.MASK.fill_(1.0)
         ex.reset_optimizer_state()
         ex.step_count = 0
@@ -122,79 +73,7 @@ class ChannelPrunedGpuLearner(AbstractLearner):  # pylint: disable=too-many-inst
         if FLAGS.enbl_multi_gpu:
             mgw.broadcast_global_variables([ex.store.P, ex.store.O, self.store_full.P, self.store_full.O])
 
-    def __save_model(self):
-        self.sync_from_compact()
-        ex = self.sess_train
-        print('model saved to ' + save_checkpoint(FLAGS.cpg_save_path, ex.store.state_dict(), ex.step_count))
-
-    def train_step(self):
-        ex = self.sess_step
-        self.h2d_bytes = self.feed(self.sess_train, self.iterator_train)
-        ex.run_step(self.lrn_rate(ex.step_count), self.grad_allreduce())
-
-    def evaluate(self, nb_iters=None):
-        self.restore_for_eval(FLAGS.cpg_save_path)
-        ex = self.sess_train
-        out = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            out.append(ex.fetch_losses()['loss'])
-        return float(np.mean(out)), float(self.pr_maskable())
-
-    def pr_maskable(self):
-        return calc_prune_ratio([self.sess_train.store.view(v) for v in self.maskable_vars])
-
-    # ------------------------------------------------------------------ graph
-    def __build(self):
-        self.graph_train = G.Graph()
-        with self.graph_train.as_default():
-            with G.variable_scope(self.data_scope):
-                self.iterator_train = self.build_dataset_train()
-                images, labels = self.iterator_train.get_next()
-            self.images, self.labels = images, labels
-            logits_dst = self.helper_dst.calc_logits(None, images) if FLAGS.enbl_dst else None
-            # model definition - full model (:207-212)
-            with G.variable_scope(self.model_scope_full):
-                logits_full = self.forward_train(images)
-            # model definition - channel-pruned model (:214-229)
-            with G.variable_scope(self.model_scope_prnd):
-                logits = self.forward_train(images)
-                loss, metrics = self.calc_loss(labels, logits, self.trainable_vars)
-                if FLAGS.enbl_dst:
-                    loss += self.helper_dst.calc_loss(logits, logits_dst)
-                self.lrn_rate, self.nb_iters_train = self.setup_lrn_rate(None)
-        # maskable = trainable variables read by ops named .../Conv2D (depthwise excluded) (:52-66); the i-th Conv2D
-        # of the full model is regressed onto by the i-th of the pruned model (:347-352)
-        conv_of = lambda scope: [op for op in self.graph_train.ops
-                                 if op.name.endswith('/Conv2D') and op.name.startswith(scope + '/')]
-        self.conv_ops_full, self.conv_ops_prnd = conv_of(self.model_scope_full), conv_of(self.model_scope_prnd)
-        assert len(self.conv_ops_full) == len(self.conv_ops_prnd)
-        self.maskable_vars = [op.vars['kernel'] for op in self.conv_ops_prnd]
-        self.maskable_var_names = [v.name for v in self.maskable_vars]
-        self.nb_layers = len(self.conv_ops_prnd)
-        world = mgw.size() if FLAGS.enbl_multi_gpu else 1
-        teacher = None
-        if FLAGS.enbl_dst:
-            teacher = Executor(self.graph_train, images, logits_dst, self.device, train=False, seed=2)
-            self.helper_dst.restore(teacher.store)
-        # both models start from the same seed: the pruned model IS the full model until channels are chosen
-        self.sess_train = Executor(self.graph_train, images, logits, self.device, train=True, loss=loss, labels=labels,
-                                   optimizer=dict(kind='momentum', momentum=FLAGS.momentum),
-                                   maskable=self.maskable_vars, teacher=teacher, seed=1, grad_scale=1.0 / world,
-                                   fuse_add=False)
-        if teacher is not None:
-            teacher.buf[images] = self.sess_train.buf[images]
-            self.sess_train.share_im2col_from(teacher)
-        # the full model: forward only, training-mode BN without moving-average updates (only the pruned scope's
-        # update ops are ever run, :283-286); built lazily — it is only needed while channels are being chosen
-        self.logits_full = logits_full
-        self.sess_full = None
-        self.store_full = ParamStore([v for v in self.graph_train.variables.values()
-                                      if v.name.startswith(self.model_scope_full + '/')], self.device, seed=1)
-        self.prune_ratios = self.__prune_ratio_list()
-
-    def __prune_ratio_list(self):
+    def layer_ratios(self):
         """each layer's pruning ratio (:448-459)"""
         if FLAGS.cpg_prune_ratio_type == 'uniform':
             ratios = [FLAGS.cpg_prune_ratio] * self.nb_layers
@@ -211,10 +90,7 @@ class ChannelPrunedGpuLearner(AbstractLearner):  # pylint: disable=too-many-inst
     # ------------------------------------------------------------------ channel selection (:445-518)
     def __selection_state(self):
         if self.sess_full is None:
-            ex = self.sess_train
-            self.sess_full = Executor(self.graph_train, self.images, self.logits_full, self.device, store=self.store_full,
-                                      train=False, fuse_add=False, update_moving_stats=False)
-            self.sess_full.buf[self.images] = ex.buf[self.images]          # one mini-batch feeds both models
+            self.sess_full = self.full_executor(self.sess_train.buf[self.images])    # one mini-batch feeds both models
             dev = self.device
             nmax = max(op.output.numel for op in self.conv_ops_prnd)
             self._sel = dict(diff=torch.empty(nmax, dtype=torch.float32, device=dev),

@@ -3,9 +3,10 @@
 Two copies of the network live in one graph, as in the reference (:332-379): the FULL model under scope 'model'
 (restored from the pre-trained checkpoint, never trained) and the channel-pruned model under 'pruned_model'
 (initialised from the full one, :375-379).  train() = channel selection, layer by layer (:546-649), then whole-network
-fine-tuning with masked gradients (:146-193).  The layers are the kernels read by ops named .../Conv2D (depthwise
-convs excluded, MobileNet's logits conv and ResNet's projection convs included, :54-77); the i-th Conv2D of the full
-model is paired with the i-th of the pruned model (:396-430).
+fine-tuning with masked gradients (:146-193); evaluate() reads cpr_save_path's latest checkpoint (:195-209, :857-869).
+The layers are the kernels read by ops named .../Conv2D (depthwise convs excluded, MobileNet's logits conv and ResNet's
+projection convs included, :54-77); the i-th Conv2D of the full model is paired with the i-th of the pruned model
+(:396-430).
 
 Selection of layer i (no gradient descent on the network):
   * sampling (:608-631, :651-725): ceil(cpr_nb_smpls / batch_size) training mini-batches are drawn once and reused
@@ -44,20 +45,15 @@ deviations: (a) producer channels that no consumer reads are frozen at their pos
 under weight decay, and the reported loss omits their L2 term; they cannot influence the logits either way; (b) the
 fp32 accumulation order of a narrowed K dimension differs from the masked one, so logits agree to rounding."""
 import math
-import os
 from timeit import default_timer as timer
 
 import numpy as np
 import torch
 
-from ... import graph as G
 from ... import ops
-from ...engine import Executor, ParamStore
 from ...flags import FLAGS, DEFINE_string, DEFINE_float, DEFINE_boolean, DEFINE_integer
-from ...utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
-from ..abstract_learner import AbstractLearner, latest_checkpoint, save_checkpoint
-from ..channel_pruning_gpu.learner import calc_prune_ratio
-from ..distillation_helper import DistillationHelper
+from ..abstract_learner import save_checkpoint
+from ..channel_pruning_base import ChannelPrunedBase
 
 DEFINE_string('cpr_save_path', './models_cpr/model.ckpt', 'CPR: model\'s save path')
 DEFINE_string('cpr_save_path_eval', './models_cpr_eval/model.ckpt', 'CPR: model\'s save path for evaluation')
@@ -161,56 +157,17 @@ def gamma_search(solve, nnz_target):
     return log
 
 
-class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-instance-attributes
+class ChannelPrunedRmtLearner(ChannelPrunedBase):  # pylint: disable=too-many-instance-attributes
+    SAVE_PATH_FLAG = 'cpr_save_path'
+
     def __init__(self, sm_writer, model_helper, seed=1):
         super(ChannelPrunedRmtLearner, self).__init__(sm_writer, model_helper)
-        self.model_scope_full = 'model'
-        self.model_scope_prnd = 'pruned_model'
-        self.model_scope = self.model_scope_prnd
         self.seed = seed                                                   # of the host RandomState
-        if FLAGS.enbl_dst:
-            self.helper_dst = DistillationHelper(sm_writer, model_helper, self.mpi_comm)
-        self.__build()
 
     # ------------------------------------------------------------------ training (:146-193)
     def train(self, nb_iters=None):
-        ex = self.sess_train
-        if not FLAGS.cpr_warm_start:
-            if self.is_primary_worker('global'):
-                time_prev = timer()
-                self.choose_channels()
-                print('time (channel selection): %.2f (s)' % (timer() - time_prev))
-            self.auto_barrier()
-        self.restore_model(FLAGS.cpr_save_path_ws)
-        self.init_masks()
-        if FLAGS.enbl_multi_gpu:
-            mgw.broadcast_global_variables([ex.store.P, ex.store.O])
-        self.start_compact_ft()
-        ex = self.sess_step
-        if self.is_primary_worker('global'):
-            self.__save_model()
-            self.evaluate()
-        self.auto_barrier()
-        time_prev = timer()
-        total = self.nb_iters_train if nb_iters is None else nb_iters
-        for idx_iter in range(total):
-            self.train_step()
-            if (idx_iter + 1) % FLAGS.summ_step == 0 and self.is_primary_worker('global'):
-                r = ex.fetch_losses()
-                speed = FLAGS.batch_size * FLAGS.summ_step / (timer() - time_prev) * (mgw.size() if FLAGS.enbl_multi_gpu else 1)
-                print('iter #%d: lr = %.4e | loss = %.4e | pr_krn = %.4e | speed = %.2f pics / sec'
-                      % (idx_iter + 1, self.lrn_rate(idx_iter), r['loss'], self.pr_maskable(), speed))
-                time_prev = timer()
-            # (the gradient all-reduce keeps the ranks in step: a barrier only where the primary worker saves)
-            if (idx_iter + 1) % FLAGS.save_step == 0:
-                if self.is_primary_worker('global'):
-                    self.__save_model()
-                    self.evaluate()
-                self.auto_barrier()
-        if self.is_primary_worker('global'):
-            self.__save_model()
-            print('model saved to ' + save_checkpoint(FLAGS.cpr_save_path_eval, self.sess_train.store.state_dict()))
-            self.evaluate()
+        self.select_on_primary(FLAGS.cpr_save_path_ws, select=not FLAGS.cpr_warm_start)
+        self.fine_tune(nb_iters, path_eval=FLAGS.cpr_save_path_eval)
 
     def init_masks(self):
         """masks = reduce_sum(W^2, [0, 1, 3]) > 0 per input channel (:255-263), fresh optimizer state (:159)"""
@@ -220,105 +177,16 @@ class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-inst
         ex.reset_optimizer_state()
         ex.step_count = 0
 
-    def __save_model(self):
-        self.sync_from_compact()
-        ex = self.sess_train
-        print('model saved to ' + save_checkpoint(FLAGS.cpr_save_path, ex.store.state_dict(), ex.step_count))
-
-    def train_step(self):
-        ex = self.sess_step
-        self.h2d_bytes = self.feed(self.sess_train, self.iterator_train)
-        ex.run_step(self.lrn_rate(ex.step_count), self.grad_allreduce())
-
-    def evaluate(self, nb_iters=None):
-        """restore the latest checkpoint of cpr_save_path's directory (:195-209, :857-869) and evaluate"""
-        self.restore_for_eval(FLAGS.cpr_save_path)
-        ex = self.sess_train
-        out = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            out.append(ex.fetch_losses()['loss'])
-        return float(np.mean(out)), float(self.pr_maskable())
-
-    def pr_maskable(self):
-        return calc_prune_ratio([self.sess_train.store.view(v) for v in self.maskable_vars])
-
-    # ------------------------------------------------------------------ graph
-    def __build(self):
-        self.graph_train = G.Graph()
-        with self.graph_train.as_default():
-            with G.variable_scope(self.data_scope):
-                self.iterator_train = self.build_dataset_train()
-                images, labels = self.iterator_train.get_next()
-            self.images, self.labels = images, labels
-            logits_dst = self.helper_dst.calc_logits(None, images) if FLAGS.enbl_dst else None
-            with G.variable_scope(self.model_scope_full):
-                logits_full = self.forward_train(images)
-            with G.variable_scope(self.model_scope_prnd):
-                logits = self.forward_train(images)
-                loss, metrics = self.calc_loss(labels, logits, self.trainable_vars)
-                if FLAGS.enbl_dst:
-                    loss += self.helper_dst.calc_loss(logits, logits_dst)
-                self.lrn_rate, self.nb_iters_train = self.setup_lrn_rate(None)
-        conv_of = lambda scope: [op for op in self.graph_train.ops
-                                 if op.name.endswith('/Conv2D') and op.name.startswith(scope + '/')]
-        self.conv_ops_full, self.conv_ops_prnd = conv_of(self.model_scope_full), conv_of(self.model_scope_prnd)
-        assert len(self.conv_ops_full) == len(self.conv_ops_prnd)
-        self.maskable_vars = [op.vars['kernel'] for op in self.conv_ops_prnd]
-        self.nb_layers = len(self.conv_ops_prnd)
-        world = mgw.size() if FLAGS.enbl_multi_gpu else 1
-        teacher = None
-        if FLAGS.enbl_dst:
-            teacher = Executor(self.graph_train, images, logits_dst, self.device, train=False, seed=2)
-            self.helper_dst.restore(teacher.store)
-        self.sess_train = Executor(self.graph_train, images, logits, self.device, train=True, loss=loss, labels=labels,
-                                   optimizer=dict(kind='momentum', momentum=FLAGS.momentum),
-                                   maskable=self.maskable_vars, teacher=teacher, seed=1, grad_scale=1.0 / world)
-        if teacher is not None:
-            teacher.buf[images] = self.sess_train.buf[images]
-            self.sess_train.share_im2col_from(teacher)
-        self.logits_full, self.logits_prnd = logits_full, logits
-        self.store_full = ParamStore([v for v in self.graph_train.variables.values()
-                                      if v.name.startswith(self.model_scope_full + '/')], self.device, seed=1)
-        self.prune_ratios = prune_ratio_list([v.name for v in self.maskable_vars], FLAGS.cpr_prune_ratio,
-                                             FLAGS.cpr_skip_frst_layer, FLAGS.cpr_skip_last_layer,
-                                             FLAGS.cpr_skip_op_names)
-
-    def init_from_full(self):
-        """restore the full model from the pre-trained checkpoint and copy it into the pruned model (:355-379)"""
-        ex = self.sess_train
-        ckpt_dir = os.path.dirname(FLAGS.save_path)
-        if os.path.isdir(ckpt_dir) and latest_checkpoint(ckpt_dir) is not None:
-            self.restore_model(FLAGS.save_path, store=self.store_full)
-        elif FLAGS.data_dir_local:
-            raise ValueError('channel pruning of a real model needs its pre-trained checkpoint in ' + ckpt_dir)
-        else:
-            print('no pre-trained checkpoint in %s: the full model keeps its seed initialisation (synthetic run)' % ckpt_dir)
-        full = self.store_full.state_dict()
-        renamed = {self.model_scope_prnd + k[len(self.model_scope_full):]: v for k, v in full.items()}
-        ex.store.load_state_dict(renamed, strict=True)
+    def layer_ratios(self):
+        return prune_ratio_list([v.name for v in self.maskable_vars], FLAGS.cpr_prune_ratio, FLAGS.cpr_skip_frst_layer,
+                                FLAGS.cpr_skip_last_layer, FLAGS.cpr_skip_op_names)
 
     # ------------------------------------------------------------------ channel selection (:546-649)
-    def selection_executors(self):
-        """the full and the pruned model for sampling: forward only, training-mode BN without moving-average updates,
-        every conv output materialised; one image buffer feeds both"""
-        ex_p = Executor(self.graph_train, self.images, self.logits_prnd, self.device, store=self.sess_train.store,
-                        train=False, fuse_add=False, update_moving_stats=False)
-        ex_f = Executor(self.graph_train, self.images, self.logits_full, self.device, store=self.store_full,
-                        train=False, fuse_add=False, update_moving_stats=False)
-        ex_f.buf[self.images] = ex_p.buf[self.images]
-        return ex_f, ex_p
-
-    def cache_batches(self):
-        """ceil(cpr_nb_smpls / batch_size) training mini-batches, drawn once (:579-582), kept on the device"""
-        nb_mbtcs = int(math.ceil(FLAGS.cpr_nb_smpls / FLAGS.batch_size))
-        ex = self.sess_train
-        cached = []
-        for _ in range(nb_mbtcs):
-            self.feed(ex, self.iterator_train)
-            cached.append(ex.buf[self.images].clone())
-        return cached
+    def cache_batches(self, nb_batches=None):
+        """ceil(cpr_nb_smpls / batch_size) training mini-batches by default, drawn once (:579-582)"""
+        if nb_batches is None:
+            nb_batches = int(math.ceil(FLAGS.cpr_nb_smpls / FLAGS.batch_size))
+        return super(ChannelPrunedRmtLearner, self).cache_batches(nb_batches)
 
     def choose_channels(self, cached=None):
         """Choose channels for all convolutional layers (:546-649), save the result to cpr_save_path_ws."""
@@ -343,9 +211,7 @@ class ChannelPrunedRmtLearner(AbstractLearner):  # pylint: disable=too-many-inst
         """sampling, sparse regression and refit of one layer; returns its log record"""
         op_f, op_p = self.conv_ops_full[idx_layer], self.conv_ops_prnd[idx_layer]
         for ex_, op in ((ex_f, op_f), (ex_p, op_p)):
-            if op in ex_.fused_act:
-                raise ValueError('%s: a conv with a fused activation has no materialised output to regress onto'
-                                 % op.name)
+            self.check_regressable(ex_, op)
         ratio = self.prune_ratios[idx_layer]
         dev = self.device
         w_p = self.sess_train.store.view(op_p.vars['kernel'])

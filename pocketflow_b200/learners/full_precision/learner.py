@@ -56,12 +56,7 @@ class FullPrecLearner(AbstractLearner):  # pylint: disable=too-many-instance-att
 
     def evaluate(self, nb_iters=None):
         self.restore_for_eval(FLAGS.save_path)
-        ex = self.sess_train
-        out = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            out.append(ex.fetch_losses()['loss'])
+        out = [r['loss'] for r in self.eval_losses(nb_iters)]
         print('loss = %.4e' % np.mean(out))
         return float(np.mean(out))
 

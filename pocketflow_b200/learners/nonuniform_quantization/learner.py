@@ -127,12 +127,7 @@ class NonUniformQuantLearner(AbstractLearner):
         if not self.is_primary_worker():
             return None
         self.restore_for_eval(FLAGS.nuql_save_quant_model_path)
-        ex = self.sess_train
-        out = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            out.append(ex.fetch_losses()['loss'])
+        out = [r['loss'] for r in self.eval_losses(nb_iters)]
         if FLAGS.nuql_use_buckets:
             self.__show_bucket_storage(self.bucket_storage)
         return float(np.mean(out))

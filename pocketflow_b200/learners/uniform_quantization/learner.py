@@ -114,14 +114,8 @@ class UniformQuantLearner(AbstractLearner):
         if not self.is_primary_worker():
             return None
         self.restore_for_eval(FLAGS.uql_save_quant_model_path)
-        ex = self.sess_train
-        losses, accuracies = [], []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            r = ex.fetch_losses()
-            losses.append(r['loss'])
-            accuracies.append(r['acc_top1'])
+        rows = self.eval_losses(nb_iters)
+        losses, accuracies = [r['loss'] for r in rows], [r['acc_top1'] for r in rows]
         print('loss: {}'.format(np.mean(np.array(losses))))
         print('accuracy: {}'.format(np.mean(np.array(accuracies))))
         if FLAGS.uql_use_buckets:

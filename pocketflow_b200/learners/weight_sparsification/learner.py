@@ -14,7 +14,7 @@ from ... import ops
 from ...engine import Executor, ParamStore
 from ...flags import FLAGS, DEFINE_string, DEFINE_float, DEFINE_integer
 from ...utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
-from ..abstract_learner import AbstractLearner, latest_checkpoint, load_checkpoint, save_checkpoint
+from ..abstract_learner import AbstractLearner, calc_prune_ratio, latest_checkpoint, load_checkpoint, save_checkpoint
 from ..distillation_helper import DistillationHelper
 from .pr_optimizer import PROptimizer
 from .utils import get_maskable_vars
@@ -34,13 +34,6 @@ DEFINE_float('ws_prune_ratio_exp', 3.0, 'WS: pruning ratio\'s exponent term')
 DEFINE_float('ws_iter_ratio_beg', 0.1, 'WS: iteration ratio (at starting time)')
 DEFINE_float('ws_iter_ratio_end', 0.5, 'WS: iteration ratio (at ending time)')
 DEFINE_float('ws_mask_update_step', 500, 'WS: step size for updating the pruning mask')
-
-
-def calc_prune_ratio(tensors):
-    """Overall pruning ratio 1 - nnz/size (learner.py:51-65)."""
-    nnz = sum(int(torch.count_nonzero(t).item()) for t in tensors)
-    tot = sum(t.numel() for t in tensors)
-    return np.float32(np.float32(1.0) - np.float32(nnz) / np.float32(tot))
 
 
 class WeightSparseLearner(AbstractLearner):  # pylint: disable=too-many-instance-attributes
@@ -98,11 +91,7 @@ class WeightSparseLearner(AbstractLearner):  # pylint: disable=too-many-instance
     def evaluate(self, nb_iters=None):
         self.restore_for_eval(FLAGS.ws_save_path)
         ex = self.sess_train
-        losses = []
-        for _ in range(self.eval_nb_iters(nb_iters)):
-            self.feed(ex, self.eval_iterator())
-            ex.forward_eval_loss()
-            losses.append(ex.fetch_losses()['loss'])
+        losses = [r['loss'] for r in self.eval_losses(nb_iters)]
         pr = calc_prune_ratio([ex.store.view(v) for v in self.maskable_vars])
         print('loss = %.4e | pr_msk = %.4e' % (np.mean(losses), pr))
         return float(np.mean(losses)), float(pr)

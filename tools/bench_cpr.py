@@ -49,6 +49,7 @@ def main():
     args = ap.parse_args()
     from pocketflow_b200.flags import FLAGS
     from pocketflow_b200.learners.learner_utils import create_learner
+    import pocketflow_b200.learners.channel_pruning_rmt.learner  # noqa: F401  (declares the learner's flags)
     FLAGS.reset()
     if args.net == 'mobilenet':
         from pocketflow_b200.nets import mobilenet_at_ilsvrc12 as M
