@@ -709,6 +709,46 @@ typedef struct pf_img_desc {
 } pf_img_desc;
 int pf_preprocess_images(const uint8_t* crops_dev, const pf_img_desc* desc_dev, int n, int out_h, int out_w,
                          float mean_r, float mean_g, float mean_b, float* dst_dev, void* stream);
+
+/* Baseline JPEG decoding for the input pipeline (pf_jpeg.cu), bit for bit with libjpeg-turbo's default
+ * decompression (islow IDCT, fancy upsampling, YCbCr -> RGB) as Pillow runs it.  The host parses the headers
+ * (pocketflow_b200/datasets/jpeg.py) and only hands over files the device supports: 8-bit, one interleaved sequential
+ * Huffman scan, grey or YCbCr with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1.
+ *   data_dev    : every image's entropy-coded segment (desc.scan_offset / scan_bytes)
+ *   coef_ws_dev : int16 workspace, 64 per block of MCU rows [0, mcu_rows) of each image from desc.coef_offset on
+ *                 (mcus_per_row * mcu_rows * blocks per MCU * 128 bytes per image)
+ *   crops_dev   : uint8 [crop_h, crop_w, 3] RGB written at desc.crop_offset
+ *   status_dev  : int32 [n], 0 = decoded; otherwise the image's data is anomalous (1 bad Huffman code, 2 data ends
+ *                 early, 3 bad restart marker, 4 run past coefficient 63, 5 bad descriptor: a field out of range, or an
+ *                 MCU window that does not hold every block the crop and its upsampling context read), its crop is
+ *                 not written and the host has to decode it.  An anomaly never touches another image's crop or
+ *                 workspace.  The caller guarantees that data_dev, coef_ws_dev and crops_dev hold what each
+ *                 descriptor's offsets and sizes point at (datasets/jpeg.py: pack, workspace_elems). */
+typedef struct pf_jpeg_huff {
+  int16_t lookup[256];    /* next 8 bits -> (code length << 8) | symbol; 0: the code is longer than 8 bits */
+  int32_t maxcode[18];    /* largest code of each length (-1: none), as jdhuff.c derives it */
+  int32_t valoffset[18];  /* huffval index = code + valoffset[length] */
+  uint8_t huffval[256];
+} pf_jpeg_huff;
+typedef struct pf_jpeg_desc {
+  int64_t scan_offset;     /* first byte of the entropy-coded segment in data_dev */
+  int64_t coef_offset;     /* first int16 of this image's workspace (a multiple of 64) */
+  int64_t crop_offset;     /* first byte of the crop in crops_dev */
+  int32_t scan_bytes;
+  int32_t height, width;
+  int32_t ncomp;           /* 1 (grey) or 3 (YCbCr) */
+  int32_t hs, vs;          /* luma sampling factors; chroma is 1x1 */
+  int32_t restart_interval;/* MCUs per restart interval, 0: none */
+  int32_t mcus_per_row;
+  int32_t mcu_rows;        /* MCU rows entropy-decoded: through the last one the crop needs */
+  int32_t mcu_row0, mcu_col0, mcu_col1;  /* MCU window inverse-transformed: rows [mcu_row0, mcu_rows) */
+  int32_t crop_y, crop_x, crop_h, crop_w;
+  int32_t dc_tbl[3], ac_tbl[3];          /* per component: index into huff[] */
+  uint16_t quant[3][64];   /* per component, zig-zag order */
+  pf_jpeg_huff huff[4];
+} pf_jpeg_desc;
+int pf_jpeg_decode(const uint8_t* data_dev, const pf_jpeg_desc* desc_dev, int n, int16_t* coef_ws_dev,
+                   uint8_t* crops_dev, int32_t* status_dev, void* stream);
 /* tf.reduce_mean over H,W (resnet_model.py:547-548) */
 int pf_global_avgpool_fwd(const float* x_dev, int n, int hw, int c, float* y_dev, void* stream);
 int pf_global_avgpool_bwd(const float* dy_dev, int n, int hw, int c, int accumulate, float* dx_dev, void* stream);

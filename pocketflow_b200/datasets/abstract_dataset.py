@@ -124,6 +124,34 @@ class PackedBatchIterator(BatchIterator):
         return slot[0], int(crops.size), slot[1], slot[2]
 
 
+class DecodeBatchIterator(PackedBatchIterator):
+    """Mini-batches for device decoding: generator(b) -> a DecodeBatch (datasets/ilsvrc12_dataset.py).  `next_decode()`
+    stages its arrays in rotating pinned buffers; the learner decodes the device images with pf_jpeg_decode one
+    batch ahead, then runs pf_preprocess_images."""
+
+    FIELDS = ('crops', 'desc', 'labels', 'jdesc', 'scans')
+
+    def next_packed(self):
+        raise TypeError('a decode iterator yields undecoded JPEG scans: use next_decode()')
+
+    def next_decode(self):
+        """({field: (pinned uint8 buffer, nbytes)} for FIELDS, the DecodeBatch)."""
+        batch = self.generator(self.batch_size)
+        i = self.last_slot = self.cursor % POOL_SIZE
+        self.cursor += 1
+        self._wait_slot_free(i)
+        slot = self.slots[i] = self.slots[i] or {}
+        staged = {}
+        for key in self.FIELDS:
+            flat = np.ascontiguousarray(getattr(batch, key)).reshape(-1).view(np.uint8)
+            buf = slot.get(key)
+            if buf is None or buf.numel() < flat.size:
+                buf = slot[key] = torch.empty(int(flat.size * 1.25) + 4096, dtype=torch.uint8, pin_memory=self.pin)
+            buf[:flat.size].copy_(torch.from_numpy(flat))
+            staged[key] = (buf, int(flat.size))
+        return staged, batch
+
+
 class AbstractDataset(ABC):
     def __init__(self, is_train):
         self.is_train = is_train
@@ -155,7 +183,9 @@ class AbstractDataset(ABC):
     def build(self, enbl_trn_val_split=False):
         gens = self._file_generators(enbl_trn_val_split) if FLAGS.data_dir_local else None
         if gens is not None:
-            its = [PackedBatchIterator(self.batch_size, self.image_shape, self.nb_classes, g_)
+            its = [DecodeBatchIterator(self.batch_size, self.image_shape, self.nb_classes, g_)
+                   if getattr(g_, 'device_decode', False) else
+                   PackedBatchIterator(self.batch_size, self.image_shape, self.nb_classes, g_)
                    if getattr(g_, 'packed', False) else
                    BatchIterator(self.batch_size, self.image_shape, self.nb_classes, g_, stream=True) for g_ in gens]
             return tuple(its) if len(its) > 1 else its[0]

@@ -34,6 +34,7 @@ import numpy as np
 from ..flags import FLAGS, DEFINE_integer, DEFINE_boolean
 from ..utils.multi_gpu_wrapper import MultiGpuWrapper as mgw
 from ..utils.tf_record import parse_example, read_records
+from . import jpeg
 from .abstract_dataset import AbstractDataset
 
 DEFINE_integer('nb_classes', 1001, '# of classes')
@@ -44,6 +45,8 @@ DEFINE_integer('batch_size', 64, 'batch size per GPU for training')
 DEFINE_integer('batch_size_eval', 100, 'batch size for evaluation')
 DEFINE_boolean('enbl_device_preprocess', False, 'ILSVRC-12: decode + crop on the host, resize / flip / mean on the GPU '
                '(pf_preprocess_images; not validated on a GPU yet)')
+DEFINE_boolean('enbl_device_decode', False, 'ILSVRC-12: decode baseline JPEGs on the GPU too (pf_jpeg_decode, bit for bit '
+               'with the host decoder; other files are decoded on the host); implies --enbl_device_preprocess')
 
 IMAGE_HEI, IMAGE_WID, IMAGE_CHN = 224, 224, 3
 CHANNEL_MEANS = np.array([123.68, 116.78, 103.94], np.float32)       # imagenet_preprocessing.py:40-43
@@ -200,18 +203,29 @@ def crop_and_descriptor(image_buffer, bbox, is_training, rng=None):
     that pf_preprocess_images — or `preprocess_from_descriptor`, its numpy statement — yields exactly
     `preprocess_image(...)`.  Training: the distorted-bounding-box crop, flip flag drawn here, resized straight to
     224x224.  Evaluation: the whole image, resized to a 256 short side, central 224x224 window."""
+    if is_training:
+        window, d = crop_window(*jpeg_shape(image_buffer), bbox, True, rng)
+        crop = decode_jpeg(image_buffer, window)
+    else:
+        crop = decode_jpeg(image_buffer)
+        window, d = crop_window(crop.shape[0], crop.shape[1], bbox, False)
+    return np.ascontiguousarray(crop), d
+
+
+def crop_window(height, width, bbox, is_training, rng=None):
+    """The crop (y, x, h, w) of an image of this size and its IMG_DESC record (offset 0), with the same random draws
+    as crop_and_descriptor: the distorted bounding box, then the flip (training); the whole image (evaluation)."""
     d = np.zeros((), IMG_DESC)
     if is_training:
-        h, w = jpeg_shape(image_buffer)
-        crop = decode_jpeg(image_buffer, sample_distorted_bounding_box(h, w, bbox, rng))
+        window = sample_distorted_bounding_box(height, width, bbox, rng)
         d['flip'] = int(rng.random() < 0.5)
         d['rh'], d['rw'] = IMAGE_HEI, IMAGE_WID
     else:
-        crop = decode_jpeg(image_buffer)
-        d['rh'], d['rw'] = smallest_size_at_least(crop.shape[0], crop.shape[1])
+        window = (0, 0, height, width)
+        d['rh'], d['rw'] = smallest_size_at_least(height, width)
         d['top'], d['left'] = (int(d['rh']) - IMAGE_HEI) // 2, (int(d['rw']) - IMAGE_WID) // 2
-    d['h'], d['w'] = crop.shape[:2]
-    return np.ascontiguousarray(crop), d
+    d['h'], d['w'] = window[2], window[3]
+    return window, d
 
 
 def preprocess_from_descriptor(crop, d, out_h=IMAGE_HEI, out_w=IMAGE_WID):
@@ -258,12 +272,54 @@ def parse_packed_fn(example_serialized, is_train, nb_classes, rng=None):
     return crop, desc, onehot
 
 
+def parse_decode_fn(example_serialized, is_train, nb_classes, rng=None):
+    """The host half of device decoding: the header is parsed and the crop drawn from its size.  Baseline files give
+    (None, IMG_DESC, one-hot label, (JPEG bytes, crop window, pf_jpeg_desc record, scan bytes)) for pf_jpeg_decode;
+    every other file is decoded here, as parse_packed_fn does: (uint8 crop, IMG_DESC, one-hot label, None)."""
+    encoded, onehot, bbox = parse_example_proto(example_serialized, nb_classes)
+    h = jpeg.parse_header(encoded)
+    if not h.device:
+        crop, desc = crop_and_descriptor(encoded, bbox, is_train, rng)
+        return crop, desc, onehot, None
+    window, desc = crop_window(h.height, h.width, bbox, is_train, rng)
+    return None, desc, onehot, (encoded, window, jpeg.descriptor(h, window), jpeg.scan(h, encoded))
+
+
+class DecodeBatch(object):
+    """One mini-batch for device decoding.  crops: the host-decoded crops back to back (they come first in the crop
+    buffer); desc: IMG_DESC [b] with every crop's offset; labels [b, k]; jdesc: pf_jpeg_desc [m] of the m device
+    images, whose crops follow the host ones; scans: their entropy-coded segments back to back; ws: workspace int16
+    elements; nbytes: the whole crop buffer; fallback: [(JPEG bytes, crop window, crop offset)] of the m device images,
+    for the host to decode the ones whose data the kernel flags."""
+
+    def __init__(self, out):
+        b = len(out)
+        self.desc = np.stack([o[1] for o in out])
+        self.labels = np.stack([o[2] for o in out])
+        host = [i for i in range(b) if out[i][3] is None]
+        dev = [i for i in range(b) if out[i][3] is not None]
+        sizes = np.array([out[i][0].size if out[i][3] is None else int(out[i][1]['h']) * int(out[i][1]['w']) * 3
+                          for i in host + dev], np.int64)
+        offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        self.desc['offset'][host + dev] = offsets[:-1]
+        self.nbytes = int(offsets[-1])
+        self.crops = (np.concatenate([out[i][0].reshape(-1) for i in host]) if host else np.zeros(0, np.uint8))
+        self.fallback = []
+        for i in dev:
+            encoded, window, d, _ = out[i][3]
+            d['crop_offset'] = self.desc['offset'][i]
+            self.fallback.append((encoded, window, int(d['crop_offset'])))
+        self.jdesc, self.scans, self.ws = jpeg.pack([out[i][3][2] for i in dev], [out[i][3][3] for i in dev])
+
+
 class ExampleStream(object):
     """generator(b) for BatchIterator(stream=True): endless, shuffled, decoded in a thread pool, prepared ahead."""
 
-    def __init__(self, files, nb_classes, is_train, seed, skip=0, take=None, augment=None, packed=False):
+    def __init__(self, files, nb_classes, is_train, seed, skip=0, take=None, augment=None, packed=False,
+                 device_decode=False):
         self.files, self.k, self.is_train = list(files), nb_classes, is_train
-        self.packed = packed                                  # True: yield (crops, descriptors, labels), see PackedBatchIterator
+        self.packed = packed or device_decode                 # True: yield (crops, descriptors, labels), see PackedBatchIterator
+        self.device_decode = device_decode                    # True: yield DecodeBatch, see DecodeBatchIterator
         self.augment = is_train if augment is None else augment
         self.skip, self.take = skip, take
         self.rng = np.random.default_rng(seed)
@@ -324,10 +380,12 @@ class ExampleStream(object):
             while True:
                 raw = [next(records) for _ in range(b)]
                 seeds = self.rng.integers(0, 2 ** 62, size=b)
-                fn = parse_packed_fn if self.packed else parse_fn
+                fn = parse_decode_fn if self.device_decode else (parse_packed_fn if self.packed else parse_fn)
                 out = list(self.pool.map(
                     lambda a: fn(a[0], self.augment, self.k, np.random.default_rng(int(a[1]))), zip(raw, seeds)))
-                if self.packed:
+                if self.device_decode:
+                    self.ready.put(DecodeBatch(out))
+                elif self.packed:
                     desc = np.stack([o[1] for o in out])
                     sizes = np.array([o[0].size for o in out], np.int64)
                     desc['offset'] = np.concatenate([[0], np.cumsum(sizes)[:-1]])
@@ -370,6 +428,9 @@ class Ilsvrc12Dataset(AbstractDataset):
         seed = 8765 + 7919 * rank + (0 if self.is_train else 1)
         if self.is_train and enbl_trn_val_split:
             nv = FLAGS.nb_smpls_val
-            return [ExampleStream(files, self.nb_classes, True, seed, skip=nv, packed=FLAGS.enbl_device_preprocess),
-                    ExampleStream(files, self.nb_classes, True, seed, take=nv, packed=FLAGS.enbl_device_preprocess)]
-        return [ExampleStream(files, self.nb_classes, self.is_train, seed, packed=FLAGS.enbl_device_preprocess)]
+            return [ExampleStream(files, self.nb_classes, True, seed, skip=nv, packed=FLAGS.enbl_device_preprocess,
+                                  device_decode=FLAGS.enbl_device_decode),
+                    ExampleStream(files, self.nb_classes, True, seed, take=nv, packed=FLAGS.enbl_device_preprocess,
+                                  device_decode=FLAGS.enbl_device_decode)]
+        return [ExampleStream(files, self.nb_classes, self.is_train, seed, packed=FLAGS.enbl_device_preprocess,
+                              device_decode=FLAGS.enbl_device_decode)]

@@ -2,6 +2,7 @@
 (/root/reference/learners/abstract_learner.py:32-158), without TensorFlow."""
 from abc import ABC
 from abc import abstractmethod
+import contextlib
 import glob
 import os
 import shutil
@@ -253,6 +254,8 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         """Device-side input preprocessing (--enbl_device_preprocess): the host decodes and crops, the uint8 crops
         (about a third of the fp32 batch's bytes), their descriptor table and the labels are copied, and ONE kernel
         (pf_preprocess_images) resizes / flips / centres them straight into the step's image placeholder."""
+        if hasattr(iterator, 'next_decode'):
+            return AbstractLearner._feed_decoded(iterator, dev_images, dev_labels)
         crops, nbytes, desc, labels = iterator.next_packed()
         dev = getattr(iterator, '_packed_dev', None)
         if dev is None or dev[0].numel() < nbytes:
@@ -264,6 +267,85 @@ class AbstractLearner(ABC):  # pylint: disable=too-many-instance-attributes
         iterator.copy_enqueued()
         ops.preprocess_images(dev[0], dev[1], dev_images)
         return nbytes + desc.numel() + labels.numel() * 4
+
+    @staticmethod
+    def _feed_decoded(iterator, dev_images, dev_labels):
+        """Device-side JPEG decoding (--enbl_device_decode).  Batch i+1's scans are copied and decoded by
+        pf_jpeg_decode on a side stream while step i runs, into one of two device slots (so a decode never overwrites
+        crops that pf_preprocess_images still reads); its per-image status comes back to pinned memory.  When batch
+        i+1 is fed, the host decodes the images the kernel flagged and copies their crops into place, then
+        pf_preprocess_images runs on the main stream.  Returns the bytes copied host -> device for the staged batch."""
+        cuda = dev_images.device.type == 'cuda'
+        st = getattr(iterator, '_decode_state', None)
+        if st is None:
+            st = iterator._decode_state = dict(slots=[{}, {}], next=0, primed=False,
+                                               stream=torch.cuda.Stream() if cuda else None)
+            if cuda:
+                for s in st['slots']:
+                    s['ready'], s['free'] = torch.cuda.Event(), torch.cuda.Event()
+                    s['free'].record(torch.cuda.current_stream())
+
+        def grown(s, key, n, dtype, pin=False):
+            t = s.get(key)
+            if t is None or t.numel() < n:
+                cap = max(int(n * 1.25) + 64, 64)
+                t = s[key] = (torch.empty(cap, dtype=dtype, pin_memory=True) if pin else
+                              torch.empty(cap, dtype=dtype, device=dev_images.device))
+            return t
+
+        def stage(s):
+            staged, batch = iterator.next_decode()
+            if cuda:
+                st['stream'].wait_event(s['free'])                     # preprocessing of the slot's last batch is done
+            with torch.cuda.stream(st['stream']) if cuda else contextlib.nullcontext():
+                crops = grown(s, 'crops', max(batch.nbytes, 1), torch.uint8)
+                desc = grown(s, 'desc', staged['desc'][1], torch.uint8)
+                labels = grown(s, 'labels', staged['labels'][1], torch.uint8)
+                m = len(batch.jdesc)
+                for key, dst in (('crops', crops), ('desc', desc), ('labels', labels)):
+                    buf, n = staged[key]
+                    dst[:n].copy_(buf[:n], non_blocking=True)
+                status = grown(s, 'status', max(m, 1), torch.int32)
+                status_host = grown(s, 'status_host', max(m, 1), torch.int32, pin=cuda)
+                if m:
+                    jdesc = grown(s, 'jdesc', staged['jdesc'][1], torch.uint8)
+                    scans = grown(s, 'scans', max(staged['scans'][1], 1), torch.uint8)
+                    ws = grown(s, 'ws', max(batch.ws, 64), torch.int16)
+                    for key, dst in (('jdesc', jdesc), ('scans', scans)):
+                        buf, n = staged[key]
+                        dst[:n].copy_(buf[:n], non_blocking=True)
+                    ops.jpeg_decode(scans, jdesc, m, ws, crops, status)
+                    status_host[:m].copy_(status[:m], non_blocking=True)
+                iterator.copy_enqueued()
+                if cuda:
+                    s['ready'].record()
+            s['batch'] = batch
+            return sum(n for _, n in staged.values())
+
+        if not st['primed']:
+            stage(st['slots'][st['next']])
+            st['primed'] = True
+        cur = st['slots'][st['next']]
+        batch = cur['batch']
+        if cuda:
+            cur['ready'].synchronize()
+        flagged = np.flatnonzero(cur['status_host'][:len(batch.jdesc)].numpy()) if len(batch.jdesc) else []
+        if len(flagged):
+            from ..datasets.ilsvrc12_dataset import decode_jpeg
+        for j in flagged:                                  # data the kernel does not vouch for: the host decoder's result
+            encoded, window, offset = batch.fallback[j]
+            crop = decode_jpeg(encoded, window).reshape(-1).copy()
+            cur['crops'][offset:offset + crop.size].copy_(torch.from_numpy(crop))
+        main = torch.cuda.current_stream() if cuda else None
+        if cuda:
+            main.wait_event(cur['ready'])
+        n, k = dev_labels.shape
+        dev_labels.copy_(cur['labels'][:n * k * 4].view(torch.float32).view(n, k), non_blocking=True)
+        ops.preprocess_images(cur['crops'], cur['desc'][:n * 40], dev_images)
+        if cuda:
+            cur['free'].record(main)
+        st['next'] ^= 1
+        return stage(st['slots'][st['next']])             # decodes under the step that is about to run
 
     def grad_allreduce(self):
         """The one collective of the data-parallel step (replaces DistributedOptimizer,

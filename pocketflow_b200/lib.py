@@ -44,6 +44,7 @@ SIGNATURES = {
     'pf_im2col': (c_i32, [c_vp, c_vp, c_i32, c_vp, c_vp]),
     'pf_s2d_planes': (c_i32, [c_vp] + [c_i32] * 9 + [c_vp, c_vp, c_vp]),
     'pf_preprocess_images': (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_f32, c_f32, c_f32, c_vp, c_vp]),
+    'pf_jpeg_decode': (c_i32, [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'pf_gather_rows': (c_i32, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
     'pf_im2col_planes': (c_i32, [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),
     'pf_conv2d_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp]),

@@ -1324,6 +1324,24 @@ def preprocess_images(crops_u8, desc, out, mean=(123.68, 116.78, 103.94)):
     return out
 
 
+def jpeg_decode(data_u8, desc, n, coef_ws, crops_u8, status):
+    """Baseline JPEG decoding on the device (pf_jpeg_decode): data_u8 = uint8 CUDA buffer of the images' entropy-coded
+    segments, desc = uint8 CUDA view of n pf_jpeg_desc records (datasets/jpeg.py:JPEG_DESC), coef_ws = int16 CUDA
+    workspace of at least sum(jpeg.workspace_elems(d)) elements, crops_u8 = uint8 CUDA buffer the RGB crops are written
+    into, status = int32 CUDA [n] (0: decoded; otherwise the host has to decode that image, datasets/jpeg.py:STATUS)."""
+    L = _lib.load()
+    for t, dt in ((data_u8, torch.uint8), (desc, torch.uint8), (coef_ws, torch.int16), (crops_u8, torch.uint8),
+                  (status, torch.int32)):
+        if t.dtype != dt or not t.is_cuda or not t.is_contiguous():
+            raise ValueError('jpeg_decode: expected contiguous CUDA buffers (uint8 data / desc / crops, int16 workspace, '
+                             'int32 status)')
+    if desc.numel() < n * 4144 or status.numel() < n:
+        raise ValueError('jpeg_decode: %d images need %d descriptor bytes and %d status words' % (n, n * 4144, n))
+    _lib.check(L.pf_jpeg_decode(_p(data_u8), _p(desc), int(n), _p(coef_ws), _p(crops_u8), _p(status), _stream()),
+               'pf_jpeg_decode')
+    return status
+
+
 
 # ----------------------------------------------------------------------------- f4 channel selection (pf_cpg.cu)
 def cpg_diff_l2(a, b, diff, loss, partial_ws):
